@@ -17,6 +17,9 @@ mode is not selected is also timed and reported under `other_scaling_mode`.
 `cpu_baseline` / --impl reference: the UNMODIFIED reference (oracle/_ref, copied from /root/reference by oracle/build_ref.py) timed on this
             host's cores; falls back to the oracle port when oracle/_ref is absent.  Only these legs touch oracle/ ; the GPU path never does.
 `secondary`: configs[2] (64->512, batch 4) and configs[4] (unconditional 128x128, batch 32) on one GPU: ms/step and fraction of bound.
+--dump-outputs DIR: after the timed steps, rank 0 writes what they computed -- the sampler state x_{t-1} after the last timed step, the
+            array GaussianDiffusion's sampler hands back -- as DIR/x_state.npy (float32, [16, 3, 128, 128]).  Inputs, weights and noise are
+            seeded, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -34,12 +37,12 @@ UNET = dict(in_channel=6, out_channel=3, inner_channel=64, channel_multiplier=[1
 GLOBAL_BATCH = 16
 IMAGE = 128
 METRIC = "diffusion steps/sec (batch16, 16->128 SR3)"
-# name -> (unet options, image size, conditional, batch, bf16 roofline bound in ms per step on ONE GPU (BASELINE.md section 3), config file)
+# name -> (unet options, image size, conditional, batch, config file)
 WORKLOADS = {
-    "sr_16_128_b16": (UNET, 128, True, 16, 0.732, "sr_sr3_16_128.json"),
+    "sr_16_128_b16": (UNET, 128, True, 16, "sr_sr3_16_128.json"),
     "sr_64_512_b4": (dict(in_channel=6, out_channel=3, inner_channel=64, norm_groups=16, channel_multiplier=[1, 2, 4, 8, 16], attn_res=[], res_blocks=1, dropout=0),
-                     512, True, 4, 2.423, "sr_sr3_64_512.json"),
-    "uncond_128_b32": (dict(UNET, in_channel=3), 128, False, 32, 1.463, "sample_sr3_128.json"),
+                     512, True, 4, "sr_sr3_64_512.json"),
+    "uncond_128_b32": (dict(UNET, in_channel=3), 128, False, 32, "sample_sr3_128.json"),
 }
 
 
@@ -79,7 +82,15 @@ def measured_peaks():
         d = json.load(open(p))
         return {"burst": d.get("bf16_tflops"), "sustained": d.get("bf16_tflops_sustained", d.get("bf16_tflops")), "hbm_gbs": d.get("hbm_gbs"),
                 "src": "measured (MEASURED_PEAKS.json)"}
-    return {"burst": 1590.0, "sustained": 1400.0, "hbm_gbs": 6650.0, "src": "fallback (B200_PROFILING.md)"}
+    return {"burst": 989.0, "sustained": 989.0, "hbm_gbs": 3350.0, "src": "NVIDIA H100 SXM data sheet (dense bf16, 700 W card; not reached)"}
+
+
+def dump_outputs(out_dir, arrays):
+    """Writes every tensor of `arrays` as out_dir/<name>.npy in float32."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), t.detach().float().cpu().numpy())
 
 
 class ClockSampler:
@@ -259,7 +270,7 @@ def secondary_workloads(dev, peaks, steps=10):
     import sr3_b200
     out = {}
     for name in ("sr_64_512_b4", "uncond_128_b32"):
-        unet, size, cond, B, bound_ms, cfgfile = WORKLOADS[name]
+        unet, size, cond, B, cfgfile = WORKLOADS[name]
         try:
             torch.manual_seed(0)
             net = sr3_b200.define_G(make_opt(SCHED, unet, size, cond)).to(dev)
@@ -270,6 +281,7 @@ def secondary_workloads(dev, peaks, steps=10):
             x = torch.randn(B, 3, size, size, generator=g).to(dev)
             ms = time_resident(eng, c, x, 0, steps, 3, SCHED["n_timestep"], torch.cuda.synchronize, None, dev) / steps
             fl = algorithmic_flops_per_image(unet, size) * B
+            bound_ms = fl / (peaks["burst"] * 1e12) * 1e3          # bf16 tensor bound of the algorithmic FLOPs
             out[name] = {"config": cfgfile, "batch": B, "ms_per_step": ms, "steps_per_s": 1e3 / ms, "launches_per_step": eng.launches_per_step(),
                          "algorithmic_tflop_per_step": fl / 1e12, "achieved_tflops": fl / (ms * 1e-3) / 1e12,
                          "frac_of_measured_burst_bf16": fl / (ms * 1e-3) / 1e12 / peaks["burst"], "roofline_bound_ms_nominal": bound_ms,
@@ -446,7 +458,7 @@ def run_train(args, rank, local, world):
         os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
     import torch
     import torch.distributed as dist
-    assert torch.cuda.is_available(), "bench.py (our arm) needs a B200; there is no CPU fallback"
+    assert torch.cuda.is_available(), "bench.py (our arm) needs an H100; there is no CPU fallback"
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
     if world > 1:
@@ -481,7 +493,7 @@ def run_train(args, rank, local, world):
                 "config": {"workload": "sr_sr3_16_128.json training step (configs[3]): p_losses in train() mode (Dropout 0.2) + backward + Adam, random-init "
                                        "(orthogonal) weights, synthetic HR/SR in [-1,1]", "global_batch": GB, "per_gpu_batch": per,
                            "parallelism": f"data parallel x{world}: %d gradient buckets all-reduced (NCCL sum) while the backward of the earlier layers runs; Adam on every rank" % n_buckets,
-                           "l2": "per-step working set (activations kept for the backward, several GB) exceeds the 126 MB L2; no explicit flush",
+                           "l2": "per-step working set (activations kept for the backward, several GB) exceeds the 50 MB L2; no explicit flush",
                            "images_per_s": GB * 1e3 / ms},
                 "e2e": {"value": 1e3 / e2e_ms, "unit": "steps/s", "h2d_bytes_per_step": 2 * img_bytes, "d2h_bytes_per_step": 8,
                         "api": "sr3_b200.parallel.DataParallelTrainer.step on pinned host HR / SR tensors, loss value read back every step"},
@@ -511,6 +523,7 @@ def main():
     ap.add_argument("--workload", default="sample", choices=["sample", "train"],
                     help="sample (default): the BASELINE metric; train: configs[3], the training step (fwd + bwd + Adam) at global batch --train-batch")
     ap.add_argument("--train-batch", type=int, default=64)
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write the sampler state after the last timed step to DIR/x_state.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
@@ -530,7 +543,7 @@ def main():
     import torch.distributed as dist
     import sr3_b200
     from sr3_b200 import parallel
-    assert torch.cuda.is_available(), "bench.py (our arm) needs a B200; there is no CPU fallback"
+    assert torch.cuda.is_available(), "bench.py (our arm) needs an H100; there is no CPU fallback"
     assert world == args.gpus or world == 1, f"WORLD_SIZE={world} but --gpus {args.gpus}"
     W = max(args.warmup, 3)
     K = args.steps
@@ -572,6 +585,8 @@ def main():
     with ClockSampler(local) as clk:
         ms = time_resident(eng, cond_h.to(dev), xT_h.to(dev), lo, K, W, T, barrier, dd, dev)
     value = units * K / (ms * 1e-3)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"x_state": eng.read_state()})
     step_prof = eng.step_kernel_profile() if eng.uses_step_kernel() else None      # per-op device times of the last timed launch
 
     # the other scaling mode at N > 1, as a supplementary number (same timing rules)
@@ -642,22 +657,13 @@ def main():
         for d in by_op.values():
             d["GB_per_s"] = round(d.pop("bytes") / (d["us"] * 1e-6) / 1e9, 1) if d["us"] > 0 else None
     achieved = alg_flops_step / (kernel_ms * 1e-3) / 1e12
-    traffic, traffic_src, whole_step_traffic = None, None, None
-    for cand in ("r02_traffic.json", "r01_traffic.json"):
-        tpath = os.path.join(ROOT, "profiles", cand)
-        if os.path.exists(tpath):
-            tj = json.load(open(tpath))
-            key = "step_kernel_dram_bytes_per_launch" if step_prof is not None else "gemm_tile_kernel_dram_bytes_per_step"
-            if key in tj:
-                traffic, traffic_src = tj[key], "profiles/" + cand + " (ncu per-launch dram__bytes_read.sum + dram__bytes_write.sum of one step of this build)"
-                whole_step_traffic = tj.get("whole_step_dram_bytes")
-                break
+    traffic, traffic_src, whole_step_traffic = None, "not measured", None
     roof = {"bound": "tensor", "kernel": kernel_name, "achieved": achieved, "peak": peaks["burst"], "unit": "TFLOP/s",
             "frac": achieved / peaks["burst"], "frac_of_sustained_peak": achieved / peaks["sustained"], "peak_sustained": peaks["sustained"],
             "peak_source": peaks["src"] + ": frac is against the BURST bf16 figure", "traffic": traffic, "traffic_source": traffic_src,
             "traffic_whole_step_incl_groupnorm_apply": whole_step_traffic, "algorithmic_flops_per_launch": alg_flops_step, "algorithmic_bytes_per_launch": 2.98e9 * per / 16.0,
             "kernel_ms_per_launch": kernel_ms, "launches_per_step": eng.launches_per_step(), "ops_per_step": eng.ops_per_step(),
-            "frac_of_nominal_bound": (0.732 * per / 16.0) / (ms / K) if per == 16 else None,
+            "frac_of_nominal_bound": (alg_flops_step / (peaks["burst"] * 1e12) * 1e3) / (ms / K),
             "step_frac_of_burst_peak": (alg_flops_step / (ms / K * 1e-3) / 1e12) / peaks["burst"], "by_op": by_op}
     if args.profile_out:
         os.makedirs(os.path.dirname(os.path.abspath(args.profile_out)), exist_ok=True)
@@ -682,7 +688,7 @@ def main():
                                    "sr_sr3_16_128.json sampling (configs[1]): batch 16 per GPU, T=2000 linear schedule, random-init weights",
                        "global_batch": global_batch, "per_gpu_batch": per, "parallelism": f"batch-sharded x{world}, no per-step collective, one all-gather of the finished images",
                        "value_unit_note": "steps/s of batch-16 work: (images x reverse steps per second) / 16, summed over all ranks",
-                       "l2": "per-step working set (~1.5 GB of activations + weights at batch 16) exceeds the 126 MB L2; no explicit flush",
+                       "l2": "per-step working set (~1.5 GB of activations + weights at batch 16) exceeds the 50 MB L2; no explicit flush",
                        "image_steps_per_s": value * GLOBAL_BATCH},
             "e2e": {"value": e2e_val, "unit": "steps/s", "h2d_bytes_per_step": 2 * img_bytes / K, "d2h_bytes_per_step": (img_bytes if world == 1 else img_bytes * world) / K,
                     "api": ("GaussianDiffusion.super_resolution on host tensors (sr3_super_resolution_host)" if world == 1 else

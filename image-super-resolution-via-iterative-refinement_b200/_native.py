@@ -90,7 +90,7 @@ def lib():
         return _lib
     if not os.path.exists(LIB_PATH):
         raise NativeLibraryError(
-            f"{LIB_PATH} is missing: run `python -c 'import __graft_entry__ as g; g.build()'` (nvcc, sm_100a). "
+            f"{LIB_PATH} is missing: run `python -c 'import __graft_entry__ as g; g.build()'` (nvcc, sm_90a). "
             "sr3_b200 has no CPU or eager-PyTorch fallback.")
     try:
         l = ctypes.CDLL(LIB_PATH)
@@ -131,7 +131,7 @@ class Engine:
         """train_dropout: None = inference plan; a float = TRAINING plan (forward keeps every intermediate, backward recorded) with that
         Dropout probability (sr3_engine_create_train)."""
         if device.type != "cuda":
-            raise NativeLibraryError("sr3_b200 runs on a CUDA (sm_100a) device only; got device=%s" % device)
+            raise NativeLibraryError("sr3_b200 runs on a CUDA (sm_90a) device only; got device=%s" % device)
         self.device = device
         self.batch = batch
         self.channels = cfg["channels"]

@@ -1,4 +1,4 @@
-"""Builds libsr3_b200.so (sm_100a only) in-tree with nvcc.  No torch involved: the library is a plain C-ABI .so."""
+"""Builds libsr3_b200.so (sm_90a only) in-tree with nvcc.  No torch involved: the library is a plain C-ABI .so."""
 import hashlib
 import os
 import subprocess
@@ -8,7 +8,7 @@ PKG = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(PKG, "csrc")
 LIB = os.path.join(PKG, "lib", "libsr3_b200.so")
 SOURCES = ["engine.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
               "--expt-relaxed-constexpr", "-Xptxas", "-v", "-shared", "-cudart", "static"]
 
 

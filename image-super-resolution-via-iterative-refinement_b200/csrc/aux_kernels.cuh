@@ -2,7 +2,7 @@
 // GroupNorm apply (+SiLU) with channel concat, fp32->bf16 cast / nearest 2x upsample, row softmax,
 // noise-level embedding MLP + FiLM projections, weight packing, layout conversion at the API boundary.
 #pragma once
-#include "gemm_tcgen05.cuh"
+#include "gemm_wgmma.cuh"
 
 namespace sr3 {
 

@@ -18,7 +18,7 @@
 
 #include "../../include/sr3_b200.h"
 #include "aux_kernels.cuh"
-#include "attn_tcgen05.cuh"
+#include "attn_wgmma.cuh"
 #include "step_megakernel.cuh"
 #include "train_kernels.cuh"
 
@@ -123,8 +123,8 @@ struct GemmDesc {
     int ksplit_max = 1;                           // split-K allowed up to this factor (image convs with few output tiles)
     int tiles_w = 1, tiles_h = 1, tiles_b = 1, n_tiles = 1, nz = 1;
     int a_zstep = 0, b_zrows = 0;
-    int z_phase = 0; long long z_off_hi = 0, z_off_lo = 0;   // nz = 4 output phases of a folded upsample conv (gemm_tcgen05.cuh)
-    int passes = 1, lo_b_col = 0, lo_a_chan[2] = {0, 0};      // precise mode: three passes over the stage table (gemm_tcgen05.cuh)
+    int z_phase = 0; long long z_off_hi = 0, z_off_lo = 0;   // nz = 4 output phases of a folded upsample conv (gemm_wgmma.cuh)
+    int passes = 1, lo_b_col = 0, lo_a_chan[2] = {0, 0};      // precise mode: three passes over the stage table (gemm_wgmma.cuh)
     long long lo_out_off = 0, lo_t_off = 0;
     // epilogue
     int mode = 0, OW = 0, OH = 1, OB = 1, n_valid = 0;
@@ -142,7 +142,7 @@ OutSpec nhwc_out(int H, int W, int C, long long off = 0) {
     OutSpec s; s.sZ = 0; s.sB = 1LL * H * W * C; s.sH = 1LL * W * C; s.sW = C; s.off = off; return s;
 }
 
-constexpr int SMEM_LIMIT = 232448;   // 227 KB opt-in maximum per CTA on sm_100
+constexpr int SMEM_LIMIT = 232448;   // 227 KB opt-in maximum per CTA on sm_90
 int pick_stages(int block_n, int a_stage_bytes, int b_taps, bool resid, int num_k) {
     int s = GEMM_MAX_STAGES;
     if (const char* e = getenv("SR3_STAGES")) s = atoi(e);
@@ -432,7 +432,7 @@ Op make_gemm_op(const GemmDesc& d, DevAllocs& mem) {
         p.out_map = p.b_map; p.res_map = p.b_map;
     }
     // split-K: when the output has too few tiles to occupy the SMs, `ksplit` CTAs share a tile, each streams a slice of K and parks its
-    // partial tile in `ws`; every one of them then finalises a 1/ksplit share of the tile (gemm_tcgen05.cuh, epilogue pass 1).
+    // partial tile in `ws`; every one of them then finalises a 1/ksplit share of the tile (gemm_wgmma.cuh, epilogue pass 1).
     // One (tile, split) pair per SM at most: all CTAs are co-resident, which the in-kernel wait relies on.
     p.ksplit = 1;
     {
@@ -485,7 +485,7 @@ Op make_gemm_op(const GemmDesc& d, DevAllocs& mem) {
     };
 }
 
-// Fused attention core (attn_tcgen05.cuh): S = q k^T / sqrt(C), softmax, O = P v in one launch.  qk [nz*Lt][2C], vT [nz*C][Lt], out [nz*Lt][C].
+// Fused attention core (attn_wgmma.cuh): S = q k^T / sqrt(C), softmax, O = P v in one launch.  qk [nz*Lt][2C], vT [nz*C][Lt], out [nz*Lt][C].
 bool attn_fusable(int Lt, int C) { return getenv("SR3_NO_FUSED_ATTN") == nullptr && (Lt == 128 || Lt == 256) && C % 128 == 0 && C >= 128; }
 
 Op make_attn_op(const bf16* qk, const bf16* vT, bf16* out, int nz, int Lt, int HW, int C) {
@@ -519,8 +519,8 @@ int pick_block_n(int cout);
 
 // Geometry of an image conv: the "tall halo" form for 3x3 stride-1 convs at >= 16x16, else a plain 128-pixel patch per tap.
 // The tile shape (rows x BLOCK_N) and the split-K factor are chosen by a byte model of the per-CTA critical path: a CTA ingests
-// stages x (A box + B boxes) through TMA at a fixed ~47 B/clk, runs ceil(tiles * split / SMs) waves, and a split tile costs an extra
-// partial-tile store + reload + a grid-level handshake.  (Measured on B200: tools/gpu_splitk_sweep.py, DESIGN.md section 8.)
+// stages x (A box + B boxes) through TMA at a fixed rate, runs ceil(tiles * split / SMs) waves, and a split tile costs an extra
+// partial-tile store + reload + a grid-level handshake (tools/gpu_splitk_sweep.py sweeps the choices on a device).
 void conv_geometry(GemmDesc& d, int OW, int OH, int Bp, int cout, bool has_resid = false, int nz = 1) {
     const int npass = d.passes > 1 ? d.passes : 1;
     bool tall_ok = getenv("SR3_NO_TALL") == nullptr && OW >= 8 && OH >= 16, has3 = false;
@@ -543,7 +543,7 @@ void conv_geometry(GemmDesc& d, int OW, int OH, int Bp, int cout, bool has_resid
         split = smax;
         const long long waves = (tiles * smax + sms - 1) / sms;
         double c = (double)waves * ((nstage + smax - 1) / smax) * (double)stage_bytes;
-        // a split tile: partial tile out (TMEM -> registers -> L2) and back, weighted 2x against streamed TMA bytes, plus ~1.4 us of
+        // a split tile: partial tile out (registers -> L2) and back, weighted 2x against streamed TMA bytes, plus ~1.4 us of
         // grid-level handshake; a residual is then read with plain loads instead of TMA
         if (smax > 1) c += 4.0 * rows * bn * 4 + 131072.0 + (has_resid ? 2.0 * rows * bn * 4 : 0.0);
         return c;
@@ -908,7 +908,7 @@ struct sr3_engine {
     void add_cast(const Act& s, bf16* dst, int up) {
         if (dry) return;
         const long long total = 1LL * B * s.H * up * s.W * up * (s.C / 4);
-        const int blocks = (int)std::min<long long>((total + 255) / 256, 148 * 16);
+        const int blocks = (int)std::min<long long>((total + 255) / 256, num_sms() * 16LL);
         const float* src = s.p; const int Bn = B, Hh = s.H, Ww = s.W, C = s.C;
         push([=](cudaStream_t st) { launch_k(cast_kernel, dim3(blocks), dim3(256), 0, st, src, dst, Bn, Hh, Ww, C, up); }, 2, 0, (double)Bn * Hh * Ww * C * (4.0 + 2.0 * up * up));
     }
@@ -1082,7 +1082,7 @@ struct sr3_engine {
             push_gemm(d);
         }
         if (attn_fusable(Lt, C) && !precise && !train) {
-            // S = q k^T / sqrt(C), softmax over the keys of the same image, O = P v: one launch (attn_tcgen05.cuh)
+            // S = q k^T / sqrt(C), softmax over the keys of the same image, O = P v: one launch (attn_wgmma.cuh)
             const double fl = 4.0 * nz * (double)Lt * Lt * C;
             push(make_attn_op(qk, vT, O, nz, Lt, HW, C), 5, fl, (double)nz * Lt * C * 2 * 4);
         } else {
@@ -1356,7 +1356,7 @@ struct sr3_engine {
         CK(cudaSetDevice(dev));
         cudaDeviceProp prop;
         CK(cudaGetDeviceProperties(&prop, dev));
-        REQUIRE(prop.major == 10, "sr3_b200 needs an sm_100 class GPU (found sm_%d%d); there is no fallback path", prop.major, prop.minor);
+        REQUIRE(prop.major == 9 && prop.minor == 0, "sr3_b200 needs an sm_90 GPU (found sm_%d%d); there is no fallback path", prop.major, prop.minor);
         REQUIRE(B >= 1, "batch must be >= 1");
         REQUIRE(cfg.inner_channel % 64 == 0, "inner_channel must be a multiple of 64 (got %d)", cfg.inner_channel);
         REQUIRE(cfg.in_channel <= 64, "in_channel must be <= 64");
@@ -1416,8 +1416,8 @@ struct sr3_engine {
 
     // ---- persistent step kernel: serialise the recorded ops (parameter blocks 128-byte aligned) and upload them
     void build_mega() {
-        // Off by default: measured on the B200 (profiles/r02_step_kernel.md) the grid barrier + per-op fill / drain costs as much as a
-        // launch inside a CUDA graph, and the 320-thread GroupNorm apply runs at half the bandwidth of the stand-alone kernel.
+        // Off by default: the grid barrier + per-op fill / drain cost about as much as a launch inside a CUDA graph, and the 288-thread
+        // GroupNorm apply has less bandwidth than the stand-alone kernel.
         // SR3_MEGA=1 selects it (bit-identical results).
         use_mega = !train && getenv("SR3_MEGA") != nullptr && atoi(getenv("SR3_MEGA")) != 0 && getenv("SR3_NO_FUSE_CAST") == nullptr && getenv("SR3_NO_FOLD_UP") == nullptr;
         if (!use_mega) return;
@@ -1501,7 +1501,7 @@ struct sr3_engine {
     void push_ctl(cudaStream_t st) { CK(cudaMemcpyAsync(ctl_dev, &ctl, sizeof(StepCtl), cudaMemcpyHostToDevice, st)); }
     void load_nchw(const float* src, int C, int coff, float* copy, cudaStream_t st) {
         const long long total = 1LL * B * C * H * W;
-        const int blocks = (int)std::min<long long>((total + 255) / 256, 148 * 8);
+        const int blocks = (int)std::min<long long>((total + 255) / 256, num_sms() * 8LL);
         load_nchw_kernel<<<blocks, 256, 0, st>>>(src, B, C, H, W, in_buf, in_C * PW, coff, copy, precise ? in_C : 0);
         CK(cudaGetLastError());
     }
@@ -1831,7 +1831,7 @@ int sr3_p_losses(sr3_engine* e, const float* hr, const float* sr, const float* g
     CK(cudaSetDevice(e->dev));
     if (e->cfg.conditional) { REQUIRE(sr != nullptr, "x_in['SR'] is required by a conditional model"); e->load_nchw(sr, e->cond_c, 0, nullptr, st); }
     const long long total = 1LL * e->B * e->cfg.channels * e->H * e->W;
-    const int blocks = (int)std::min<long long>((total + 255) / 256, 148 * 8);
+    const int blocks = (int)std::min<long long>((total + 255) / 256, num_sms() * 8LL);
     q_sample_load_kernel<<<blocks, 256, 0, st>>>(hr, noise, gamma, e->B, e->cfg.channels, e->H, e->W, e->in_buf, e->in_C * e->PW, e->cond_c,
                                                  e->precise ? e->in_C : 0);
     CK(cudaGetLastError());
@@ -2124,7 +2124,7 @@ int sr3_tensor2img(const float* src, unsigned char* dst, int n, int C, int H, in
         GH = rows * (H + 2) + 2; GW = ncol * (W + 2) + 2;
     }
     const long long total = 1LL * GH * GW * C;
-    const int blocks = (int)std::min<long long>((total + 255) / 256, 148 * 8);
+    const int blocks = (int)std::min<long long>((total + 255) / 256, num_sms() * 8LL);
     tensor2img_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(src, dst, n, C, H, W, ncol, GH, GW, min_v, max_v);
     CK(cudaGetLastError());
     API_END
@@ -2209,14 +2209,14 @@ int sr3_resize_bicubic_u8(const unsigned char* src, unsigned char* dst_u8, float
     unsigned char* tmp = static_cast<unsigned char*>(mem.alloc((size_t)B * h * W * C, false));
     {
         const long long total = 1LL * B * h * W * C;
-        resample_u8_kernel<<<(int)std::min<long long>((total + 255) / 256, 148 * 16), 256, 0, st>>>(
+        resample_u8_kernel<<<(int)std::min<long long>((total + 255) / 256, num_sms() * 16LL), 256, 0, st>>>(
             src, tmp, nullptr, B, /*lines*/ h, /*out*/ W, C, /*in axis*/ C, /*in line*/ 1LL * w * C, /*in img*/ 1LL * h * w * C,
             /*out axis*/ C, /*out line*/ 1LL * W * C, /*out img*/ 1LL * h * W * C, dbh, dch, ksh, 0, 0.f, 1.f);
         CK(cudaGetLastError());
     }
     {
         const long long total = 1LL * B * W * H * C;
-        resample_u8_kernel<<<(int)std::min<long long>((total + 255) / 256, 148 * 16), 256, 0, st>>>(
+        resample_u8_kernel<<<(int)std::min<long long>((total + 255) / 256, num_sms() * 16LL), 256, 0, st>>>(
             tmp, dst_u8, dst_f32, B, /*lines = x*/ W, /*out = y*/ H, C, /*in axis (y)*/ 1LL * W * C, /*in line (x)*/ C, /*in img*/ 1LL * h * W * C,
             /*out axis*/ 1LL * W * C, /*out line*/ C, /*out img*/ 1LL * H * W * C, dbv, dcv, ksv, flip, min_v, max_v);
         CK(cudaGetLastError());
@@ -2232,7 +2232,7 @@ int sr3_ssd_u8(const unsigned char* a, const unsigned char* b, int64_t n, unsign
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     DevAllocs mem;
     unsigned long long* d = static_cast<unsigned long long*>(mem.alloc(sizeof(unsigned long long)));
-    ssd_u8_kernel<<<(int)std::min<long long>((n + 255) / 256, 148 * 8), 256, 0, st>>>(a, b, (long long)n, d);
+    ssd_u8_kernel<<<(int)std::min<long long>((n + 255) / 256, num_sms() * 8LL), 256, 0, st>>>(a, b, (long long)n, d);
     CK(cudaGetLastError());
     CK(cudaMemcpyAsync(ssd_host, d, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));

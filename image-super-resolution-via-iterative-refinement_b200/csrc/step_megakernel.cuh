@@ -8,11 +8,11 @@
 //
 //     for op in ops:  [grid barrier]  ->  gemm tile loop | GroupNorm apply | fused attention | row softmax | embedding + FiLM | ...
 //
-// TMEM (512 columns) is allocated once, mbarriers live in a fixed shared-memory header and are recycled per op, parameter blocks
-// (incl. TMA descriptors) live in global memory and are copied into the header by every CTA.
+// mbarriers live in a fixed shared-memory header and are recycled per op, parameter blocks (incl. TMA descriptors) live in global
+// memory and are copied into the header by every CTA.
 #pragma once
 #include "aux_kernels.cuh"
-#include "attn_tcgen05.cuh"
+#include "attn_wgmma.cuh"
 
 namespace sr3 {
 
@@ -91,7 +91,7 @@ struct GridBarrier {
 };
 
 // ---------------------------------------------------------------------------------------------------------------- GroupNorm apply
-// Same arithmetic as prep_kernel (aux_kernels.cuh) for the 320-thread CTAs of the step kernel: a CTA owns a contiguous range of
+// Same arithmetic as prep_kernel (aux_kernels.cuh) for the 288-thread CTAs of the step kernel: a CTA owns a contiguous range of
 // (image, pixel block) items; scale / shift are rebuilt when the image changes.  Loads are L2-coherent (.cg): the data was produced
 // earlier in the same launch.
 __device__ __noinline__ void prep_body(const PrepParams& p, float* sm, const int cta, const int ncta) {
@@ -267,14 +267,13 @@ __device__ __noinline__ void embed_film_body(const EmbedFilmParams& p, float* sm
 // ---------------------------------------------------------------------------------------------------------------- the step kernel
 // (not inlined: every tile variant / op body gets its own register allocation instead of sharing the step kernel's)
 template <int BN, int MH>
-__device__ __noinline__ void mega_gemm(const uint8_t* hdr_params, const uint8_t* gparams, uint32_t base, uint8_t* base_ptr, uint32_t tmem_base,
-                                          int cta, int ncta) {
+__device__ __noinline__ void mega_gemm(const uint8_t* hdr_params, const uint8_t* gparams, uint32_t base, uint8_t* base_ptr, int cta, int ncta) {
     gemm_tile_body<BN, MH, true>(*reinterpret_cast<const GemmParams*>(hdr_params), reinterpret_cast<const GemmParams*>(gparams), base, base_ptr,
-                                 tmem_base, cta, ncta);
+                                 cta, ncta);
 }
 
-__device__ __noinline__ void mega_attn(const AttnParams& ap, const AttnParams* gp, uint32_t base, uint8_t* base_ptr, uint32_t tmem_base, int qt, int dc, int z) {
-    attn_unit<true>(ap, gp, base, base_ptr, tmem_base, qt, dc, z);
+__device__ __noinline__ void mega_attn(const AttnParams& ap, const AttnParams* gp, uint32_t base, uint8_t* base_ptr, int qt, int dc, int z) {
+    attn_unit<true>(ap, gp, base, base_ptr, qt, dc, z);
 }
 
 __global__ void __launch_bounds__(GEMM_THREADS, 1) step_kernel(const __grid_constant__ MegaParams mp) {
@@ -284,9 +283,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) step_kernel(const __grid_cons
     uint8_t* base_ptr = smem_raw + (base - raw);
     uint8_t* hdr_params = base_ptr + HDR_PARAMS;
     uint8_t* op_smem = base_ptr + GEMM_HDR_BYTES;
-    volatile uint32_t* tmem_slot = reinterpret_cast<volatile uint32_t*>(base_ptr + HDR_TMEM_SLOT);
-    volatile int* t_slot = reinterpret_cast<volatile int*>(base_ptr + HDR_TMEM_SLOT + 8);
-    const int warp = threadIdx.x >> 5;
+    volatile int* t_slot = reinterpret_cast<volatile int*>(base_ptr + HDR_SCALARS + 8);
     const int cta = blockIdx.x, ncta = gridDim.x;
 
     if (threadIdx.x == 0) {
@@ -294,16 +291,9 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) step_kernel(const __grid_cons
         fence_mbar_init();
         *t_slot = mp.ctl->t_next;                                                // this step's timestep (CTA 0 advances it at the very end)
     }
-    if (warp == 1) {
-        tmem_alloc(smem_u32(const_cast<uint32_t*>(tmem_slot)), 512);
-        tmem_relinquish();
-    }
     GridBarrier gb;
     gb.init(mp.bar, ncta);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     const int t_step = *t_slot;
 
     for (int i = 0; i < mp.n_ops; ++i) {
@@ -320,7 +310,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) step_kernel(const __grid_cons
         if (op.type == MOP_GEMM) {
             if (threadIdx.x == 0) reinterpret_cast<GemmParams*>(hdr_params)->t_fixed = t_step;
             gemm_stage_setup(*reinterpret_cast<const GemmParams*>(hdr_params), reinterpret_cast<const GemmParams*>(gparams), base, base_ptr,
-                             op.variant & 0xffff, true);
+                             op.variant & 0xffff, op.variant >> 16, true);
         }
         if (stamp) mp.prof[4 * i + 1] = globaltimer_ns();
         if (op.sync_before) gb.wait(i); else __syncthreads();
@@ -328,13 +318,13 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) step_kernel(const __grid_cons
         switch (op.type) {
             case MOP_GEMM: {
                 switch (op.variant) {
-                    case 16 | (1 << 16): mega_gemm<16, 1>(hdr_params, gparams, base, base_ptr, tmem_base, cta, ncta); break;
-                    case 16 | (2 << 16): mega_gemm<16, 2>(hdr_params, gparams, base, base_ptr, tmem_base, cta, ncta); break;
-                    case 32 | (1 << 16): mega_gemm<32, 1>(hdr_params, gparams, base, base_ptr, tmem_base, cta, ncta); break;
-                    case 64 | (1 << 16): mega_gemm<64, 1>(hdr_params, gparams, base, base_ptr, tmem_base, cta, ncta); break;
-                    case 64 | (2 << 16): mega_gemm<64, 2>(hdr_params, gparams, base, base_ptr, tmem_base, cta, ncta); break;
-                    case 128 | (1 << 16): mega_gemm<128, 1>(hdr_params, gparams, base, base_ptr, tmem_base, cta, ncta); break;
-                    case 128 | (2 << 16): mega_gemm<128, 2>(hdr_params, gparams, base, base_ptr, tmem_base, cta, ncta); break;
+                    case 16 | (1 << 16): mega_gemm<16, 1>(hdr_params, gparams, base, base_ptr, cta, ncta); break;
+                    case 16 | (2 << 16): mega_gemm<16, 2>(hdr_params, gparams, base, base_ptr, cta, ncta); break;
+                    case 32 | (1 << 16): mega_gemm<32, 1>(hdr_params, gparams, base, base_ptr, cta, ncta); break;
+                    case 64 | (1 << 16): mega_gemm<64, 1>(hdr_params, gparams, base, base_ptr, cta, ncta); break;
+                    case 64 | (2 << 16): mega_gemm<64, 2>(hdr_params, gparams, base, base_ptr, cta, ncta); break;
+                    case 128 | (1 << 16): mega_gemm<128, 1>(hdr_params, gparams, base, base_ptr, cta, ncta); break;
+                    case 128 | (2 << 16): mega_gemm<128, 2>(hdr_params, gparams, base, base_ptr, cta, ncta); break;
                     default: if (threadIdx.x == 0) printf("sr3: step kernel: unsupported tile variant %x\n", op.variant); __trap();
                 }
                 break;
@@ -347,7 +337,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) step_kernel(const __grid_cons
                 const int n_dc = ap.C / ap.dn, per_z = (ap.Lt / 128) * n_dc, units = per_z * ap.nz;
                 for (int u = cta; u < units; u += ncta) {
                     const int z = u / per_z, r = u % per_z;
-                    mega_attn(ap, reinterpret_cast<const AttnParams*>(gparams), base, base_ptr, tmem_base, r / n_dc, r % n_dc, z);
+                    mega_attn(ap, reinterpret_cast<const AttnParams*>(gparams), base, base_ptr, r / n_dc, r % n_dc, z);
                 }
                 break;
             }
@@ -377,9 +367,6 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) step_kernel(const __grid_cons
         mp.ctl->t_cur = t_step;               // what the per-layer path's step_begin_kernel does at the start of a step
         mp.ctl->t_next = t_step - 1;
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_base, 512);
 }
 
 }  // namespace sr3

@@ -1,9 +1,9 @@
 // Kernels of the TRAINING path (reference: model/model.py:48-58 optimize_parameters, model/sr3_modules/diffusion.py:221-246 p_losses):
 // everything the backward pass needs that is not the forward tile kernel.
 //
-//   * data gradients of every conv are the forward tile kernel (gemm_tcgen05.cuh) on re-packed weights (mirrored taps for 3x3 stride 1,
+//   * data gradients of every conv are the forward tile kernel (gemm_wgmma.cuh) on re-packed weights (mirrored taps for 3x3 stride 1,
 //     the four output-parity phases for the stride-2 Downsample conv, a 4x4 stride-2 kernel for nearest-2x + conv3x3): the packers are here;
-//   * weight gradients are a tcgen05 GEMM that contracts over PIXELS with both operands MN-major (wgrad_kernel);
+//   * weight gradients are a wgmma GEMM that contracts over PIXELS with both operands MN-major (wgrad_kernel);
 //   * GroupNorm + SiLU (+ Dropout) backward, bias / FiLM / noise-MLP gradients, attention backward, loss gradient, Adam.
 #pragma once
 #include "aux_kernels.cuh"
@@ -68,18 +68,17 @@ __global__ void __launch_bounds__(256) pack_up_dgrad_weight_kernel(const float* 
     }
 }
 
-// ------------------------------------------------------------------------------------------------ weight gradient (tcgen05, MN-major operands)
+// ------------------------------------------------------------------------------------------------ weight gradient (wgmma, MN-major operands)
 //     dW[co][tap][ci] = sum over pixels p of  dY[p][co] * X[p + tap][ci]
 // The contraction runs over PIXELS.  With NHWC activations both operands are MN-major (channels contiguous): a TMA box {64 channels, 8 x 8
-// pixels} with the 128-byte swizzle IS the canonical MN-major layout of the UMMA shared-memory descriptor
-//     Swizzle<3,4,3> o ((8,8,m),(8,k)) : ((1,8,LBO),(64,SBO))   [units of 16 bytes]
-// (CUTLASS cute/atom/mma_traits_sm100.hpp, make_umma_desc<Major::MN>): one 128 B row = 64 channels of one pixel, 8 pixels = one 1024 B atom
-// (SBO), the next 64-channel panel LBO bytes further; instruction-descriptor bits 15 / 16 select MN-major A / B.  A tap is the X box shifted
-// (TMA zero fill = padding); the stride-2 conv reads X through the parity view of the forward kernel.
-// One CTA = (128 output channels, 64 input channels, a group of <= 3 taps, a slice of the 8x8-pixel patches): <= 3 accumulators of 128 x 64
-// fp32 in TMEM, written as a partial tile into ws[slice][co][tap][ci]; wgrad_reduce_kernel sums the slices (fixed order: deterministic) and
-// writes the parameter gradient in the reference's OIHW layout.
-constexpr int WGRAD_THREADS = 192;
+// pixels} with the 128-byte swizzle IS the canonical MN-major layout of a wgmma shared-memory operand: one 128 B row = 64 channels of one
+// pixel, 8 pixels = one 1024 B atom, and a K step of 16 pixels is two atoms.  A tap is the X box shifted (TMA zero fill = padding); the
+// stride-2 conv reads X through the parity view of the forward kernel.
+// One CTA = (128 output channels, 64 input channels, a group of <= 3 taps, a slice of the 8x8-pixel patches): warpgroup g owns output
+// channels [64 g, 64 g + 64) and holds <= 3 accumulators of 64 x 64 fp32 in registers, written as a partial tile into
+// ws[slice][co][tap][ci]; wgrad_reduce_kernel sums the slices (fixed order: deterministic) and writes the parameter gradient in the
+// reference's OIHW layout.
+constexpr int WGRAD_THREADS = 288;                      // warps 0..7: two consumer warpgroups, warp 8: TMA producer
 constexpr int WGRAD_STAGES = 4;
 constexpr int WGRAD_STAGE_BYTES = 16384 + 3 * 8192;     // dY: 2 panels of 64 co x 64 px | X: 3 taps x (64 px x 64 ci)
 constexpr int WGRAD_SMEM_BYTES = 1024 + WGRAD_STAGES * WGRAD_STAGE_BYTES + 256;
@@ -98,30 +97,13 @@ struct WgradParams {
     WgradTap taps[WGRAD_MAX_TAPS];
 };
 
-// MN-major operand, 128-byte swizzle: [0,14) addr>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [46,48) version=1 | [61,64) layout=2
-__device__ __forceinline__ uint64_t umma_desc_mnmajor_sw128(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-    uint64_t d = 0;
-    d |= static_cast<uint64_t>((saddr & 0x3FFFF) >> 4);
-    d |= static_cast<uint64_t>(lbo_bytes >> 4) << 16;
-    d |= static_cast<uint64_t>(sbo_bytes >> 4) << 32;
-    d |= static_cast<uint64_t>(1) << 46;
-    d |= static_cast<uint64_t>(2) << 61;
-    return d;
-}
-__host__ __device__ constexpr uint32_t umma_idesc_bf16_mn(int m, int n) {      // as umma_idesc_bf16, both operands MN-major
-    return (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | (1u << 16) | (static_cast<uint32_t>(n >> 3) << 17) | (static_cast<uint32_t>(m >> 4) << 24);
-}
-
 __global__ void __launch_bounds__(WGRAD_THREADS, 1) wgrad_kernel(const __grid_constant__ WgradParams p) {
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw = smem_u32(smem_raw);
     const uint32_t base = (raw + 1023u) & ~1023u;
-    uint8_t* base_ptr = smem_raw + (base - raw);
     const uint32_t bar_base = base + WGRAD_STAGES * WGRAD_STAGE_BYTES;
     auto full_bar = [&](int s) { return bar_base + 8u * s; };
     auto empty_bar = [&](int s) { return bar_base + 8u * (WGRAD_STAGES + s); };
-    const uint32_t acc_full = bar_base + 8u * (2 * WGRAD_STAGES);
-    volatile uint32_t* tmem_slot = reinterpret_cast<volatile uint32_t*>(base_ptr + WGRAD_STAGES * WGRAD_STAGE_BYTES + 8 * (2 * WGRAD_STAGES + 1));
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int n_ci = p.Cin / 64;
@@ -134,25 +116,17 @@ __global__ void __launch_bounds__(WGRAD_THREADS, 1) wgrad_kernel(const __grid_co
     const int iters = it_end - it_begin;
     const int tiles_w = p.OW / 8, tiles_h = p.OH / 8;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         tma_prefetch_desc(&p.dy_map);
         tma_prefetch_desc(&p.x_map);
-        for (int s = 0; s < WGRAD_STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 1); }
-        mbar_init(acc_full, 1);
+        for (int s = 0; s < WGRAD_STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 2); }   // empty: one arrive per warpgroup
         fence_mbar_init();
     }
-    if (warp == 1) {
-        tmem_alloc(smem_u32(const_cast<uint32_t*>(tmem_slot)), 256);
-        tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     pdl_launch_dependents();
     pdl_wait();
 
-    if (warp == 0) {
+    if (warp == 8) {
         int s = 0;
         uint32_t ph = 0;
         for (int it = it_begin; it < it_end; ++it) {
@@ -173,60 +147,53 @@ __global__ void __launch_bounds__(WGRAD_THREADS, 1) wgrad_kernel(const __grid_co
             __syncwarp();
             if (++s == WGRAD_STAGES) { s = 0; ph ^= 1u; }
         }
-    } else if (warp == 1) {
-        // the X boxes of the CTA's taps lie 8192 B apart = the panel stride (LBO) of an MN-major operand: ONE UMMA of N = 64 * taps covers all
-        // of them (accumulator columns [tap * 64 + ci]), so the dY tile is read from shared memory once per K step, not once per tap
-        const uint32_t idesc = umma_idesc_bf16_mn(128, 64 * nt);
-        int s = 0;
+    } else if (warp < 8) {
+        // warpgroup g: output channels [co0 + 64 g, co0 + 64 g + 64); one 64 x 64 accumulator per tap (each tap's X box is one MN panel)
+        const int g = warp >> 2;
+        const bool leader = (threadIdx.x & 127) == 0;
+        float acc[3][32];
+#pragma unroll
+        for (int t = 0; t < 3; ++t)
+#pragma unroll
+            for (int j = 0; j < 32; ++j) acc[t][j] = 0.f;
+        int s = 0, prev = -1;
         uint32_t ph = 0;
         for (int it = 0; it < iters; ++it) {
             mbar_wait(full_bar(s), ph, 22);
-            tc_fence_after();
-            if (elect_one_sync()) {
-                const uint32_t st = base + s * WGRAD_STAGE_BYTES;
+            wgmma_fence();
+            const uint32_t st = base + s * WGRAD_STAGE_BYTES;
 #pragma unroll
-                for (int kk = 0; kk < 4; ++kk) {                       // 16 pixels = two 8-pixel atoms per UMMA
-                    const uint64_t adesc = umma_desc_mnmajor_sw128(st + kk * 2048, 8192, 1024);
-                    const uint64_t bdesc = umma_desc_mnmajor_sw128(st + 16384 + kk * 2048, 8192, 1024);
-                    umma_bf16_ss(tmem_base, adesc, bdesc, idesc, (it | kk) != 0);
-                }
-                umma_commit(empty_bar(s));
-                if (it == iters - 1) umma_commit(acc_full);
+            for (int kk = 0; kk < 4; ++kk) {                       // 16 pixels = two 8-pixel atoms per wgmma
+                const uint64_t adesc = wgmma_desc_sw128(st + g * 8192 + kk * 2048, 1024, 1024);
+#pragma unroll
+                for (int t = 0; t < 3; ++t)
+                    if (t < nt) Wgmma<64>::template mma<1, 1>(acc[t], adesc, wgmma_desc_sw128(st + 16384 + t * 8192 + kk * 2048, 1024, 1024), (it | kk) != 0);
             }
-            __syncwarp();
+            wgmma_commit();
+            if (prev >= 0) {
+                wgmma_wait<1>();
+                if (leader) mbar_arrive(empty_bar(prev));
+            }
+            prev = s;
             if (++s == WGRAD_STAGES) { s = 0; ph ^= 1u; }
         }
-    } else {
-        const int q = warp & 3;
-        const int co = co0 + q * 32 + lane;
-        const uint32_t t_row = tmem_base + (static_cast<uint32_t>(q * 32) << 16);
-        if (iters > 0) {
-            mbar_wait(acc_full, 0, 23);
-            tc_fence_after();
-        }
-#pragma unroll 1
-        for (int t = 0; t < nt; ++t) {
-#pragma unroll 1
-            for (int ch = 0; ch < 2; ++ch) {
-                uint32_t v[32];
-                if (iters > 0) {
-                    tmem_ld_32x32(t_row + t * 64 + ch * 32, v);
-                    tmem_ld_wait();
-                } else {
+        wgmma_wait<0>();
 #pragma unroll
-                    for (int j = 0; j < 32; ++j) v[j] = 0u;
-                }
+        for (int t = 0; t < 3; ++t) wgmma_fence_regs(acc[t]);
+        // register j of a thread: output channel row 16 (warp % 4) + lane / 4 + 8 ((j / 2) % 2), input channel 8 (j / 4) + 2 (lane % 4) + j % 2
+#pragma unroll
+        for (int t = 0; t < 3; ++t) {
+            if (t >= nt) continue;
+#pragma unroll
+            for (int j = 0; j < 32; j += 2) {
+                const int co = co0 + 64 * g + 16 * (warp & 3) + (lane >> 2) + 8 * ((j >> 1) & 1);
                 if (co >= p.cout_valid) continue;               // padded rows of the 128-row tile (Cout = 64 / 3): nobody reads them
-                float4* dst = reinterpret_cast<float4*>(p.ws + slice * p.ws_slice_stride + co * p.ws_row_stride + static_cast<long long>(tap0 + t) * p.Cin + ci0 + ch * 32);
-#pragma unroll
-                for (int j = 0; j < 8; ++j)
-                    dst[j] = make_float4(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1]), __uint_as_float(v[4 * j + 2]), __uint_as_float(v[4 * j + 3]));
+                const int ci = 8 * (j >> 2) + 2 * (lane & 3);
+                *reinterpret_cast<float2*>(p.ws + slice * p.ws_slice_stride + co * p.ws_row_stride + static_cast<long long>(tap0 + t) * p.Cin + ci0 + ci) =
+                    make_float2(acc[t][j], acc[t][j + 1]);
             }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_base, 256);
 }
 
 // grad[co][ci][tap] (OIHW) = gscale * sum over slices of ws[slice][co][tap][ci]   (ci < cin_valid, co < cout_valid).

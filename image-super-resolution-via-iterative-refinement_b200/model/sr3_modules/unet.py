@@ -2,7 +2,7 @@
 
 Unlike the reference this is NOT a tree of torch.nn layers: it is a flat parameter store whose `state_dict()` has exactly
 the reference's keys / shapes (so public `*_gen.pth` checkpoints load with strict=True) plus a handle to the native
-engine that executes the whole forward as hand-written sm_100a kernels.  `forward(x, time)` has the reference signature.
+engine that executes the whole forward as hand-written sm_90a kernels.  `forward(x, time)` has the reference signature.
 """
 import math
 from typing import Dict, List, Tuple

@@ -1,7 +1,7 @@
 """Multi-GPU sampling: the reverse trajectories of different images are independent (GroupNorm and attention are per
 sample), so the batch is sharded across ranks with NO per-step communication and the finished images are collected with one
 all-gather (SURVEY.md 8e).  The reference only offers nn.DataParallel for training and samples on GPU 0
-(model/model.py:60-78); this is the B200-native replacement for that path: one process per GPU, NCCL over NVLink.
+(model/model.py:60-78); this is the H100-native replacement for that path: one process per GPU, NCCL over NVLink.
 
 Noise comes from Philox streams keyed by the GLOBAL sample index, so the result does not depend on the number of ranks.
 

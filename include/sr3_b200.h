@@ -1,4 +1,4 @@
-/* sr3_b200 -- C ABI of the B200-native SR3 hot path (libsr3_b200.so).
+/* sr3_b200 -- C ABI of the H100-native SR3 hot path (libsr3_b200.so).
  *
  * The reference (Janspiry/Image-Super-Resolution-via-Iterative-Refinement) is pure Python/PyTorch and has no
  * FFI; its boundary for this path is the Python factory model/networks.py:83-116 `define_G(opt)` and the methods of

@@ -1,7 +1,7 @@
 """CPU oracle for the SR3 hot path  --  TEST INFRASTRUCTURE, NOT PRODUCT CODE.
 
 Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference
-legs may import this file.  The product path (the sm_100a CUDA library behind
+legs may import this file.  The product path (the sm_90a CUDA library behind
 include/sr3_b200.h) never routes through it.
 
 What it is: a functional (stateless) fp32/fp64 restatement, on CPU torch ops, of the

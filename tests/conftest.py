@@ -10,7 +10,7 @@ sys.dont_write_bytecode = False
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs a real H100 (run with -m gpu on a GPU machine)")
 
 
 def pytest_collection_modifyitems(config, items):

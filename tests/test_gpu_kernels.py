@@ -1,4 +1,4 @@
-"""GPU parity of the single tensor-core tile kernel (tcgen05 + TMA) against fp32 torch references on CPU,
+"""GPU parity of the single tensor-core tile kernel (wgmma + TMA) against fp32 torch references on CPU,
 called through the C ABI (sr3_test_gemm / sr3_test_conv)."""
 import pytest
 import torch

@@ -1,5 +1,5 @@
 """GPU parity of the TRAINING row (SURVEY.md 8f rank 1; reference model/model.py:48-58 optimize_parameters, diffusion.py:221-246 p_losses):
-gradients of every parameter from the native backward (dgrad = forward tile kernel on re-packed weights, wgrad = tcgen05 MN-major GEMM,
+gradients of every parameter from the native backward (dgrad = forward tile kernel on re-packed weights, wgrad = wgmma MN-major GEMM,
 GroupNorm / SiLU / Dropout / attention backward kernels) against the oracle's fp32 CPU autograd, Adam iterations against the golden fixture.
 bf16 tensor-core operands: tolerance 1e-2 on smooth losses; the L1 loss (sign(eps - noise) is discontinuous: a forward error of 1e-2 flips
 ~0.1 % of the signs, each flip moving the gradient by 2/N) is held to cosine similarity instead."""

@@ -6,7 +6,7 @@ reference's file naming and strict key matching, and a checkpoint written by the
 
 Needs the reference sources: /root/reference in the build container, or the verbatim copy oracle/build_ref.py puts into the
 git-ignored oracle/_ref (that copy travels to the GPU box, so the `gpu` test below -- the unmodified `DDPM.test()` / `DDPM.sample()`
-of model/model.py:60-78 driving our native sampler on a B200 -- runs there)."""
+of model/model.py:60-78 driving our native sampler on an H100 -- runs there)."""
 import os
 import sys
 
