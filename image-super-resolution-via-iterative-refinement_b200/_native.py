@@ -25,6 +25,17 @@ class UNetConfigC(ctypes.Structure):
 PRECISIONS = {"bf16": 0, "fp32": 1}          # "fp32" = precise mode: (hi, lo) bf16 operand pairs, three tensor-core passes
 
 
+class GemmGeometryC(ctypes.Structure):
+    _fields_ = [(n, c_int) for n in ("tall", "mh", "block_n", "h_box", "b_box", "ksplit", "stages", "ctas", "tiles", "res_smem")]
+
+
+class TestConvArgsC(ctypes.Structure):
+    _fields_ = [("x", c_void_p), ("w", c_void_p), ("bias", c_void_p), ("bias2", c_void_p), ("resid", c_void_p),
+                ("x2", c_void_p), ("w2", c_void_p),
+                ("y", c_void_p), ("y_bf16", c_void_p), ("stats", c_void_p)] + \
+               [(n, c_int) for n in ("B", "H", "W", "Cin", "Cout", "Cin2", "ksize", "stride", "fold_up", "precise")]
+
+
 _SIGS = {
     "sr3_last_error": (c_char_p, []),
     "sr3_abi_version": (c_int, []),
@@ -79,6 +90,9 @@ _SIGS = {
                                         c_int, c_void_p]),
     "sr3_test_conv": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
                               c_void_p]),
+    "sr3_test_conv_ex": (c_int, [POINTER(TestConvArgsC), POINTER(GemmGeometryC), c_void_p]),
+    "sr3_test_wgrad": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float,
+                               c_int, POINTER(c_int), c_void_p]),
 }
 EXPORTED_SYMBOLS = tuple(_SIGS.keys())
 
@@ -448,6 +462,46 @@ def test_conv(x_nhwc_bf16, w_oihw, bias, ksize, stride, want_stats=False):
     stats = torch.zeros(B, Cout, 2, device=y.device, dtype=torch.float64) if want_stats else None
     _check(lib().sr3_test_conv(_ptr(x_nhwc_bf16), _ptr(w_oihw), _ptr(bias), _ptr(y), _ptr(stats), B, H, W, Cin, Cout, ksize, stride, _stream()))
     return y, stats
+
+
+def test_conv_ex(x, w, ksize=3, stride=1, bias=None, bias2=None, resid=None, x2=None, w2=None, want_bf16=False, want_stats=False,
+                 fold_up=False, precise=False):
+    """One image conv as a UNet layer builds it (sr3_test_conv_ex); CUDA operands.  x bf16 NHWC [B,H,W,Cin] ([B,H,W,2Cin] = [hi | lo] when
+    precise), w fp32 OIHW.  Returns (y fp32 NHWC, y_bf16 or None, stats fp64 [B,Cout,2] or None, geometry dict)."""
+    B, H, W, CX = x.shape
+    Cin = CX // 2 if precise else CX
+    Cout = w.shape[0]
+    OH, OW = (2 * H, 2 * W) if fold_up else (H // stride, W // stride)
+    y = torch.empty(B, OH, OW, Cout, device=x.device, dtype=torch.float32)
+    yb = torch.empty(B, OH, OW, Cout * (2 if precise else 1), device=x.device, dtype=torch.bfloat16) if want_bf16 else None
+    stats = torch.zeros(B, Cout, 2, device=x.device, dtype=torch.float64) if want_stats else None
+    keep = [_f32c(t, x.device) if t is not None else None for t in (w, bias, bias2, resid, w2)]
+    a = TestConvArgsC()
+    a.x, a.w, a.bias, a.bias2, a.resid = x.data_ptr(), *[(t.data_ptr() if t is not None else None) for t in keep[:4]]
+    a.x2 = x2.data_ptr() if x2 is not None else None
+    a.w2 = keep[4].data_ptr() if keep[4] is not None else None
+    a.y, a.y_bf16, a.stats = y.data_ptr(), (yb.data_ptr() if yb is not None else None), (stats.data_ptr() if stats is not None else None)
+    a.B, a.H, a.W, a.Cin, a.Cout = B, H, W, Cin, Cout
+    a.Cin2 = (x2.shape[3] // (2 if precise else 1)) if x2 is not None else 0
+    a.ksize, a.stride, a.fold_up, a.precise = ksize, stride, int(bool(fold_up)), int(bool(precise))
+    geo = GemmGeometryC()
+    _check(lib().sr3_test_conv_ex(ctypes.byref(a), ctypes.byref(geo), _stream()))
+    return y, yb, stats, {n: getattr(geo, n) for n, _ in GemmGeometryC._fields_}
+
+
+def test_wgrad(dy, x, ksize, stride=1, cout_valid=None, cin_valid=None, slices=0, gscale=1.0, raw=False):
+    """Weight gradient through wgrad_kernel + wgrad_reduce_kernel (sr3_test_wgrad).  dy bf16 NHWC [B,OH,OW,CY], x bf16 NHWC [B,H,W,Cin].
+    Returns (grad fp32 OIHW [cout_valid, cin_valid, k, k], or [B, CY, Cin] when raw; slices used)."""
+    B, OH, OW, CY = dy.shape
+    Cin = x.shape[3]
+    cv = CY if cout_valid is None else cout_valid
+    civ = Cin if cin_valid is None else cin_valid
+    shape = (B, CY, Cin) if raw else (cv, civ, ksize, ksize)
+    g = torch.empty(shape, device=dy.device, dtype=torch.float32)
+    used = c_int()
+    _check(lib().sr3_test_wgrad(_ptr(dy), _ptr(x), _ptr(g), B, OH, OW, CY, Cin, ksize, stride, cv, civ, int(slices), float(gscale), int(bool(raw)),
+                                ctypes.byref(used), _stream()))
+    return g, used.value
 
 
 def test_conv_groupnorm(x_nhwc_bf16, w_oihw, bias, gamma, beta, groups, silu, ksize):

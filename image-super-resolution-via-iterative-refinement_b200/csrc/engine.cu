@@ -301,8 +301,9 @@ void mega_record(int type, const T& params) {
 }
 static thread_local std::vector<GemmHandle>* g_gemm_registry = nullptr;   // set by the engine while it builds its plan
 
-// Turns a GemmDesc into a launchable op (encodes the TMA maps, uploads the K-slab table).
-Op make_gemm_op(const GemmDesc& d, DevAllocs& mem) {
+// Turns a GemmDesc into a launchable op (encodes the TMA maps, uploads the K-slab table).  `geo` (optional) receives the variant and
+// launch shape that were actually chosen, after every host-side override and cap.
+Op make_gemm_op(const GemmDesc& d, DevAllocs& mem, sr3_gemm_geometry* geo = nullptr) {
     REQUIRE(d.w_box * d.h_box * d.b_box == 128 * d.mh, "tile box must cover %d rows", 128 * d.mh);
     REQUIRE(!d.slabs.empty(), "gemm without K slabs");
     GemmParams p;
@@ -455,6 +456,8 @@ Op make_gemm_op(const GemmDesc& d, DevAllocs& mem) {
     const int total_tiles = d.tiles_w * d.tiles_h * d.tiles_b * d.n_tiles * d.nz * p.ksplit;
     int ctas = total_tiles < num_sms() ? total_tiles : num_sms();
     if (const char* e = getenv("SR3_MAX_CTAS")) { int v = atoi(e); if (v > 0 && v < ctas) ctas = v; }
+    // the split-K partners of a tile wait for each other inside the kernel: a CTA that owned two splits of one tile would wait for itself
+    REQUIRE(p.ksplit == 1 || ctas == total_tiles, "split-K launch needs one CTA per (tile, split) pair: %d CTAs for %d (SR3_MAX_CTAS with a split tile)", ctas, total_tiles);
     const dim3 grid(ctas, 1, 1);
     const int bn = d.block_n;
     const int mh = d.mh;
@@ -464,6 +467,10 @@ Op make_gemm_op(const GemmDesc& d, DevAllocs& mem) {
     REQUIRE(smem <= SMEM_LIMIT, "gemm shared memory %d exceeds the limit", smem);
     init_gemm_attrs();
     REQUIRE((bn == 16 || bn == 32 || bn == 64 || bn == 128 || bn == 256) && (mh == 1 || (mh == 2 && bn <= 128 && bn != 32)), "unsupported tile %dx%d", 128 * mh, bn);
+    if (geo) {
+        geo->tall = d.tall; geo->mh = mh; geo->block_n = bn; geo->h_box = d.h_box; geo->b_box = d.b_box;
+        geo->ksplit = p.ksplit; geo->stages = p.stages; geo->ctas = ctas; geo->tiles = total_tiles / p.ksplit; geo->res_smem = res_smem ? 1 : 0;
+    }
     std::shared_ptr<GemmParams> sp = std::make_shared<GemmParams>(p);
     if (g_gemm_registry) {
         GemmHandle h; h.p = sp; h.w_ptr = d.b_ptr; h.w_bytes = 2LL * d.b_rows * d.b_K; h.w_is_param = d.b_is_param; h.bn = bn; h.mh = mh;
@@ -667,6 +674,153 @@ struct ParamEntry {
 
 struct LayerSpec { std::string name; int kind; int cin, cout; bool attn; int res; };   // kind: 0 conv, 1 res, 2 down, 3 up
 
+// precise mode: three passes over the stage table; the low halves of A source i start c_i channels after its high halves, those of the
+// weights ktot columns after theirs
+void set_precise_fields(GemmDesc& d, int c0, int c1, int ktot) {
+    d.passes = 3; d.lo_a_chan[0] = c0; d.lo_a_chan[1] = c1; d.lo_b_col = ktot;
+}
+
+// generic image conv: A sources already bf16; out fp32 NHWC (+stats)
+struct ConvArgs {
+    ASrc a[2]; int n_a = 1;
+    std::vector<KSlab> slabs;
+    const bf16* w = nullptr; int ktot = 0; int cout = 0;
+    int OH = 0, OW = 0;
+    const float* bias = nullptr; const float* bias2 = nullptr; int bias2_stride = 0;
+    const float* resid = nullptr;
+    Act out;
+    bf16* raw_out = nullptr;          // also store bf16(out) (input of a following Down / Upsample conv): no separate cast pass
+    bool custom_os = false; OutSpec os{};   // output addressing other than plain NHWC (phase of a folded upsample conv)
+    int nz = 1, b_zrows = 0, z_phase = 0; long long z_off_hi = 0, z_off_lo = 0;   // the four phases of a folded upsample conv in ONE launch
+    int c0 = 0, c1 = 0;               // channels of the A sources (precise mode: where their low halves start)
+};
+
+// Tile-kernel descriptor of an image conv over B images (Bp allocated, B <= Bp); PW = 2 in precise mode ([hi | lo] operand pairs).
+// The engine's layer builders and the stand-alone test hook both go through here.
+GemmDesc conv_desc(const ConvArgs& c, int B, int Bp, int PW) {
+    GemmDesc d;
+    d.n_a = c.n_a; d.a[0] = c.a[0]; d.a[1] = c.a[1];
+    d.slabs = c.slabs;
+    REQUIRE(PW == 1 || c.c0 > 0, "precise mode: conv without source channel counts");
+    // the bf16 store addresses plain NHWC rows: it has no phase offsets (z_off_*) and no custom output map
+    REQUIRE(!(c.raw_out && c.custom_os), "a bf16 copy of a phase-addressed (folded upsample) output is not supported");
+    if (PW == 2) set_precise_fields(d, c.c0, c.c1, c.ktot);
+    conv_geometry(d, c.OW, c.OH, Bp, c.cout, c.resid != nullptr, c.nz);
+    d.b_ptr = c.w; d.b_K = PW * c.ktot; d.b_rows = (long long)c.nz * (((c.cout + 127) / 128) * 128);      // weights are padded to 128 rows (new_weight)
+    d.b_is_param = true;
+    d.n_tiles = (c.cout + d.block_n - 1) / d.block_n; d.nz = c.nz; d.a_zstep = 0; d.b_zrows = c.b_zrows;
+    d.z_phase = c.z_phase; d.z_off_hi = c.z_off_hi; d.z_off_lo = c.z_off_lo;
+    d.OW = c.OW; d.OH = c.OH; d.OB = B; d.n_valid = c.cout;
+    d.bias = c.bias; d.bias2 = c.bias2; d.bias2_stride = c.bias2_stride;
+    d.resid = c.resid; d.rs = nhwc_out(c.OH, c.OW, c.cout);
+    d.out_f32 = c.out.p; d.os = c.custom_os ? c.os : nhwc_out(c.OH, c.OW, c.cout);
+    if (c.raw_out) { d.out_bf16 = c.raw_out; d.hs = nhwc_out(c.OH, c.OW, PW * c.cout); d.lo_out_off = PW == 2 ? c.cout : 0; }
+    d.stats = c.out.stats; d.stats_C = c.cout; d.stats_coff = 0;
+    return d;
+}
+
+// Upsample folded (nearest 2x -> conv3x3 on a Hl x Wl x C input, bf16 NHWC rows of PW * C at `raw`): output pixel (2i+py, 2j+px) only sees
+// a 2x2 neighbourhood of the low-res input, with the 3x3 taps that alias onto the same low-res pixel summed into one weight
+// (fold_upsample_weight_kernel: exact in real arithmetic, 2.25x fewer MACs, no 4x-sized intermediate).  Fills the A source, K slabs and
+// output addressing of phase `ph` (py = ph / 2, px = ph % 2), each phase writing its quarter of the NHWC output; merge: all four phases in
+// one op (gemm-batch z = phase, weights of phase z start at row z * rows_pad).  The caller sets weights, bias and output.
+void fold_up_conv(ConvArgs& c, const bf16* raw, int Bp, int Hl, int Wl, int C, int PW, int ph, bool merge) {
+    const int py = ph >> 1, px = ph & 1;
+    c.n_a = 1; c.a[0] = nhwc_src(raw, Bp, Hl, Wl, C * PW); c.c0 = C;
+    for (int a = 0; a < 2; ++a)
+        for (int bb = 0; bb < 2; ++bb)
+            for (int ch = 0; ch < C; ch += 64) {
+                KSlab k; k.a_sel = 0; k.a_chan = ch; k.dh = py - 1 + a; k.dw = px - 1 + bb; k.p = 0; k.b_col = (a * 2 + bb) * C + ch;
+                c.slabs.push_back(k);
+            }
+    c.ktot = 4 * C; c.cout = C; c.OH = Hl; c.OW = Wl;
+    c.custom_os = true;
+    c.os.sZ = 0; c.os.sB = 4LL * Hl * Wl * C; c.os.sH = 4LL * Wl * C; c.os.sW = 2LL * C; c.os.off = (long long)py * 2 * Wl * C + (long long)px * C;
+    if (merge) { c.nz = 4; c.b_zrows = ((C + 127) / 128) * 128; c.z_phase = 1; c.z_off_hi = 2LL * Wl * C; c.z_off_lo = C; }
+}
+
+// ---- weight gradient (wgrad_kernel + wgrad_reduce_kernel), shared by the training plan and the stand-alone test hook
+std::vector<WgradTap> taps_3x3() {
+    std::vector<WgradTap> t;
+    for (int r = 0; r < 3; ++r) for (int s = 0; s < 3; ++s) t.push_back({0, s - 1, 0, r - 1});
+    return t;
+}
+std::vector<WgradTap> taps_1x1() { return {{0, 0, 0, 0}}; }
+// stride-2 conv: input pixel (2 oh + r - 1, 2 ow + s - 1) in the (2C, W/2, 2, H/2, B) parity view (see add_conv_slabs)
+std::vector<WgradTap> taps_3x3_stride2(int C) {
+    std::vector<WgradTap> t;
+    for (int r = 0; r < 3; ++r) for (int s = 0; s < 3; ++s) t.push_back({(s == 1) ? 0 : C, (s == 0) ? -1 : 0, (r == 1) ? 0 : 1, (r == 0) ? -1 : 0});
+    return t;
+}
+
+// WgradOut: instead of a parameter gradient, every one of `nb` batches (one slice each, no reduction) writes its own [CY][Cin] result at
+// ptr + batch * slice_stride + row * row_stride + col: the attention backward's dV = P^T dO and dK = dS^T Q (contractions over the query index)
+struct WgradOut { float* ptr = nullptr; long long slice_stride = 0, row_stride = 0; int nb = 0; };
+
+// Grid of the weight gradient of one conv: x = (co_pad / 128) * (Cin / 64) output tiles, y = groups of <= 3 taps, z = slices of the
+// nbatch * (OH/8) * (OW/8) pixel patches.  slices = 0: the default (one wave of CTAs); raw: one slice per batch.
+struct WgradShape { int co_pad = 0, tpc = 0, nx = 0, ny = 0, patches = 0, slices = 0; };
+WgradShape wgrad_shape(int CY, int OHh, int OWw, int nbatch, int Cin, int ntaps, int slices, const WgradOut* raw) {
+    REQUIRE(OHh % 8 == 0 && OWw % 8 == 0 && Cin % 64 == 0 && CY % 64 == 0, "wgrad geometry %dx%d Cin=%d CY=%d", OHh, OWw, Cin, CY);
+    REQUIRE(ntaps >= 1 && ntaps <= WGRAD_MAX_TAPS, "too many taps");
+    WgradShape s;
+    s.co_pad = ((CY + 127) / 128) * 128;
+    s.tpc = ntaps < 3 ? ntaps : 3;
+    s.ny = (ntaps + s.tpc - 1) / s.tpc;
+    s.nx = (s.co_pad / 128) * (Cin / 64);
+    s.patches = nbatch * (OHh / 8) * (OWw / 8);
+    if (raw) {
+        s.slices = raw->nb;
+    } else if (slices > 0) {
+        REQUIRE(slices <= s.patches, "%d slices of %d patches", slices, s.patches);
+        s.slices = slices;
+    } else {
+        // one wave of CTAs: a CTA's fixed cost (pipeline fill, 96 KB partial tile out) is as long as ~10 K steps of its main loop,
+        // and every extra slice is another partial tile for the reduction kernel to read
+        const int nxy = s.nx * s.ny;
+        s.slices = getenv("SR3_WGRAD_WAVES") ? (atoi(getenv("SR3_WGRAD_WAVES")) * num_sms() + nxy - 1) / nxy : (num_sms() + nxy / 2) / nxy;
+        if (s.slices > s.patches / 2) s.slices = s.patches / 2;
+        if (s.slices < 1) s.slices = 1;
+    }
+    return s;
+}
+// dW[co][tap][ci] = sum_p dY[p][co] X[p + tap][ci] as partial tiles ws[slice][co][tap][ci].  dy: bf16 [nmap][OH][OW][CY] (nmap >= the
+// batches the patches cover); xs: the X view the taps index (nhwc_src / nhwc_stride2_src)
+WgradParams wgrad_params(const WgradShape& s, const bf16* dy, int CY, int OHh, int OWw, int nmap, int nbatch, const ASrc& xs, int Cin,
+                         const std::vector<WgradTap>& taps, int cout_valid, float* ws, const WgradOut* raw) {
+    WgradParams p; memset(&p, 0, sizeof(p));
+    const int ntaps = (int)taps.size();
+    {
+        const uint64_t dims[5] = {(uint64_t)CY, (uint64_t)OWw, 1ull, (uint64_t)OHh, (uint64_t)nmap};
+        const uint64_t str[4] = {2ull * CY, 2ull * OWw * CY, 2ull * OWw * CY, 2ull * OHh * OWw * CY};
+        const uint32_t box[5] = {64u, 8u, 1u, 8u, 1u};
+        p.dy_map = encode_map(5, dy, dims, str, box);
+    }
+    {
+        const uint64_t dims[5] = {(uint64_t)xs.C, (uint64_t)xs.W, (uint64_t)xs.P, (uint64_t)xs.H, (uint64_t)xs.Bn};
+        const uint64_t str[4] = {(uint64_t)xs.sW, (uint64_t)xs.sP, (uint64_t)xs.sH, (uint64_t)xs.sB};
+        const uint32_t box[5] = {64u, 8u, 1u, 8u, 1u};
+        p.x_map = encode_map(5, xs.ptr, dims, str, box);
+    }
+    p.ws = ws; p.Cin = Cin; p.co_pad = s.co_pad; p.cout_valid = cout_valid;
+    p.ws_slice_stride = raw ? raw->slice_stride : (long long)s.co_pad * ntaps * Cin; p.ws_row_stride = raw ? raw->row_stride : (long long)ntaps * Cin;
+    p.OH = OHh; p.OW = OWw; p.B = nbatch; p.ntaps = ntaps; p.taps_per_cta = s.tpc; p.patches = s.patches; p.slices = s.slices;
+    for (int i = 0; i < ntaps; ++i) p.taps[i] = taps[i];
+    return p;
+}
+// slice reduction into the OIHW gradient [cout_valid][cin_valid][taps] (block range and destination are set where the launch is batched)
+WgradReduceDesc wgrad_reduce_desc(const WgradShape& s, const float* ws, int ntaps, int Cin, int cout_valid, int cin_valid) {
+    const int sw = s.slices >= 8 ? 8 : (s.slices >= 4 ? 4 : (s.slices >= 2 ? 2 : 1));
+    const int ci_per_block = 32 * (8 / sw);
+    WgradReduceDesc rd{}; rd.ws = ws; rd.grad = nullptr; rd.slices = s.slices; rd.co_pad = s.co_pad; rd.ntaps = ntaps; rd.Cin = Cin; rd.cout_valid = cout_valid;
+    rd.cin_valid = cin_valid; rd.sw = sw; rd.blocks_x = (cin_valid + ci_per_block - 1) / ci_per_block;
+    return rd;
+}
+void init_wgrad_attrs() {
+    static std::vector<int> seen;
+    if (first_use_on_device(seen)) CK(cudaFuncSetAttribute(wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WGRAD_SMEM_BYTES));
+}
+
 }  // namespace
 
 struct sr3_engine {
@@ -832,8 +986,7 @@ struct sr3_engine {
     }
     // precise-mode fields of an image conv whose A sources have c0 (c1) channels and whose weight rows hold ktot (high) columns
     void set_precise(GemmDesc& d, int c0, int c1, int ktot) {
-        if (!precise) return;
-        d.passes = 3; d.lo_a_chan[0] = c0; d.lo_a_chan[1] = c1; d.lo_b_col = ktot;
+        if (precise) set_precise_fields(d, c0, c1, ktot);
     }
     void push(Op op, int kind = 4, double flops = 0, double bytes = 0) {
         if (dry) return;
@@ -913,39 +1066,9 @@ struct sr3_engine {
         push([=](cudaStream_t st) { launch_k(cast_kernel, dim3(blocks), dim3(256), 0, st, src, dst, Bn, Hh, Ww, C, up); }, 2, 0, (double)Bn * Hh * Ww * C * (4.0 + 2.0 * up * up));
     }
 
-    // generic image conv: A sources already bf16; out fp32 NHWC (+stats)
-    struct ConvArgs {
-        ASrc a[2]; int n_a = 1;
-        std::vector<KSlab> slabs;
-        const bf16* w = nullptr; int ktot = 0; int cout = 0;
-        int OH = 0, OW = 0;
-        const float* bias = nullptr; const float* bias2 = nullptr; int bias2_stride = 0;
-        const float* resid = nullptr;
-        Act out;
-        bf16* raw_out = nullptr;          // also store bf16(out) (input of a following Down / Upsample conv): no separate cast pass
-        bool custom_os = false; OutSpec os{};   // output addressing other than plain NHWC (phase of a folded upsample conv)
-        int nz = 1, b_zrows = 0, z_phase = 0; long long z_off_hi = 0, z_off_lo = 0;   // the four phases of a folded upsample conv in ONE launch
-        int c0 = 0, c1 = 0;               // channels of the A sources (precise mode: where their low halves start)
-    };
     void add_conv(const ConvArgs& c) {
         if (dry) return;
-        GemmDesc d;
-        d.n_a = c.n_a; d.a[0] = c.a[0]; d.a[1] = c.a[1];
-        d.slabs = c.slabs;
-        REQUIRE(!precise || c.c0 > 0, "precise mode: conv without source channel counts");
-        set_precise(d, c.c0, c.c1, c.ktot);
-        conv_geometry(d, c.OW, c.OH, Bp, c.cout, c.resid != nullptr, c.nz);
-        d.b_ptr = c.w; d.b_K = PW * c.ktot; d.b_rows = (long long)c.nz * (((c.cout + 127) / 128) * 128);      // weights are padded to 128 rows (new_weight)
-        d.b_is_param = true;
-        d.n_tiles = (c.cout + d.block_n - 1) / d.block_n; d.nz = c.nz; d.a_zstep = 0; d.b_zrows = c.b_zrows;
-        d.z_phase = c.z_phase; d.z_off_hi = c.z_off_hi; d.z_off_lo = c.z_off_lo;
-        d.OW = c.OW; d.OH = c.OH; d.OB = B; d.n_valid = c.cout;
-        d.bias = c.bias; d.bias2 = c.bias2; d.bias2_stride = c.bias2_stride;
-        d.resid = c.resid; d.rs = nhwc_out(c.OH, c.OW, c.cout);
-        d.out_f32 = c.out.p; d.os = c.custom_os ? c.os : nhwc_out(c.OH, c.OW, c.cout);
-        if (c.raw_out) { d.out_bf16 = c.raw_out; d.hs = nhwc_out(c.OH, c.OW, PW * c.cout); d.lo_out_off = precise ? c.cout : 0; }
-        d.stats = c.out.stats; d.stats_C = c.cout; d.stats_coff = 0;
-        push_gemm(d);
+        push_gemm(conv_desc(c, B, Bp, PW));
     }
 
     // ResnetBlock (+ optional SelfAttention): reference unet.py:94-158
@@ -1270,9 +1393,7 @@ struct sr3_engine {
                 add_conv(c);
                 x = y;
             } else {
-                // Upsample folded: output pixel (2i+py, 2j+px) only sees a 2x2 neighbourhood of the low-res input, with the
-                // 3x3 taps that alias onto the same low-res pixel summed into one weight (exact in real arithmetic, 2.25x fewer
-                // MACs, no 4x-sized intermediate).  One GEMM per phase, each writing its quarter of the NHWC output.
+                // Upsample folded onto the low-res input (fold_up_conv)
                 const int C = x.C, Hl = x.H, Wl = x.W;
                 const int rows_pad = ((C + 127) / 128) * 128;
                 const bool merge = getenv("SR3_NO_MERGE_UP") == nullptr;        // all four phases in one launch / op (gemm-batch z = phase)
@@ -1302,18 +1423,9 @@ struct sr3_engine {
                 }
                 Act y = new_act(C, Hl * 2, Wl * 2, L.name);
                 for (int ph = 0; ph < (merge ? 1 : 4); ++ph) {
-                    const int py = ph >> 1, px = ph & 1;
-                    ConvArgs c; c.n_a = 1; c.a[0] = nhwc_src(raw, Bp, Hl, Wl, C * PW); c.c0 = C;
-                    for (int a = 0; a < 2; ++a)
-                        for (int bb = 0; bb < 2; ++bb)
-                            for (int ch = 0; ch < C; ch += 64) {
-                                KSlab k; k.a_sel = 0; k.a_chan = ch; k.dh = py - 1 + a; k.dw = px - 1 + bb; k.p = 0; k.b_col = (a * 2 + bb) * C + ch;
-                                c.slabs.push_back(k);
-                            }
-                    c.w = wf[ph]; c.ktot = 4 * C; c.cout = C; c.OH = Hl; c.OW = Wl; c.bias = b; c.out = y;
-                    c.custom_os = true;
-                    c.os.sZ = 0; c.os.sB = 4LL * Hl * Wl * C; c.os.sH = 4LL * Wl * C; c.os.sW = 2LL * C; c.os.off = (long long)py * 2 * Wl * C + (long long)px * C;
-                    if (merge) { c.nz = 4; c.b_zrows = rows_pad; c.z_phase = 1; c.z_off_hi = 2LL * Wl * C; c.z_off_lo = C; }
+                    ConvArgs c;
+                    fold_up_conv(c, raw, Bp, Hl, Wl, C, PW, ph, merge);
+                    c.w = wf[ph]; c.bias = b; c.out = y;
                     add_conv(c);
                 }
                 if (train) bwd_upsample(L.name, x, y, upb);
@@ -2083,31 +2195,91 @@ int sr3_bench_conv(int B, int H, int W, int Cin, int Cout, int ksize, int stride
     API_END
 }
 
-int sr3_test_conv(const void* x, const float* w_oihw, const float* bias, float* y, double* stats, int B, int H, int W, int Cin, int Cout,
-                  int ksize, int stride, void* stream) {
+int sr3_test_conv_ex(const sr3_test_conv_args* a, sr3_gemm_geometry* geometry, void* stream) {
     API_BEGIN
-    REQUIRE((ksize == 1 || ksize == 3) && (stride == 1 || stride == 2) && Cin % 64 == 0 && Cout % 64 == 0, "bad test conv shape");
+    REQUIRE(a && a->x && a->w && a->y, "null argument");
+    const int B = a->B, H = a->H, W = a->W, Cin = a->Cin, Cout = a->Cout, k = a->ksize, s = a->stride;
+    const int PW = a->precise ? 2 : 1;
+    REQUIRE(B >= 1 && (k == 1 || k == 3) && (s == 1 || s == 2) && Cin % 64 == 0 && Cout % 64 == 0, "bad test conv shape");
+    REQUIRE(!a->fold_up || (k == 3 && s == 1 && Cin == Cout && !a->x2), "folded upsample: 3x3 stride 1 with Cin == Cout and one source");
+    REQUIRE(!a->x2 || (a->w2 && a->Cin2 > 0 && a->Cin2 % 64 == 0 && s == 1), "second source: 1x1 weights over Cin2 (multiple of 64) channels, stride 1");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     DevAllocs mem;
-    const int ktot = ksize * ksize * Cin;
-    bf16* wp = static_cast<bf16*>(mem.alloc((size_t)Cout * ktot * 2));
-    pack_conv_weight_kernel<<<1024, 256, 0, st>>>(w_oihw, wp, Cout, Cin, ksize, ksize, ktot, 0, Cin, 0);
-    CK(cudaGetLastError());
-    const int OH = H / stride, OW = W / stride;
-    GemmDesc d; d.n_a = 1;
-    d.a[0] = stride == 1 ? nhwc_src(x, B, H, W, Cin) : nhwc_stride2_src(x, B, H, W, Cin);
-    add_conv_slabs(d.slabs, 0, Cin, ksize, stride, 0);
-    conv_geometry(d, OW, OH, B, Cout);
-    d.b_ptr = wp; d.b_K = ktot; d.b_rows = Cout;
+    const int rows_pad = ((Cout + 127) / 128) * 128;
+    ConvArgs c;
+    if (a->fold_up) {
+        fold_up_conv(c, static_cast<const bf16*>(a->x), B, H, W, Cin, PW, 0, true);
+        const int ldw = PW * c.ktot;
+        bf16* wall = static_cast<bf16*>(mem.alloc((size_t)4 * rows_pad * ldw * sizeof(bf16)));     // [phase][rows_pad][PW * 4C]
+        const long long phase = (long long)rows_pad * ldw;
+        fold_upsample_weight_kernel<<<1024, 256, 0, st>>>(a->w, wall, wall + phase, wall + 2 * phase, wall + 3 * phase, Cout, Cin, ldw, PW == 2 ? c.ktot : 0);
+        CK(cudaGetLastError());
+        c.w = wall;
+    } else {
+        const int ktot = k * k * Cin + (a->x2 ? a->Cin2 : 0), ld = PW * ktot, lo_off = PW == 2 ? ktot : 0;
+        bf16* wp = static_cast<bf16*>(mem.alloc((size_t)rows_pad * ld * sizeof(bf16)));
+        pack_conv_weight_kernel<<<1024, 256, 0, st>>>(a->w, wp, Cout, Cin, k, k, ld, 0, Cin, lo_off);
+        CK(cudaGetLastError());
+        c.a[0] = s == 1 ? nhwc_src(a->x, B, H, W, Cin * PW) : nhwc_stride2_src(a->x, B, H, W, Cin * PW); c.c0 = Cin;
+        add_conv_slabs(c.slabs, 0, Cin, k, s, 0, Cin * PW);
+        if (a->x2) {      // ResnetBlock block2 + res_conv (add_res_block): the 1x1 shortcut is K columns [k*k*Cin, ktot) of the same GEMM
+            pack_conv_weight_kernel<<<1024, 256, 0, st>>>(a->w2, wp, Cout, a->Cin2, 1, 1, ld, k * k * Cin, a->Cin2, lo_off);
+            CK(cudaGetLastError());
+            c.n_a = 2; c.a[1] = nhwc_src(a->x2, B, H, W, a->Cin2 * PW); c.c1 = a->Cin2;
+            add_conv_slabs(c.slabs, 1, a->Cin2, 1, 1, k * k * Cin);
+        }
+        c.w = wp; c.ktot = ktot; c.cout = Cout; c.OH = H / s; c.OW = W / s;
+    }
+    c.bias = a->bias; c.bias2 = a->bias2; c.bias2_stride = Cout; c.resid = a->resid;
+    c.out.p = a->y; c.out.stats = a->stats;
+    c.raw_out = static_cast<bf16*>(a->y_bf16);
+    const GemmDesc d = conv_desc(c, B, B, PW);
     REQUIRE(B % d.b_box == 0, "batch must be a multiple of %d at this resolution", d.b_box);
-    REQUIRE(Cout >= d.block_n, "Cout smaller than the tile");
-    d.n_tiles = Cout / d.block_n;
-    d.OW = OW; d.OH = OH; d.OB = B; d.n_valid = Cout; d.bias = bias;
-    d.out_f32 = y; d.os = nhwc_out(OH, OW, Cout);
-    d.stats = stats; d.stats_C = Cout;
-    Op op = make_gemm_op(d, mem);
+    Op op = make_gemm_op(d, mem, geometry);
     op(st);
     CK(cudaStreamSynchronize(st));
+    API_END
+}
+
+int sr3_test_conv(const void* x, const float* w_oihw, const float* bias, float* y, double* stats, int B, int H, int W, int Cin, int Cout,
+                  int ksize, int stride, void* stream) {
+    sr3_test_conv_args a;
+    memset(&a, 0, sizeof(a));
+    a.x = x; a.w = w_oihw; a.bias = bias; a.y = y; a.stats = stats;
+    a.B = B; a.H = H; a.W = W; a.Cin = Cin; a.Cout = Cout; a.ksize = ksize; a.stride = stride;
+    return sr3_test_conv_ex(&a, nullptr, stream);
+}
+
+int sr3_test_wgrad(const void* dy, const void* x, float* grad, int B, int OH, int OW, int CY, int Cin, int ksize, int stride, int cout_valid,
+                   int cin_valid, int slices, float gscale, int raw, int* slices_used, void* stream) {
+    API_BEGIN
+    REQUIRE(dy && x && grad, "null argument");
+    REQUIRE(B >= 1 && ((ksize == 1 && stride == 1) || (ksize == 3 && (stride == 1 || stride == 2))), "bad wgrad shape");
+    REQUIRE(cout_valid >= 1 && cout_valid <= CY && cin_valid >= 1 && cin_valid <= Cin, "valid channels %d / %d of %d / %d", cout_valid, cin_valid, CY, Cin);
+    REQUIRE(!raw || (ksize == 1 && slices == 0 && cout_valid == CY && cin_valid == Cin), "batched form: 1x1, one slice per batch, every channel");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    DevAllocs mem;
+    const std::vector<WgradTap> taps = ksize == 1 ? taps_1x1() : (stride == 2 ? taps_3x3_stride2(Cin) : taps_3x3());
+    const int ntaps = (int)taps.size();
+    const ASrc xs = stride == 2 ? nhwc_stride2_src(x, B, 2 * OH, 2 * OW, Cin) : nhwc_src(x, B, OH, OW, Cin);
+    WgradOut ro;
+    if (raw) { ro.ptr = grad; ro.slice_stride = (long long)CY * Cin; ro.row_stride = Cin; ro.nb = B; }
+    const WgradShape s = wgrad_shape(CY, OH, OW, B, Cin, ntaps, slices, raw ? &ro : nullptr);
+    float* ws = raw ? grad : static_cast<float*>(mem.alloc((size_t)s.slices * s.co_pad * ntaps * Cin * sizeof(float), false));
+    const WgradParams p = wgrad_params(s, static_cast<const bf16*>(dy), CY, OH, OW, B, B, xs, Cin, taps, cout_valid, ws, raw ? &ro : nullptr);
+    init_wgrad_attrs();
+    launch_k(wgrad_kernel, dim3(s.nx, s.ny, s.slices), dim3(WGRAD_THREADS), (size_t)WGRAD_SMEM_BYTES, st, p);
+    if (!raw) {
+        WgradReduceDesc rd = wgrad_reduce_desc(s, ws, ntaps, Cin, cout_valid, cin_valid);
+        rd.grad = grad; rd.block_begin = 0; rd.block_end = rd.blocks_x * cout_valid;
+        WgradReduceDesc* tab = static_cast<WgradReduceDesc*>(mem.alloc(sizeof(WgradReduceDesc), false));
+        int* ends = static_cast<int*>(mem.alloc(sizeof(int), false));
+        CK(cudaMemcpyAsync(tab, &rd, sizeof(rd), cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(ends, &rd.block_end, sizeof(int), cudaMemcpyHostToDevice, st));
+        launch_k(wgrad_reduce_kernel, dim3(rd.block_end), dim3(256), 0, st, (const WgradReduceDesc*)tab, (const int*)ends, 0, 1, 0, gscale);
+    }
+    CK(cudaStreamSynchronize(st));           // the partial tiles and the table die with this call
+    if (slices_used) *slices_used = s.slices;
     API_END
 }
 

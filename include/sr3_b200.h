@@ -204,6 +204,36 @@ int sr3_test_attention(const void* qk_bf16, const void* vT_bf16, void* out_bf16,
 int sr3_test_conv(const void* x_bf16, const float* w_oihw, const float* bias, float* y, double* stats, int B, int H, int W, int Cin,
                   int Cout, int ksize, int stride, void* stream);
 
+/* The tile-kernel variant and launch shape one conv actually ran with (after every SR3_* override and host-side cap): tall-halo form,
+ * 128-row halves per tile, BLOCK_N, the tile's pixel box (h_box rows x b_box images), split-K factor, pipeline stages, grid CTAs, output
+ * tiles (times the z phases), and whether the residual was staged through shared memory by TMA (0: plain loads). */
+typedef struct sr3_gemm_geometry {
+    int tall, mh, block_n, h_box, b_box, ksplit, stages, ctas, tiles, res_smem;
+} sr3_gemm_geometry;
+/* One image conv exactly as a UNet layer builds it, every operand on the DEVICE:
+ *   y = conv(x, w) [+ conv1x1(x2, w2)] + bias + bias2[image] + resid,   y fp32 NHWC [B][OH][OW][Cout]
+ * x bf16 NHWC [B][H][W][Cin]; w fp32 OIHW [Cout][Cin][k][k]; optional: bias [Cout], bias2 [B][Cout] (per-image FiLM bias), resid fp32 NHWC
+ * like y, a second A source x2 bf16 NHWC [B][H][W][Cin2] whose 1x1 conv w2 [Cout][Cin2][1][1] is appended as extra K columns (ResnetBlock
+ * block2 + res_conv), y_bf16 = bf16(y) NHWC, stats fp64 [B][Cout][2] zeroed by the caller.
+ * fold_up = 1: the Upsample conv, nearest 2x then conv3x3 (Cin == Cout, stride 1), run as the merged four-phase op on the folded weights;
+ * y is then [B][2H][2W][Cout].  precise = 1: x / x2 rows are [hi | lo] (2 Cin channels: hi = bf16(v), lo = bf16(v - hi)), three tensor-core
+ * passes, y_bf16 rows [hi | lo] of 2 Cout.  geometry (optional) receives the variant that ran. */
+typedef struct sr3_test_conv_args {
+    const void* x; const float* w; const float* bias; const float* bias2; const float* resid;
+    const void* x2; const float* w2;
+    float* y; void* y_bf16; double* stats;
+    int B, H, W, Cin, Cout, Cin2, ksize, stride;
+    int fold_up, precise;
+} sr3_test_conv_args;
+int sr3_test_conv_ex(const sr3_test_conv_args* args, sr3_gemm_geometry* geometry, void* stream);
+/* Weight gradient of one conv through wgrad_kernel + wgrad_reduce_kernel (the training plan's path): dy bf16 NHWC [B][OH][OW][CY], x bf16
+ * NHWC [B][OH*stride][OW*stride][Cin]; k = 1 (stride 1) or 3 (stride 1 or 2, padding 1).  grad fp32 OIHW [cout_valid][cin_valid][k][k] =
+ * gscale * dW over the first cout_valid / cin_valid channels.  slices = 0: the training plan's slice count; *slices_used (optional) reports it.
+ * raw = 1: the batched form of the attention backward (k = 1, every channel): grad [B][CY][Cin], image b alone contracted into slice b, no
+ * reduction and no gscale. */
+int sr3_test_wgrad(const void* dy_bf16, const void* x_bf16, float* grad, int B, int OH, int OW, int CY, int Cin, int ksize, int stride,
+                   int cout_valid, int cin_valid, int slices, float gscale, int raw, int* slices_used, void* stream);
+
 /* Test hook for the GroupNorm path of a Block (unet.py:80-91): y = conv(x) + bias with the statistics taken in the conv epilogue, then
  * a = [silu](GroupNorm(y; groups, gamma, beta, eps 1e-5)) as bf16 NHWC.  Shapes as sr3_test_conv (stride 1). */
 int sr3_test_conv_groupnorm(const void* x_bf16, const float* w_oihw, const float* bias, const float* gamma, const float* beta, int groups,
