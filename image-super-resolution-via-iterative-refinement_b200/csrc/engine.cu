@@ -175,7 +175,6 @@ bool first_use_on_device(std::vector<int>& seen) {
 }
 // Every kernel of the step is launched with programmatic stream serialization (PDL): its prologue overlaps the tail of the
 // previous kernel; the kernels call griddepcontrol.wait before touching upstream data.
-bool use_pdl() { static int v = -1; if (v < 0) v = getenv("SR3_NO_PDL") ? 0 : 1; return v == 1; }
 template <typename... KArgs, typename... Args>
 void launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
     cudaLaunchConfig_t cfg{};
@@ -183,46 +182,27 @@ void launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cuda
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = use_pdl() ? 1 : 0;
+    cfg.attrs = attr; cfg.numAttrs = 1;
     CK(cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...));
 }
 // Split-K layers: the `ksplit` CTAs that share an output tile are consecutive blocks and wait for each other inside the kernel.  They are
 // launched as ONE THREAD-BLOCK CLUSTER (cluster dimension = ksplit): the hardware gang-schedules a cluster, so the partners are co-resident
 // by construction -- no assumption about what else occupies the device (other engines / streams, NCCL, library kernels), inside or outside
-// graph capture, and the launch keeps its programmatic-dependent-launch edge.  SR3_NO_CLUSTER=1: the round-1 form (plain launch inside
-// graphs, cooperative launch outside).
-bool use_cluster_split() { static int v = -1; if (v < 0) v = getenv("SR3_NO_CLUSTER") ? 0 : 1; return v == 1; }
+// graph capture, and the launch keeps its programmatic-dependent-launch edge.
 constexpr int MAX_CLUSTER_SPLIT = 8;               // portable cluster size limit
 template <int BN, int MH>
 void launch_gemm_bn(const GemmParams& p, dim3 grid, int smem, cudaStream_t st) {
-    if (p.ksplit > 1 && use_cluster_split()) {
-        REQUIRE(p.ksplit <= MAX_CLUSTER_SPLIT && grid.x % p.ksplit == 0, "split-K factor %d does not form clusters of grid %u", p.ksplit, grid.x);
-        cudaLaunchConfig_t cfg{};
-        cfg.gridDim = grid; cfg.blockDim = dim3(GEMM_THREADS); cfg.dynamicSmemBytes = (size_t)smem; cfg.stream = st;
-        cudaLaunchAttribute attr[2];
-        attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = (unsigned)p.ksplit; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-        attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        attr[1].val.programmaticStreamSerializationAllowed = 1;
-        cfg.attrs = attr; cfg.numAttrs = use_pdl() ? 2 : 1;
-        CK(cudaLaunchKernelEx(&cfg, gemm_tile_kernel<BN, MH>, p));
-        return;
-    }
-    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-    if (p.ksplit > 1) CK(cudaStreamIsCapturing(st, &cap));
-    if (p.ksplit > 1 && cap == cudaStreamCaptureStatusNone && getenv("SR3_NO_COOP") == nullptr) {
-        // (SR3_NO_CLUSTER) split-K CTAs wait for their partners inside the kernel: launch cooperatively so that the runtime guarantees
-        // co-residency (or fails the launch) even when another stream / engine / library kernel holds SMs.  No PDL overlap for these launches.
-        cudaLaunchConfig_t cfg{};
-        cfg.gridDim = grid; cfg.blockDim = dim3(GEMM_THREADS); cfg.dynamicSmemBytes = (size_t)smem; cfg.stream = st;
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeCooperative;
-        attr[0].val.cooperative = 1;
-        cfg.attrs = attr; cfg.numAttrs = 1;
-        CK(cudaLaunchKernelEx(&cfg, gemm_tile_kernel<BN, MH>, p));
-        return;
-    }
-    launch_k(gemm_tile_kernel<BN, MH>, grid, dim3(GEMM_THREADS), (size_t)smem, st, p);
+    if (p.ksplit == 1) { launch_k(gemm_tile_kernel<BN, MH>, grid, dim3(GEMM_THREADS), (size_t)smem, st, p); return; }
+    REQUIRE(p.ksplit <= MAX_CLUSTER_SPLIT && grid.x % p.ksplit == 0, "split-K factor %d does not form clusters of grid %u", p.ksplit, grid.x);
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = grid; cfg.blockDim = dim3(GEMM_THREADS); cfg.dynamicSmemBytes = (size_t)smem; cfg.stream = st;
+    cudaLaunchAttribute attr[2];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = (unsigned)p.ksplit; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+    attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[1].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr; cfg.numAttrs = 2;
+    CK(cudaLaunchKernelEx(&cfg, gemm_tile_kernel<BN, MH>, p));
 }
 void init_gemm_attrs() {
     static std::vector<int> seen;
@@ -259,13 +239,11 @@ int cluster_capacity(int c) {
         cudaGetLastError();
         n = 8 * ((num_sms() / 8) / c);               // eight GPCs of equal size, conservatively
     }
-    if (const char* e = getenv("SR3_CLUSTER_DEBUG")) { if (atoi(e)) fprintf(stderr, "sr3: cluster_capacity(%d) = %d\n", c, n); }
     cache[key] = n;
     return n;
 }
 // largest split-K factor <= want whose clusters all fit the device together with `tiles` output tiles
 int fit_split(int want, long long tiles) {
-    if (!use_cluster_split()) return want;
     if (want > MAX_CLUSTER_SPLIT) want = MAX_CLUSTER_SPLIT;
     while (want > 1 && cluster_capacity(want) < tiles) --want;
     return want;
@@ -331,7 +309,6 @@ Op make_gemm_op(const GemmDesc& d, DevAllocs& mem, sr3_gemm_geometry* geo = null
     // Generic mode: up to three consecutive K slabs of the same source are grouped into a stage (one box each).
     std::vector<StageDesc> tab;
     int b_taps = 1, a_boxes = 1;
-    const int group_max = getenv("SR3_GROUP") ? atoi(getenv("SR3_GROUP")) : 3;
     for (size_t i = 0; i < d.slabs.size(); ++i) {
         const KSlab& k = d.slabs[i];
         REQUIRE(k.a_sel < d.n_a, "slab refers to missing A source");
@@ -359,7 +336,7 @@ Op make_gemm_op(const GemmDesc& d, DevAllocs& mem, sr3_gemm_geometry* geo = null
         } else {
             e.a_multi = 1;
             int n = 1;
-            while (n < group_max && i + n < d.slabs.size() && d.slabs[i + n].a_sel == k.a_sel) ++n;
+            while (n < 3 && i + n < d.slabs.size() && d.slabs[i + n].a_sel == k.a_sel) ++n;
             e.ntaps = n;
             for (int t = 0; t < n; ++t) {
                 const KSlab& o = d.slabs[i + t];
@@ -387,7 +364,6 @@ Op make_gemm_op(const GemmDesc& d, DevAllocs& mem, sr3_gemm_geometry* geo = null
         p.w_shift = lg(d.w_box); p.h_shift = lg(d.h_box);
     }
     p.a_zstep = d.a_zstep; p.b_zrows = d.b_zrows;
-    p.dbg = getenv("SR3_DBG") ? atoi(getenv("SR3_DBG")) : 0;
     p.n_tiles = d.n_tiles; p.nz = d.nz;
     p.mode = d.mode; p.OW = d.OW; p.OH = d.OH; p.OB = d.OB; p.n_valid = d.n_valid; p.scale = d.scale;
     p.bias = d.bias; p.bias2 = d.bias2; p.bias2_stride = d.bias2_stride;
@@ -400,7 +376,7 @@ Op make_gemm_op(const GemmDesc& d, DevAllocs& mem, sr3_gemm_geometry* geo = null
     p.lo_out_off = d.lo_out_off; p.lo_t_off = d.lo_t_off;
     if (d.stats) REQUIRE((d.w_box * d.h_box) % 32 == 0, "stats need whole warps per image");
     // fp32 output / residual through smem + TMA: one 32-row x 32-column box per epilogue warp
-    p.tma_epi = (d.mode == 0 && getenv("SR3_NO_TMA_EPI") == nullptr && (d.out_f32 || d.resid)) ? 1 : 0;
+    p.tma_epi = (d.mode == 0 && (d.out_f32 || d.resid)) ? 1 : 0;
     if (p.tma_epi) {
         const int w_sub = d.w_box < 32 ? d.w_box : 32, h_sub = 32 / w_sub;
         REQUIRE(d.w_box % w_sub == 0 && (d.h_box % h_sub == 0 || d.h_box == 1) && (h_sub == 1 || (128 / w_sub) % h_sub == 0), "tile box %dx%d cannot be split into per-warp boxes", d.w_box, d.h_box);
@@ -493,7 +469,7 @@ Op make_gemm_op(const GemmDesc& d, DevAllocs& mem, sr3_gemm_geometry* geo = null
 }
 
 // Fused attention core (attn_wgmma.cuh): S = q k^T / sqrt(C), softmax, O = P v in one launch.  qk [nz*Lt][2C], vT [nz*C][Lt], out [nz*Lt][C].
-bool attn_fusable(int Lt, int C) { return getenv("SR3_NO_FUSED_ATTN") == nullptr && (Lt == 128 || Lt == 256) && C % 128 == 0 && C >= 128; }
+bool attn_fusable(int Lt, int C) { return (Lt == 128 || Lt == 256) && C % 128 == 0 && C >= 128; }
 
 Op make_attn_op(const bf16* qk, const bf16* vT, bf16* out, int nz, int Lt, int HW, int C) {
     REQUIRE(attn_fusable(Lt, C) && Lt % HW == 0, "attention shape Lt=%d HW=%d C=%d is not supported by the fused kernel", Lt, HW, C);
@@ -530,15 +506,14 @@ int pick_block_n(int cout);
 // partial-tile store + reload + a grid-level handshake (tools/gpu_splitk_sweep.py sweeps the choices on a device).
 void conv_geometry(GemmDesc& d, int OW, int OH, int Bp, int cout, bool has_resid = false, int nz = 1) {
     const int npass = d.passes > 1 ? d.passes : 1;
-    bool tall_ok = getenv("SR3_NO_TALL") == nullptr && OW >= 8 && OH >= 16, has3 = false;
+    bool tall_ok = OW >= 8 && OH >= 16, has3 = false;
     for (const KSlab& k : d.slabs) { if (k.p != 0) tall_ok = false; if (k.dh != 0) has3 = true; }
     tall_ok = tall_ok && has3 && (OH >= 32 || Bp % 2 == 0);
-    const bool allow_split = getenv("SR3_NO_KSPLIT") == nullptr;
     const int sms = num_sms();
     // cost in bytes of the slowest CTA; `split` returns the factor the cost was computed for
     auto model = [&](long long tiles, int nstage, long long stage_bytes, int rows, int bn, int& split) -> double {
         int smax = 1;
-        if (allow_split && bn >= 32 && cout % 32 == 0) {
+        if (bn >= 32 && cout % 32 == 0) {
             smax = (int)(sms / tiles);
             const int units = (rows / 128) * (bn / 32) * 4;
             if (smax > units) smax = units;
@@ -592,7 +567,7 @@ void conv_geometry(GemmDesc& d, int OW, int OH, int Bp, int cout, bool has_resid
         if (const char* e = getenv("SR3_TALL_BN")) { int v = atoi(e); if ((v == 32 || v == 64 || v == 128) && cout % v == 0) { bn = v; split = 16; } }
         if (const char* e = getenv("SR3_TALL_MH")) { int v = atoi(e); if (v == 1 || v == 2) { mh = v; split = 16; } }
         if (mh == 2 && bn == 32) bn = 64;
-        d.mh = mh; d.block_n = bn; d.ksplit_max = allow_split ? split : 1;
+        d.mh = mh; d.block_n = bn; d.ksplit_max = split;
         geom(mh, d.h_box, d.b_box);
         d.a_box_w = 8; d.a_box_b = d.b_box;
         if (mh == 2 && d.b_box == 1) { d.a_box_h = 34; d.a_half_off = 16 * 1024; }
@@ -722,21 +697,21 @@ GemmDesc conv_desc(const ConvArgs& c, int B, int Bp, int PW) {
 // Upsample folded (nearest 2x -> conv3x3 on a Hl x Wl x C input, bf16 NHWC rows of PW * C at `raw`): output pixel (2i+py, 2j+px) only sees
 // a 2x2 neighbourhood of the low-res input, with the 3x3 taps that alias onto the same low-res pixel summed into one weight
 // (fold_upsample_weight_kernel: exact in real arithmetic, 2.25x fewer MACs, no 4x-sized intermediate).  Fills the A source, K slabs and
-// output addressing of phase `ph` (py = ph / 2, px = ph % 2), each phase writing its quarter of the NHWC output; merge: all four phases in
-// one op (gemm-batch z = phase, weights of phase z start at row z * rows_pad).  The caller sets weights, bias and output.
-void fold_up_conv(ConvArgs& c, const bf16* raw, int Bp, int Hl, int Wl, int C, int PW, int ph, bool merge) {
-    const int py = ph >> 1, px = ph & 1;
+// output addressing of one op that runs all four phases (gemm-batch z = 2 py + px = phase, weights of phase z start at row z * rows_pad),
+// each phase writing its quarter of the NHWC output.  The slabs are those of phase 0; the kernel shifts them by (py, px) for the others.
+// The caller sets weights, bias and output.
+void fold_up_conv(ConvArgs& c, const bf16* raw, int Bp, int Hl, int Wl, int C, int PW) {
     c.n_a = 1; c.a[0] = nhwc_src(raw, Bp, Hl, Wl, C * PW); c.c0 = C;
     for (int a = 0; a < 2; ++a)
         for (int bb = 0; bb < 2; ++bb)
             for (int ch = 0; ch < C; ch += 64) {
-                KSlab k; k.a_sel = 0; k.a_chan = ch; k.dh = py - 1 + a; k.dw = px - 1 + bb; k.p = 0; k.b_col = (a * 2 + bb) * C + ch;
+                KSlab k; k.a_sel = 0; k.a_chan = ch; k.dh = a - 1; k.dw = bb - 1; k.p = 0; k.b_col = (a * 2 + bb) * C + ch;
                 c.slabs.push_back(k);
             }
     c.ktot = 4 * C; c.cout = C; c.OH = Hl; c.OW = Wl;
     c.custom_os = true;
-    c.os.sZ = 0; c.os.sB = 4LL * Hl * Wl * C; c.os.sH = 4LL * Wl * C; c.os.sW = 2LL * C; c.os.off = (long long)py * 2 * Wl * C + (long long)px * C;
-    if (merge) { c.nz = 4; c.b_zrows = ((C + 127) / 128) * 128; c.z_phase = 1; c.z_off_hi = 2LL * Wl * C; c.z_off_lo = C; }
+    c.os.sZ = 0; c.os.sB = 4LL * Hl * Wl * C; c.os.sH = 4LL * Wl * C; c.os.sW = 2LL * C; c.os.off = 0;
+    c.nz = 4; c.b_zrows = ((C + 127) / 128) * 128; c.z_phase = 1; c.z_off_hi = 2LL * Wl * C; c.z_off_lo = C;
 }
 
 // ---- weight gradient (wgrad_kernel + wgrad_reduce_kernel), shared by the training plan and the stand-alone test hook
@@ -778,7 +753,7 @@ WgradShape wgrad_shape(int CY, int OHh, int OWw, int nbatch, int Cin, int ntaps,
         // one wave of CTAs: a CTA's fixed cost (pipeline fill, 96 KB partial tile out) is as long as ~10 K steps of its main loop,
         // and every extra slice is another partial tile for the reduction kernel to read
         const int nxy = s.nx * s.ny;
-        s.slices = getenv("SR3_WGRAD_WAVES") ? (atoi(getenv("SR3_WGRAD_WAVES")) * num_sms() + nxy - 1) / nxy : (num_sms() + nxy / 2) / nxy;
+        s.slices = (num_sms() + nxy / 2) / nxy;
         if (s.slices > s.patches / 2) s.slices = s.patches / 2;
         if (s.slices < 1) s.slices = 1;
     }
@@ -885,7 +860,6 @@ struct sr3_engine {
     cudaStream_t side_stream = nullptr;            // graph capture only: the noise-level embedding + FiLM projections run beside the first conv
     cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
     int side_begin = -1, side_end = -1, side_join = -1;   // ops [side_begin, side_end) on the side branch, joined before op side_join
-    bool use_graph = true;
     uint64_t seed = 0, first_index = 0;
     bool have_cond = false;
 
@@ -1028,10 +1002,10 @@ struct sr3_engine {
         const int threads = vpp * kpix;                                // <= 512, every thread owns one 4-channel column
         // ONE wave of blocks: the kernel uses 64 registers per thread, i.e. 4 resident 256-thread blocks (2 of 512) per SM; a grid sized
         // for 8 per SM (round 1, 32-register version) runs as two waves and pays the statistics set-up twice (24 vs 15 us on the 128x128
-        // level).  SR3_PREP_SLOTS overrides the number of resident blocks per SM assumed here.
+        // level).
         int ppb;
         {
-            const int per_sm = getenv("SR3_PREP_SLOTS") ? atoi(getenv("SR3_PREP_SLOTS")) : (threads > 256 ? 2 : 4);
+            const int per_sm = threads > 256 ? 2 : 4;
             int bpi = per_sm * num_sms() / B; if (bpi < 1) bpi = 1;    // blocks per image
             const int q = kpix * 4;                                    // 4 loads in flight per thread
             ppb = (p.HW + bpi - 1) / bpi;
@@ -1180,28 +1154,17 @@ struct sr3_engine {
             if (train) { AttnBwdCtx c; c.p = p; c.x = x; c.y = y; c.C = C; c.Hh = Hh; c.Ww = Ww; c.Lt = Lt; c.per = per; c.nz = nz; c.n = n; c.qk = qk; c.vT = vT; c.P = P; c.O = O; c.gn_w = gn_w; c.gn_b = gn_b; c.mr = mr_attn; bwd_attention(c); }
             return y;
         }
-        const bool merged_qkv = (getenv("SR3_NO_MERGED_QKV") == nullptr || precise) && C % 128 == 0;     // whole 128-column tiles on either side of 2C
-        {   // q,k (,v) = Wqkv n : [Bp*HW tokens] x [2C (3C)]; the v columns are stored transposed as vT[z][d][token]
+        {   // q,k,v = Wqkv n : [Bp*HW tokens] x [3C]; the v columns (whole 128-column tiles: C % 128 == 0) are stored transposed as vT[z][d][token]
             GemmDesc d; d.n_a = 1; d.a[0] = nhwc_src(n, Bp, Hh, Ww, C * PW);
             add_conv_slabs(d.slabs, 0, C, 1, 1, 0);
             set_precise(d, C, 0, C);
-            const int ncol = merged_qkv ? 3 * C : 2 * C;
+            const int ncol = 3 * C;
             d.block_n = 128; d.b_ptr = wqkv; d.b_K = C * PW; d.b_rows = ncol; d.b_is_param = true;
             pick_image_box(Ww, Hh, d.w_box, d.h_box, d.b_box);
             d.tiles_w = Ww / d.w_box; d.tiles_h = Hh / d.h_box; d.tiles_b = Bp / d.b_box; d.n_tiles = ncol / 128;
             d.OW = Ww; d.OH = Hh; d.OB = Bp; d.n_valid = ncol;
             d.out_bf16 = qk; d.hs = nhwc_out(Hh, Ww, 2 * C * PW); d.lo_out_off = precise ? 2 * C : 0;      // rows [q_hi | k_hi | q_lo | k_lo]
-            if (merged_qkv) { d.out_t = vT; d.t_col0 = 2 * C; d.t_rows = C; d.t_ld = Lt * PW; d.t_per = per; d.lo_t_off = precise ? Lt : 0; }
-            push_gemm(d);
-        }
-        if (!merged_qkv) {   // vT[z][d][token] = Wv[d,:] . n[token,:]  (weights are the A operand, tokens the B operand)
-            GemmDesc d; d.n_a = 1; d.a[0] = matrix_src(wqkv + (size_t)2 * C * C, 1, C, C, C, 0);
-            for (int c = 0; c < C; c += 64) d.slabs.push_back({0, c, 0, 0, 0, c});
-            d.block_n = 128; d.b_ptr = n; d.b_K = C; d.b_rows = (long long)Bp * HW;
-            d.w_box = 128; d.h_box = 1; d.b_box = 1; d.tiles_w = C / 128; d.tiles_h = 1; d.tiles_b = 1;
-            d.n_tiles = Lt / 128; d.nz = nz; d.a_zstep = 0; d.b_zrows = Lt;
-            d.OW = C; d.OH = 1; d.OB = 1; d.n_valid = Lt;
-            d.out_bf16 = vT; d.hs = OutSpec{(long long)C * Lt, 0, 0, Lt, 0};
+            d.out_t = vT; d.t_col0 = 2 * C; d.t_rows = C; d.t_ld = Lt * PW; d.t_per = per; d.lo_t_off = precise ? Lt : 0;
             push_gemm(d);
         }
         if (attn_fusable(Lt, C) && !precise && !train) {
@@ -1333,8 +1296,7 @@ struct sr3_engine {
         int film_off = 0;
         std::vector<Act> feats;
         Act x;
-        const bool fuse_cast = getenv("SR3_NO_FUSE_CAST") == nullptr;     // producers also emit the bf16 copy Down / Upsample convs read
-        const bool fold_up = getenv("SR3_NO_FOLD_UP") == nullptr;         // nearest-2x + conv3x3 as four 2x2-tap phase convs on the low-res input
+        // the res block in front of a Down / Upsample also emits the bf16 copy ("xraw") that conv reads
         for (size_t li = 0; li < downs.size(); ++li) {
             auto& L = downs[li];
             const bool next_is_down = li + 1 < downs.size() && downs[li + 1].kind == 2;
@@ -1350,7 +1312,7 @@ struct sr3_engine {
                 if (train) bwd_first_conv(L.name, x);
                 if (!dry) side_join = (int)ops.size();      // the FiLM biases are first read by the next block's conv1 epilogue
             } else if (L.kind == 1) {
-                bf16* xr = (fuse_cast && next_is_down) ? static_cast<bf16*>(role("xraw", (size_t)Bp * x.H * x.W * L.cout * 2 * PW)) : nullptr;
+                bf16* xr = next_is_down ? static_cast<bf16*>(role("xraw", (size_t)Bp * x.H * x.W * L.cout * 2 * PW)) : nullptr;
                 last_xraw = xr;
                 x = add_res_block(L, x, nullptr, film_off, xr, /*x_has_skip=*/true);
             } else {                    // Downsample: conv3x3 stride 2 on the raw stream (unet.py:68-74)
@@ -1358,8 +1320,7 @@ struct sr3_engine {
                 bf16* w = new_weight(C, 9 * C, pick_block_n(C));
                 conv_weight_param(L.name + ".conv.weight", w, C, C, 3, 9 * C, 0, C);
                 float* b = f32_param(L.name + ".conv.bias", {C});
-                bf16* raw = (train && fuse_cast) ? last_xraw : static_cast<bf16*>(role(fuse_cast ? "xraw" : "raw", (size_t)Bp * x.H * x.W * C * 2 * PW));
-                if (!fuse_cast) add_cast(x, raw, 1);
+                bf16* raw = train ? last_xraw : static_cast<bf16*>(role("xraw", (size_t)Bp * x.H * x.W * C * 2 * PW));
                 Act y = new_act(C, x.H / 2, x.W / 2, L.name);
                 ConvArgs c; c.n_a = 1; c.a[0] = nhwc_stride2_src(raw, Bp, x.H, x.W, C * PW); c.c0 = C;
                 add_conv_slabs(c.slabs, 0, C, 3, 2, 0, C * PW);
@@ -1376,27 +1337,13 @@ struct sr3_engine {
             const bool next_is_up = li + 1 < ups.size() && ups[li + 1].kind == 3;
             if (L.kind == 1) {
                 Act skip = feats.back(); feats.pop_back();
-                bf16* xr = (fuse_cast && fold_up && next_is_up) ? static_cast<bf16*>(role("xraw", (size_t)Bp * x.H * x.W * L.cout * 2 * PW)) : nullptr;
+                bf16* xr = next_is_up ? static_cast<bf16*>(role("xraw", (size_t)Bp * x.H * x.W * L.cout * 2 * PW)) : nullptr;
                 last_xraw = xr;
                 x = add_res_block(L, x, &skip, film_off, xr);
-            } else if (!fold_up) {      // Upsample: nearest 2x then conv3x3 (unet.py:58-65), materialised
-                const int C = x.C;
-                bf16* w = new_weight(C, 9 * C, pick_block_n(C));
-                conv_weight_param(L.name + ".conv.weight", w, C, C, 3, 9 * C, 0, C);
-                float* b = f32_param(L.name + ".conv.bias", {C});
-                bf16* upb = static_cast<bf16*>(role("raw", (size_t)Bp * x.H * 2 * x.W * 2 * C * 2));
-                add_cast(x, upb, 2);
-                Act y = new_act(C, x.H * 2, x.W * 2, L.name);
-                ConvArgs c; c.n_a = 1; c.a[0] = nhwc_src(upb, Bp, y.H, y.W, C);
-                add_conv_slabs(c.slabs, 0, C, 3, 1, 0);
-                c.w = w; c.ktot = 9 * C; c.cout = C; c.OH = y.H; c.OW = y.W; c.bias = b; c.out = y;
-                add_conv(c);
-                x = y;
             } else {
-                // Upsample folded onto the low-res input (fold_up_conv)
+                // Upsample (nearest 2x then conv3x3, unet.py:58-65) folded onto the low-res input (fold_up_conv)
                 const int C = x.C, Hl = x.H, Wl = x.W;
                 const int rows_pad = ((C + 127) / 128) * 128;
-                const bool merge = getenv("SR3_NO_MERGE_UP") == nullptr;        // all four phases in one launch / op (gemm-batch z = phase)
                 bf16* wf[4];
                 if (dry) { for (int ph = 0; ph < 4; ++ph) wf[ph] = nullptr; }
                 else {
@@ -1414,20 +1361,17 @@ struct sr3_engine {
                     { PackDesc d{}; d.type = 5; d.dst = w0; d.Cout = C; d.Cin = C; d.ld = ldw; d.n = (long long)rows_pad * 4 * C * PW; add_pack(L.name + ".conv.weight", d); }
                 }
                 float* b = f32_param(L.name + ".conv.bias", {C});
-                bf16* raw = (train && fuse_cast) ? last_xraw : static_cast<bf16*>(role(fuse_cast ? "xraw" : "raw", (size_t)Bp * Hl * Wl * C * 2 * PW));
-                if (!fuse_cast) add_cast(x, raw, 1);
+                bf16* raw = train ? last_xraw : static_cast<bf16*>(role("xraw", (size_t)Bp * Hl * Wl * C * 2 * PW));
                 bf16* upb = nullptr;
                 if (train) {      // the weight gradient contracts dY with the nearest-2x upsampled input: keep a bf16 copy of it
                     upb = static_cast<bf16*>(role("up_x", (size_t)Bp * Hl * 2 * Wl * 2 * C * 2));
                     add_cast(x, upb, 2);
                 }
                 Act y = new_act(C, Hl * 2, Wl * 2, L.name);
-                for (int ph = 0; ph < (merge ? 1 : 4); ++ph) {
-                    ConvArgs c;
-                    fold_up_conv(c, raw, Bp, Hl, Wl, C, PW, ph, merge);
-                    c.w = wf[ph]; c.bias = b; c.out = y;
-                    add_conv(c);
-                }
+                ConvArgs c;
+                fold_up_conv(c, raw, Bp, Hl, Wl, C, PW);
+                c.w = wf[0]; c.bias = b; c.out = y;
+                add_conv(c);
                 if (train) bwd_upsample(L.name, x, y, upb);
                 x = y;
             }
@@ -1479,7 +1423,6 @@ struct sr3_engine {
         precise = cfg.precision == 1; PW = precise ? 2 : 1;
         cond_c = cfg.conditional ? cfg.in_channel - cfg.channels : 0;
         Bp = (B + 1) & ~1;                         // 8x8 levels tile two images per CTA
-        use_graph = getenv("SR3_NO_GRAPH") == nullptr;
         T_cap = 4096;
         REQUIRE(!(train && precise), "the training plan supports the bf16 precision only");
         // pass 1: sizes
@@ -1511,7 +1454,7 @@ struct sr3_engine {
         try { build_plan(); } catch (...) { g_gemm_registry = nullptr; g_mega_registry = nullptr; throw; }
         g_gemm_registry = nullptr;
         g_mega_registry = nullptr;
-        if (getenv("SR3_NO_PREFETCH") == nullptr && !train) {
+        if (!train) {
             // every tile kernel pulls the weights of the next one into L2 (the last one those of the next step's first)
             for (size_t i = 0; i < gemms.size(); ++i) {
                 const GemmHandle& nx = gemms[(i + 1) % gemms.size()];
@@ -1531,7 +1474,7 @@ struct sr3_engine {
         // Off by default: the grid barrier + per-op fill / drain cost about as much as a launch inside a CUDA graph, and the 288-thread
         // GroupNorm apply has less bandwidth than the stand-alone kernel.
         // SR3_MEGA=1 selects it (bit-identical results).
-        use_mega = !train && getenv("SR3_MEGA") != nullptr && atoi(getenv("SR3_MEGA")) != 0 && getenv("SR3_NO_FUSE_CAST") == nullptr && getenv("SR3_NO_FOLD_UP") == nullptr;
+        use_mega = !train && getenv("SR3_MEGA") != nullptr && atoi(getenv("SR3_MEGA")) != 0;
         if (!use_mega) return;
         std::vector<MegaOp> host_ops;
         std::vector<uint8_t> blob;
@@ -1577,16 +1520,15 @@ struct sr3_engine {
         cudaLaunchAttribute attr[1];
         attr[0].id = cudaLaunchAttributeCooperative;            // all CTAs co-resident: the grid barriers (and split-K meets) cannot deadlock
         attr[0].val.cooperative = 1;
-        cfg.attrs = attr; cfg.numAttrs = getenv("SR3_NO_COOP") ? 0 : 1;
+        cfg.attrs = attr; cfg.numAttrs = 1;
         CK(cudaLaunchKernelEx(&cfg, step_kernel, mp));
     }
 
     void run_step(cudaStream_t st) {
         if (use_mega) { launch_mega(st); return; }
-        if (!use_graph) { for (auto& op : ops) op(st); return; }
         if (!graph) {
             cudaGraph_t g;
-            const bool fork = getenv("SR3_NO_FORK") == nullptr && side_begin > 0 && side_end > side_begin && side_join >= side_end;
+            const bool fork = side_begin > 0 && side_end > side_begin && side_join >= side_end;
             if (fork && !side_stream) {
                 CK(cudaStreamCreateWithFlags(&side_stream, cudaStreamNonBlocking));
                 CK(cudaEventCreateWithFlags(&ev_fork, cudaEventDisableTiming));
@@ -1808,7 +1750,7 @@ int sr3_engine_load_all_params(sr3_engine* e, const float* const* srcs, int n, v
     CK(cudaSetDevice(e->dev));
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     for (int i = 0; i < n; ++i) REQUIRE(srcs[i] != nullptr, "null pointer for %s", e->params[i].name.c_str());
-    if (!e->pack_descs.empty() && !e->precise && getenv("SR3_NO_PACK_TABLE") == nullptr) {
+    if (!e->pack_descs.empty() && !e->precise) {
         // one launch over the descriptor table (rebuilt only when a parameter moved)
         const size_t nd = e->pack_descs.size();
         if (e->pack_last_ptrs.size() != (size_t)n || memcmp(e->pack_last_ptrs.data(), srcs, n * sizeof(float*)) != 0 || !e->pack_dev) {
@@ -2208,7 +2150,7 @@ int sr3_test_conv_ex(const sr3_test_conv_args* a, sr3_gemm_geometry* geometry, v
     const int rows_pad = ((Cout + 127) / 128) * 128;
     ConvArgs c;
     if (a->fold_up) {
-        fold_up_conv(c, static_cast<const bf16*>(a->x), B, H, W, Cin, PW, 0, true);
+        fold_up_conv(c, static_cast<const bf16*>(a->x), B, H, W, Cin, PW);
         const int ldw = PW * c.ktot;
         bf16* wall = static_cast<bf16*>(mem.alloc((size_t)4 * rows_pad * ldw * sizeof(bf16)));     // [phase][rows_pad][PW * 4C]
         const long long phase = (long long)rows_pad * ldw;

@@ -98,8 +98,6 @@ struct GemmParams {
     unsigned int* counters;  // [tiles] arrival counters (monotonic: +ksplit per launch)
     const void* pf_ptr;      // weights of the NEXT tile-kernel launch: pulled into L2 while this launch runs (they would otherwise be
     long long pf_bytes;      // first-touch HBM reads on the critical path of every pipeline stage of that launch)
-    int dbg;                 // SR3_DBG bit mask (timing experiments only): 1 skip epilogue body, 2 skip stats, 4 skip out store,
-                             // 8 skip A loads, 16 skip B loads, 32 skip MMAs
     int w_box, h_box, b_box; // pixel patch of one tile: w_box * h_box * b_box == MH * 128 (all powers of two)
     int w_shift, h_shift;    // log2(w_box), log2(h_box): the epilogue splits a tile row into (w, h, image) with shifts, not divisions
     int a_zstep, b_zrows;
@@ -416,16 +414,12 @@ __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmPa
                     const int a_lo = (pass == 2) ? p.lo_a_chan[e.a_sel] : 0, b_lo = (pass == 1) ? p.lo_b_col : 0;
                     const uint32_t a_dst = stage_base + s * stage_bytes;
                     const int na = e.a_multi ? e.ntaps : 1;
-                    mbar_arrive_expect_tx(full_bar(s), ((p.dbg & 8) ? 0 : na * p.a_box_bytes) + ((p.dbg & 16) ? 0 : e.ntaps * B_BYTES));
-                    if (!(p.dbg & 8)) {
-                        for (int t = 0; t < na; ++t)
-                            tma_load_5d(a_dst + (e.a_multi ? e.tap[t].a_off : 0), &pm->a_map[e.a_sel], full_bar(s), e.tap[t].a_chan + a_lo, w0 + e.tap[t].dw + zdw, e.tap[t].p,
-                                        h0 + e.tap[t].dh + (e.a_multi ? zdh : 0), b0);     // tall halo boxes always start one row above the tile
-                    }
-                    if (!(p.dbg & 16)) {
-                        for (int t = 0; t < e.ntaps; ++t)
-                            tma_load_2d(a_dst + p.a_stage_bytes + t * B_BYTES, &pm->b_map, full_bar(s), e.tap[t].b_col + b_lo, brow);
-                    }
+                    mbar_arrive_expect_tx(full_bar(s), na * p.a_box_bytes + e.ntaps * B_BYTES);
+                    for (int t = 0; t < na; ++t)
+                        tma_load_5d(a_dst + (e.a_multi ? e.tap[t].a_off : 0), &pm->a_map[e.a_sel], full_bar(s), e.tap[t].a_chan + a_lo, w0 + e.tap[t].dw + zdw, e.tap[t].p,
+                                    h0 + e.tap[t].dh + (e.a_multi ? zdh : 0), b0);     // tall halo boxes always start one row above the tile
+                    for (int t = 0; t < e.ntaps; ++t)
+                        tma_load_2d(a_dst + p.a_stage_bytes + t * B_BYTES, &pm->b_map, full_bar(s), e.tap[t].b_col + b_lo, brow);
                 }
                 __syncwarp();
                 if (++s == stages) { s = 0; ph ^= 1u; }
@@ -547,18 +541,16 @@ __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmPa
                     mbar_wait(full_bar(s), ph, 2);
                     const StageDesc& e = ktab_s[k % p.num_k];
                     wgmma_fence();
-                    if (!(p.dbg & 32)) {
-                        for (int t = 0; t < e.ntaps; ++t) {
-                            const uint32_t a_addr = a_base + s * stage_bytes + e.tap[t].a_off + (e.a_multi ? 0 : zrow_off);
-                            const uint32_t b_addr = b_base + s * stage_bytes + t * B_BYTES;
+                    for (int t = 0; t < e.ntaps; ++t) {
+                        const uint32_t a_addr = a_base + s * stage_bytes + e.tap[t].a_off + (e.a_multi ? 0 : zrow_off);
+                        const uint32_t b_addr = b_base + s * stage_bytes + t * B_BYTES;
 #pragma unroll
-                            for (int kk = 0; kk < 4; ++kk) {   // 4 x K(16) = 64 channels; +32 B inside the 128 B swizzle row
-                                const uint64_t bdesc = wgmma_desc_sw128(b_addr + kk * 32, 16, 1024);
+                        for (int kk = 0; kk < 4; ++kk) {   // 4 x K(16) = 64 channels; +32 B inside the 128 B swizzle row
+                            const uint64_t bdesc = wgmma_desc_sw128(b_addr + kk * 32, 16, 1024);
 #pragma unroll
-                                for (int i = 0; i < 2; ++i)    // row groups 2 g' + i, g' = 0..7
-                                    Wgmma<WN>::template mma<0, 0>(acc[i], wgmma_desc_sw128(a_addr + i * 1024 + kk * 32, 16, 2048), bdesc,
-                                                                  ((k - k0) | t | kk) != 0);
-                            }
+                            for (int i = 0; i < 2; ++i)    // row groups 2 g' + i, g' = 0..7
+                                Wgmma<WN>::template mma<0, 0>(acc[i], wgmma_desc_sw128(a_addr + i * 1024 + kk * 32, 16, 2048), bdesc,
+                                                              ((k - k0) | t | kk) != 0);
                         }
                     }
                     wgmma_commit();
@@ -633,7 +625,7 @@ __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmPa
                 const int bb = row >> (p.w_shift + p.h_shift);
                 const int ow = w0 + w, oh = h0 + h, img = b0 + bb;
                 const bool row_ok = (ow < p.OW) && (oh < p.OH) && (img < p.OB);
-                if (p.stats && !(p.dbg & 2) && !to_ws) {
+                if (p.stats && !to_ws) {
                     const int img0 = __shfl_sync(0xffffffffu, img, 0);      // all rows of a warp belong to one image
                     if (img0 != st_img || n0 != st_n0) { flush_stats(); st_img = img0; st_n0 = n0; }
                 }
@@ -706,15 +698,6 @@ __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmPa
                         for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(acc_f[j]);
                     }
                     const float ep_scale = p.scale;
-                    if (p.dbg & 1) {
-                        if (use_res_tma) {
-                            const uint32_t b = (res_count - 1) & 1;
-                            mbar_wait(res_bar(ew, b), (res_phase >> b) & 1u, 5);
-                            res_phase ^= (1u << b);
-                            __syncwarp();
-                        }
-                        continue;
-                    }
                     float f[32];
                     const bool full = (nb + 32 <= p.n_valid);
 #pragma unroll
@@ -745,8 +728,7 @@ __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmPa
                         for (int j = 0; j < 32; ++j)
                             if (nb + j < p.n_valid) f[j] += __ldcg(&p.resid[ro + nb + j]);
                     }
-                    if (p.dbg & 4) {
-                    } else if (use_out_tma) {
+                    if (use_out_tma) {
                         if (out_pending) {                       // the previous bulk store must have finished reading the staging buffer
                             if (lane == 0) tma_store_wait_read<0>();
                             __syncwarp();
@@ -826,9 +808,11 @@ __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmPa
                             }
                         }
                     }
-                    if (p.stats && !(p.dbg & 2)) {
+                    // `!to_ws` always holds here (a split partial tile took the `continue` above); stating it saves ptxas one spilled
+                    // register in gemm_tile_kernel<64, 1>
+                    if (p.stats && !to_ws) {
                         double cs, cq;
-                        if (use_out_tma && !(p.dbg & 4)) {
+                        if (use_out_tma) {
                             // the 32x32 tile sits in the (swizzled) staging buffer: lane c walks down column c -- conflict free, and a
                             // third of the instructions of the shuffle transposition below
                             const unsigned int okm = __ballot_sync(0xffffffffu, row_ok);
@@ -879,7 +863,7 @@ __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmPa
             }       // items
             }       // pass
         }           // tiles
-        if (p.stats && !(p.dbg & 2)) flush_stats();
+        if (p.stats) flush_stats();
         if constexpr (MEGA) {
             // the consumer is a later op of the SAME launch (other CTAs, after a grid barrier): the bulk stores must be complete in
             // global memory, not merely done reading shared memory

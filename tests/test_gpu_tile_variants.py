@@ -18,7 +18,7 @@ import torch.nn.functional as F
 
 pytestmark = pytest.mark.gpu
 
-TALL_ENV = ("SR3_TALL_BN", "SR3_TALL_MH", "SR3_BLOCK_N", "SR3_NO_TALL", "SR3_KSPLIT", "SR3_STAGES", "SR3_MAX_CTAS")
+TALL_ENV = ("SR3_TALL_BN", "SR3_TALL_MH", "SR3_BLOCK_N", "SR3_KSPLIT", "SR3_STAGES", "SR3_MAX_CTAS")
 REPORTS = {}          # case id -> (intended cell, reported geometry)
 
 

@@ -7,7 +7,7 @@ torch.zeros(1).cuda()
 SHAPES = {"8x8 512 B16": (16, 8, 8, 512, 512), "8x8 1024 B16": (16, 8, 8, 1024, 512), "8x8 512 B2": (2, 8, 8, 512, 512), "8x8 1024 B2": (2, 8, 8, 1024, 512),
           "16x16 512 B16": (16, 16, 16, 512, 512), "16x16 1024 B16": (16, 16, 16, 1024, 512), "32x32 256 B4": (4, 32, 32, 256, 256), "64x64 128 B2": (2, 64, 64, 128, 128),
           "16x16 512 B2": (2, 16, 16, 512, 512), "16x16 1024 B2": (2, 16, 16, 1024, 512), "16x16 512 B4": (4, 16, 16, 512, 512)}
-KEYS = ("SR3_NO_KSPLIT", "SR3_DBG", "SR3_KSPLIT", "SR3_BLOCK_N", "SR3_NO_TALL", "SR3_TALL_BN", "SR3_TALL_MH", "SR3_GROUP")
+KEYS = ("SR3_KSPLIT", "SR3_BLOCK_N", "SR3_TALL_BN", "SR3_TALL_MH")
 def run(tag, shape, env=None, **kw):
     for k in KEYS:
         os.environ.pop(k, None)
@@ -24,12 +24,12 @@ def run(tag, shape, env=None, **kw):
 for shape in SHAPES:
     run("model (default)", shape)
     run("model, resid", shape, resid=True)
-    run("no split-K", shape, {"SR3_NO_KSPLIT": 1})
-    run("no split-K, resid", shape, {"SR3_NO_KSPLIT": 1}, resid=True)
+    run("no split-K", shape, {"SR3_KSPLIT": 1})
+    run("no split-K, resid", shape, {"SR3_KSPLIT": 1}, resid=True)
     if shape.startswith("8x8"):
         for bn in (128, 64, 32):
             run(f"BN{bn} split<=16", shape, {"SR3_BLOCK_N": bn, "SR3_KSPLIT": 16})
     else:
         for mh, bn in ((2, 128), (2, 64), (1, 64), (1, 32)):
             run(f"tall {mh*128}x{bn} split<=16", shape, {"SR3_TALL_MH": mh, "SR3_TALL_BN": bn})
-            run(f"tall {mh*128}x{bn} no split", shape, {"SR3_TALL_MH": mh, "SR3_TALL_BN": bn, "SR3_NO_KSPLIT": 1})
+            run(f"tall {mh*128}x{bn} no split", shape, {"SR3_TALL_MH": mh, "SR3_TALL_BN": bn, "SR3_KSPLIT": 1})
