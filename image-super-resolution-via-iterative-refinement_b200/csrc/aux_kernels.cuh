@@ -1,6 +1,6 @@
 // Bandwidth-bound helper kernels of the SR3 step (everything that is not a tensor-core tile):
 // GroupNorm apply (+SiLU) with channel concat, fp32->bf16 cast / nearest 2x upsample, row softmax,
-// noise-level embedding MLP + FiLM projections, weight packing, layout conversion at the API boundary.
+// noise-level embedding MLP + FiLM projections, layout conversion at the API boundary.  (Weight packing: pack_entry, train_kernels.cuh.)
 #pragma once
 #include "gemm_wgmma.cuh"
 
@@ -328,60 +328,6 @@ __global__ void __launch_bounds__(256) film_kernel(const float* __restrict__ wf,
         for (int i = 0; i < inner; ++i) a += w[i] * t[i];
         film[static_cast<long long>(b) * F + j] = a;
     }
-}
-
-// OIHW fp32 conv weight -> K-major bf16 GEMM operand: dst[o][k_off + (r*KW+s)*cin_pad + c]
-// precise mode (lo_off != 0): the row is [hi (ktot) | lo (ktot)], lo_off = ktot; `ld` = row length in elements.
-// One thread per (o, c): it reads the KH*KW contiguous taps of that pair (the warp reads one contiguous span) and writes tap by tap (for a
-// fixed tap the warp's c are contiguous in dst): both sides coalesced.  Runs after every optimizer step of the training loop.
-__global__ void __launch_bounds__(256) pack_conv_weight_kernel(const float* __restrict__ src, __nv_bfloat16* __restrict__ dst, int Cout, int Cin,
-                                                               int KH, int KW, int ld, int k_off, int cin_pad, int lo_off) {
-    const long long total = static_cast<long long>(Cout) * Cin;
-    const int taps = KH * KW;
-    for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
-         i += static_cast<long long>(gridDim.x) * blockDim.x) {
-        const int c = static_cast<int>(i % Cin);
-        const int o = static_cast<int>(i / Cin);
-        const float* sp = src + i * taps;
-        for (int t = 0; t < taps; ++t) {
-            const float v = sp[t];
-            const long long di = static_cast<long long>(o) * ld + k_off + t * cin_pad + c;
-            dst[di] = __float2bfloat16_rn(v);
-            if (lo_off) dst[di + lo_off] = __float2bfloat16_rn(bf16_residual(v));
-        }
-    }
-}
-
-// Weights of the four phase convs of a folded (nearest-2x -> conv3x3): for output parity py the kernel rows that land on low-res
-// row offset a are R(0,0)={0}, R(0,1)={1,2}, R(1,0)={0,1}, R(1,1)={2} (same for columns); summed in fp32, rounded once to bf16.
-// dst[phase][o][(a*2+b)*Cin + c]
-__global__ void __launch_bounds__(256) fold_upsample_weight_kernel(const float* __restrict__ src, __nv_bfloat16* __restrict__ d0,
-                                                                   __nv_bfloat16* __restrict__ d1, __nv_bfloat16* __restrict__ d2,
-                                                                   __nv_bfloat16* __restrict__ d3, int Cout, int Cin, int ld, int lo_off) {
-    const long long total = 4LL * Cout * Cin * 4;
-    for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
-         i += static_cast<long long>(gridDim.x) * blockDim.x) {
-        long long r = i;
-        const int c = static_cast<int>(r % Cin); r /= Cin;
-        const int ab = static_cast<int>(r % 4); r /= 4;
-        const int o = static_cast<int>(r % Cout);
-        const int ph = static_cast<int>(r / Cout);
-        const int py = ph >> 1, px = ph & 1, a = ab >> 1, b = ab & 1;
-        const int r0 = (py == 0) ? (a == 0 ? 0 : 1) : (a == 0 ? 0 : 2), r1 = (py == 0) ? (a == 0 ? 0 : 2) : (a == 0 ? 1 : 2);
-        const int s0 = (px == 0) ? (b == 0 ? 0 : 1) : (b == 0 ? 0 : 2), s1 = (px == 0) ? (b == 0 ? 0 : 2) : (b == 0 ? 1 : 2);
-        float acc = 0.f;
-        for (int rr = r0; rr <= r1; ++rr)
-            for (int ss = s0; ss <= s1; ++ss) acc += src[((static_cast<long long>(o) * Cin + c) * 3 + rr) * 3 + ss];
-        __nv_bfloat16* d = ph == 0 ? d0 : (ph == 1 ? d1 : (ph == 2 ? d2 : d3));
-        const long long di = static_cast<long long>(o) * ld + ab * Cin + c;
-        d[di] = __float2bfloat16_rn(acc);
-        if (lo_off) d[di + lo_off] = __float2bfloat16_rn(bf16_residual(acc));
-    }
-}
-
-__global__ void add_vec_kernel(const float* a, const float* b, float* out, int n) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) out[i] = a[i] + (b ? b[i] : 0.f);
 }
 
 // API boundary: NCHW fp32 (reference layout) -> bf16 NHWC channel slice of the UNet input buffer (+ optional fp32 NCHW copy).

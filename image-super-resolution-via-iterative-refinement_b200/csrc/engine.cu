@@ -642,8 +642,6 @@ struct ParamEntry {
     std::string name;
     std::vector<int64_t> shape;
     int64_t numel = 0;
-    std::function<void(const float*, cudaStream_t)> load;
-    std::vector<std::function<void(const float*, cudaStream_t)>> hooks;   // training plan: further packed copies of the same tensor (data-gradient weights)
     bool loaded = false;
 };
 
@@ -696,7 +694,7 @@ GemmDesc conv_desc(const ConvArgs& c, int B, int Bp, int PW) {
 
 // Upsample folded (nearest 2x -> conv3x3 on a Hl x Wl x C input, bf16 NHWC rows of PW * C at `raw`): output pixel (2i+py, 2j+px) only sees
 // a 2x2 neighbourhood of the low-res input, with the 3x3 taps that alias onto the same low-res pixel summed into one weight
-// (fold_upsample_weight_kernel: exact in real arithmetic, 2.25x fewer MACs, no 4x-sized intermediate).  Fills the A source, K slabs and
+// (pack_entry type 5: exact in real arithmetic, 2.25x fewer MACs, no 4x-sized intermediate).  Fills the A source, K slabs and
 // output addressing of one op that runs all four phases (gemm-batch z = 2 py + px = phase, weights of phase z start at row z * rows_pad),
 // each phase writing its quarter of the NHWC output.  The slabs are those of phase 0; the kernel shifts them by (py, px) for the others.
 // The caller sets weights, bias and output.
@@ -791,6 +789,11 @@ WgradReduceDesc wgrad_reduce_desc(const WgradShape& s, const float* ws, int ntap
     rd.cin_valid = cin_valid; rd.sw = sw; rd.blocks_x = (cin_valid + ci_per_block - 1) / ci_per_block;
     return rd;
 }
+// one packed copy (pack_entry) as its own launch: loading a single parameter, sr3_test_conv_ex
+void pack_one(const PackDesc& d, cudaStream_t st) {
+    pack_one_kernel<<<pack_entry_blocks(d), 256, 0, st>>>(d);
+    CK(cudaGetLastError());
+}
 void init_wgrad_attrs() {
     static std::vector<int> seen;
     if (first_use_on_device(seen)) CK(cudaFuncSetAttribute(wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WGRAD_SMEM_BYTES));
@@ -806,7 +809,7 @@ struct sr3_engine {
     DevAllocs mem;
     std::vector<ParamEntry> params;
     std::map<std::string, int> pindex;
-    std::vector<Op> ops, finalize_ops;
+    std::vector<Op> ops;
     std::vector<GemmHandle> gemms;          // tile-kernel launches of the step, in order (for next-layer weight prefetch)
     struct OpInfo { int kind; double flops; double bytes; };   // kind: 0 gemm, 1 groupnorm-apply, 2 cast/upsample, 3 softmax, 4 other
     std::vector<OpInfo> op_info;
@@ -820,12 +823,14 @@ struct sr3_engine {
     std::vector<Op>* bwd_sink = nullptr;                   // where push() records while a layer's backward is being described
     std::vector<std::vector<Op>> bwd_blocks;               // one op list per forward layer, executed last to first
     std::vector<std::vector<int>> bwd_kinds;               // op kinds (profiling): 0 data-gradient tile kernel, 1 GroupNorm / elementwise, 4 other, 6 weight gradient, 7 attention GEMMs
-    // single-launch re-pack (bf16 precision): one PackDesc per packed copy, its source = parameter `pack_src[i]` (second source of a fused
-    // bias: `pack_src2[i]`); device table rebuilt only when the parameter pointers change
+    // every packed copy of a parameter: one PackDesc, its source = parameter `pack_src[i]` (second source of a fused bias: `pack_src2[i]`).
+    // sr3_engine_load_all_params binds the sources to the caller's tensors and packs the whole table in one launch (device table rebuilt
+    // only when the parameter pointers change); sr3_engine_load_param packs the entries of one parameter, and sr3_engine_finalize_params
+    // the fused biases, from the engine's own fp32 copies of their two parameters (the src / src2 registered with them).
     std::vector<PackDesc> pack_descs; std::vector<int> pack_src, pack_src2;
     PackDesc* pack_dev = nullptr; int* pack_ends_dev = nullptr; int pack_blocks = 0; std::vector<const float*> pack_last_ptrs;
     void add_pack(const std::string& pname, PackDesc d, const std::string& pname2 = "") {
-        if (dry || precise) return;
+        if (dry) return;
         pack_descs.push_back(d); pack_src.push_back(pindex.at(pname)); pack_src2.push_back(pname2.empty() ? -1 : pindex.at(pname2));
     }
     std::vector<float*> grad_dst;                          // per parameter (state_dict order): where the running backward writes its gradient
@@ -913,15 +918,10 @@ struct sr3_engine {
         zero_used += n;
         return p;
     }
-    void add_param_hook(const std::string& name, std::function<void(const float*, cudaStream_t)> fn) {
-        if (dry) return;
-        params[pindex.at(name)].hooks.push_back(std::move(fn));
-    }
-    void add_param(const std::string& name, std::vector<int64_t> shape, std::function<void(const float*, cudaStream_t)> load) {
+    void add_param(const std::string& name, std::vector<int64_t> shape) {
         if (dry) return;
         ParamEntry e; e.name = name; e.shape = shape; e.numel = 1;
         for (auto s : shape) e.numel *= s;
-        e.load = std::move(load);
         pindex[name] = (int)params.size();
         params.push_back(std::move(e));
     }
@@ -929,32 +929,25 @@ struct sr3_engine {
         if (dry) return nullptr;
         int64_t n = 1; for (auto s : shape) n *= s;
         float* dst = static_cast<float*>(mem.alloc(n * sizeof(float)));
-        add_param(name, shape, [dst, n](const float* src, cudaStream_t st) { CK(cudaMemcpyAsync(dst, src, n * sizeof(float), cudaMemcpyDeviceToDevice, st)); });
-        { PackDesc d{}; d.type = 0; d.dst = dst; d.n = n; add_pack(name, d); }
+        f32_param_into(name, shape, dst);
         return dst;
     }
     // f32 parameter stored into a slice of a bigger array
     void f32_param_into(const std::string& name, std::vector<int64_t> shape, float* dst) {
         if (dry) return;
-        int64_t n = 1; for (auto s : shape) n *= s;
-        add_param(name, shape, [dst, n](const float* src, cudaStream_t st) { CK(cudaMemcpyAsync(dst, src, n * sizeof(float), cudaMemcpyDeviceToDevice, st)); });
-        { PackDesc d{}; d.type = 0; d.dst = dst; d.n = n; add_pack(name, d); }
+        add_param(name, shape);
+        PackDesc d{}; d.type = 0; d.dst = dst; d.n = params.back().numel; add_pack(name, d);
     }
     // conv weight packed into rows [0,Cout) of a [rows_pad][ktot] bf16 matrix at column k_off
     void conv_weight_param(const std::string& name, bf16* dst, int Cout, int Cin, int k, int ktot, int k_off, int cin_pad) {
         if (dry) return;
-        const int ld = PW * ktot, lo_off = precise ? ktot : 0;
-        add_param(name, {Cout, Cin, k, k}, [=](const float* src, cudaStream_t st) {
-            const long long total = 1LL * Cout * Cin;
-            const int blocks = (int)std::min<long long>((total + 255) / 256, 4096);
-            pack_conv_weight_kernel<<<blocks, 256, 0, st>>>(src, dst, Cout, Cin, k, k, ld, k_off, cin_pad, lo_off);
-            CK(cudaGetLastError());
-        });
-        { PackDesc d{}; d.type = 1; d.dst = dst; d.Cout = Cout; d.Cin = Cin; d.k = k; d.ld = ld; d.k_off = k_off; d.cin_pad = cin_pad; add_pack(name, d); }
+        add_param(name, {Cout, Cin, k, k});
+        PackDesc d{}; d.type = 1; d.dst = dst; d.Cout = Cout; d.Cin = Cin; d.k = k; d.ld = PW * ktot; d.k_off = k_off; d.tap_stride = cin_pad;
+        d.lo_off = precise ? ktot : 0;
+        add_pack(name, d);
     }
-    bf16* new_weight(int rows, int ktot, int block_n) {      // [rows_pad][PW * ktot]: precise mode appends the low halves of every row
+    bf16* new_weight(int rows, int ktot) {      // [rows_pad][PW * ktot]: precise mode appends the low halves of every row
         if (dry) return nullptr;
-        (void)block_n;
         const int rows_pad = ((rows + 127) / 128) * 128;
         return static_cast<bf16*>(mem.alloc((size_t)rows_pad * PW * ktot * sizeof(bf16)));
     }
@@ -1057,13 +1050,13 @@ struct sr3_engine {
         f32_param_into(p + ".noise_func.noise_func.0.bias", {cout}, dry ? nullptr : film_b + foff);
         float* g1 = f32_param(p + ".block1.block.0.weight", {cin});
         float* b1 = f32_param(p + ".block1.block.0.bias", {cin});
-        bf16* w1 = new_weight(cout, 9 * cin, pick_block_n(cout));
+        bf16* w1 = new_weight(cout, 9 * cin);
         conv_weight_param(p + ".block1.block.3.weight", w1, cout, cin, 3, 9 * cin, 0, cin);
         f32_param_into(p + ".block1.block.3.bias", {cout}, dry ? nullptr : film_cb + foff);
         float* g2 = f32_param(p + ".block2.block.0.weight", {cout});
         float* b2 = f32_param(p + ".block2.block.0.bias", {cout});
         const int k2 = 9 * cout + (has_res ? cin : 0);
-        bf16* w2 = new_weight(cout, k2, pick_block_n(cout));
+        bf16* w2 = new_weight(cout, k2);
         conv_weight_param(p + ".block2.block.3.weight", w2, cout, cout, 3, k2, 0, cout);
         float* cb2 = f32_param(p + ".block2.block.3.bias", {cout});
         float* bias_total = cb2;
@@ -1072,9 +1065,8 @@ struct sr3_engine {
             float* cbr = f32_param(p + ".res_conv.bias", {cout});
             if (!dry) {
                 bias_total = static_cast<float*>(mem.alloc(cout * sizeof(float)));
-                float* bt = bias_total;
-                finalize_ops.push_back([=](cudaStream_t st) { add_vec_kernel<<<(cout + 255) / 256, 256, 0, st>>>(cb2, cbr, bt, cout); CK(cudaGetLastError()); });
-                { PackDesc d{}; d.type = 6; d.dst = bt; d.n = cout; add_pack(p + ".block2.block.3.bias", d, p + ".res_conv.bias"); }
+                PackDesc d{}; d.type = 6; d.dst = bias_total; d.src = cb2; d.src2 = cbr; d.n = cout;
+                add_pack(p + ".block2.block.3.bias", d, p + ".res_conv.bias");
             }
         }
         // scratch
@@ -1136,9 +1128,9 @@ struct sr3_engine {
         const int nz = Bp / per;
         float* gn_w = f32_param(p + ".norm.weight", {C});
         float* gn_b = f32_param(p + ".norm.bias", {C});
-        bf16* wqkv = new_weight(3 * C, C, 128);
+        bf16* wqkv = new_weight(3 * C, C);
         conv_weight_param(p + ".qkv.weight", wqkv, 3 * C, C, 1, C, 0, C);
-        bf16* wout = new_weight(C, C, 128);
+        bf16* wout = new_weight(C, C);
         conv_weight_param(p + ".out.weight", wout, C, C, 1, C, 0, C);
         float* bout = f32_param(p + ".out.bias", {C});
         bf16* n = static_cast<bf16*>(role("a1", (size_t)Bp * HW * C * 2 * PW));
@@ -1301,7 +1293,7 @@ struct sr3_engine {
             auto& L = downs[li];
             const bool next_is_down = li + 1 < downs.size() && downs[li + 1].kind == 2;
             if (L.kind == 0) {          // first conv on the (zero-padded to 64 ch) input buffer
-                bf16* w = new_weight(inner, 9 * in_C, pick_block_n(inner));
+                bf16* w = new_weight(inner, 9 * in_C);
                 conv_weight_param(L.name + ".weight", w, inner, cfg.in_channel, 3, 9 * in_C, 0, in_C);
                 float* b = f32_param(L.name + ".bias", {inner});
                 x = new_act(inner, H, W, L.name);
@@ -1317,7 +1309,7 @@ struct sr3_engine {
                 x = add_res_block(L, x, nullptr, film_off, xr, /*x_has_skip=*/true);
             } else {                    // Downsample: conv3x3 stride 2 on the raw stream (unet.py:68-74)
                 const int C = x.C;
-                bf16* w = new_weight(C, 9 * C, pick_block_n(C));
+                bf16* w = new_weight(C, 9 * C);
                 conv_weight_param(L.name + ".conv.weight", w, C, C, 3, 9 * C, 0, C);
                 float* b = f32_param(L.name + ".conv.bias", {C});
                 bf16* raw = train ? last_xraw : static_cast<bf16*>(role("xraw", (size_t)Bp * x.H * x.W * C * 2 * PW));
@@ -1344,21 +1336,13 @@ struct sr3_engine {
                 // Upsample (nearest 2x then conv3x3, unet.py:58-65) folded onto the low-res input (fold_up_conv)
                 const int C = x.C, Hl = x.H, Wl = x.W;
                 const int rows_pad = ((C + 127) / 128) * 128;
-                bf16* wf[4];
-                if (dry) { for (int ph = 0; ph < 4; ++ph) wf[ph] = nullptr; }
-                else {
-                    bf16* wall = static_cast<bf16*>(mem.alloc((size_t)4 * rows_pad * 4 * C * PW * sizeof(bf16)));   // [phase][rows_pad][PW * 4C]
-                    for (int ph = 0; ph < 4; ++ph) wf[ph] = wall + (size_t)ph * rows_pad * 4 * C * PW;
-                }
+                bf16* wall = nullptr;     // [phase][rows_pad][PW * 4C]
                 if (!dry) {
-                    bf16* w0 = wf[0]; bf16* w1 = wf[1]; bf16* w2 = wf[2]; bf16* w3 = wf[3];
-                    const int ldw = 4 * C * PW, low = precise ? 4 * C : 0;
-                    add_param(L.name + ".conv.weight", {C, C, 3, 3}, [=](const float* src, cudaStream_t st) {
-                        const long long total = 4LL * C * C * 4;
-                        fold_upsample_weight_kernel<<<(int)std::min<long long>((total + 255) / 256, 4096), 256, 0, st>>>(src, w0, w1, w2, w3, C, C, ldw, low);
-                        CK(cudaGetLastError());
-                    });
-                    { PackDesc d{}; d.type = 5; d.dst = w0; d.Cout = C; d.Cin = C; d.ld = ldw; d.n = (long long)rows_pad * 4 * C * PW; add_pack(L.name + ".conv.weight", d); }
+                    wall = static_cast<bf16*>(mem.alloc((size_t)4 * rows_pad * 4 * C * PW * sizeof(bf16)));
+                    add_param(L.name + ".conv.weight", {C, C, 3, 3});
+                    PackDesc d{}; d.type = 5; d.dst = wall; d.Cout = C; d.Cin = C; d.ld = 4 * C * PW; d.lo_off = precise ? 4 * C : 0;
+                    d.n = (long long)rows_pad * 4 * C * PW;
+                    add_pack(L.name + ".conv.weight", d);
                 }
                 float* b = f32_param(L.name + ".conv.bias", {C});
                 bf16* raw = train ? last_xraw : static_cast<bf16*>(role("xraw", (size_t)Bp * Hl * Wl * C * 2 * PW));
@@ -1370,7 +1354,7 @@ struct sr3_engine {
                 Act y = new_act(C, Hl * 2, Wl * 2, L.name);
                 ConvArgs c;
                 fold_up_conv(c, raw, Bp, Hl, Wl, C, PW);
-                c.w = wf[0]; c.bias = b; c.out = y;
+                c.w = wall; c.bias = b; c.out = y;
                 add_conv(c);
                 if (train) bwd_upsample(L.name, x, y, upb);
                 x = y;
@@ -1382,7 +1366,7 @@ struct sr3_engine {
             REQUIRE(co <= 4 && co == cfg.channels, "out_channel must equal diffusion channels (<=4)");
             float* g = f32_param("final_conv.block.0.weight", {C});
             float* be = f32_param("final_conv.block.0.bias", {C});
-            bf16* w = new_weight(co, 9 * C, 16);
+            bf16* w = new_weight(co, 9 * C);
             conv_weight_param("final_conv.block.3.weight", w, co, C, 3, 9 * C, 0, C);
             float* b = f32_param("final_conv.block.3.bias", {co});
             bf16* a = static_cast<bf16*>(role("a1", (size_t)Bp * H * W * C * 2 * PW));
@@ -1737,8 +1721,11 @@ int sr3_engine_load_param(sr3_engine* e, const char* name, const float* src, int
     ParamEntry& p = e->params[it->second];
     REQUIRE(p.numel == numel, "size mismatch for %s: expected %lld elements, got %lld", name, (long long)p.numel, (long long)numel);
     CK(cudaSetDevice(e->dev));
-    p.load(src, static_cast<cudaStream_t>(stream));
-    for (auto& h : p.hooks) h(src, static_cast<cudaStream_t>(stream));
+    for (size_t i = 0; i < e->pack_descs.size(); ++i) {      // every packed copy of this parameter; the fused biases wait for finalize
+        if (e->pack_src[i] != it->second || e->pack_descs[i].type == 6) continue;
+        PackDesc d = e->pack_descs[i]; d.src = src;
+        pack_one(d, static_cast<cudaStream_t>(stream));
+    }
     p.loaded = true;
     API_END
 }
@@ -1750,59 +1737,35 @@ int sr3_engine_load_all_params(sr3_engine* e, const float* const* srcs, int n, v
     CK(cudaSetDevice(e->dev));
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     for (int i = 0; i < n; ++i) REQUIRE(srcs[i] != nullptr, "null pointer for %s", e->params[i].name.c_str());
-    if (!e->pack_descs.empty() && !e->precise) {
-        // one launch over the descriptor table (rebuilt only when a parameter moved)
-        const size_t nd = e->pack_descs.size();
-        if (e->pack_last_ptrs.size() != (size_t)n || memcmp(e->pack_last_ptrs.data(), srcs, n * sizeof(float*)) != 0 || !e->pack_dev) {
-            std::vector<PackDesc> tab = e->pack_descs;
-            for (size_t i = 0; i < nd; ++i) { tab[i].src = srcs[e->pack_src[i]]; tab[i].src2 = e->pack_src2[i] >= 0 ? srcs[e->pack_src2[i]] : nullptr; }
-            if (!e->pack_dev) {
-                e->pack_dev = static_cast<PackDesc*>(e->mem.alloc(nd * sizeof(PackDesc)));
-                e->pack_ends_dev = static_cast<int*>(e->mem.alloc(nd * sizeof(int)));
-                // blocks in proportion to the work of an entry: ~8 (o, c) pairs (x k*k taps) or 32 plain elements per thread
-                std::vector<int> ends(nd);
-                int acc = 0;
-                for (size_t i = 0; i < nd; ++i) {
-                    const PackDesc& d = tab[i];
-                    long long items;
-                    switch (d.type) {
-                        case 0: case 6: items = (d.n + 3) / 4; break;
-                        case 1: case 2: items = 1LL * d.Cout * d.Cin; break;
-                        case 3: items = 2LL * d.Cin * d.Cout; break;
-                        case 4: items = 4LL * d.Cin * d.Cout; break;
-                        default: items = 4LL * d.Cin * d.Cout; break;
-                    }
-                    long long nb = (items + 256 * 8 - 1) / (256 * 8);
-                    if (nb < 1) nb = 1;
-                    if (nb > 4096) nb = 4096;
-                    acc += (int)nb; ends[i] = acc;
-                }
-                e->pack_blocks = acc;
-                CK(cudaMemcpy(e->pack_ends_dev, ends.data(), nd * sizeof(int), cudaMemcpyHostToDevice));
-            }
-            CK(cudaMemcpyAsync(e->pack_dev, tab.data(), nd * sizeof(PackDesc), cudaMemcpyHostToDevice, st));
-            CK(cudaStreamSynchronize(st));                 // `tab` is pageable host memory
-            e->pack_last_ptrs.assign(srcs, srcs + n);
+    // one launch over the descriptor table (rebuilt only when a parameter moved)
+    const size_t nd = e->pack_descs.size();
+    if (e->pack_last_ptrs.size() != (size_t)n || memcmp(e->pack_last_ptrs.data(), srcs, n * sizeof(float*)) != 0 || !e->pack_dev) {
+        std::vector<PackDesc> tab = e->pack_descs;
+        for (size_t i = 0; i < nd; ++i) { tab[i].src = srcs[e->pack_src[i]]; tab[i].src2 = e->pack_src2[i] >= 0 ? srcs[e->pack_src2[i]] : nullptr; }
+        if (!e->pack_dev) {
+            e->pack_dev = static_cast<PackDesc*>(e->mem.alloc(nd * sizeof(PackDesc)));
+            e->pack_ends_dev = static_cast<int*>(e->mem.alloc(nd * sizeof(int)));
+            std::vector<int> ends(nd);
+            int acc = 0;
+            for (size_t i = 0; i < nd; ++i) { acc += pack_entry_blocks(tab[i]); ends[i] = acc; }
+            e->pack_blocks = acc;
+            CK(cudaMemcpy(e->pack_ends_dev, ends.data(), nd * sizeof(int), cudaMemcpyHostToDevice));
         }
-        pack_all_kernel<<<dim3((unsigned)e->pack_blocks), 256, 0, st>>>(e->pack_dev, e->pack_ends_dev, (int)nd);
-        CK(cudaGetLastError());
-        for (auto& p : e->params) p.loaded = true;
-        return 0;
+        CK(cudaMemcpyAsync(e->pack_dev, tab.data(), nd * sizeof(PackDesc), cudaMemcpyHostToDevice, st));
+        CK(cudaStreamSynchronize(st));                 // `tab` is pageable host memory
+        e->pack_last_ptrs.assign(srcs, srcs + n);
     }
-    for (int i = 0; i < n; ++i) {
-        ParamEntry& p = e->params[i];
-        p.load(srcs[i], st);
-        for (auto& h : p.hooks) h(srcs[i], st);
-        p.loaded = true;
-    }
-    for (auto& op : e->finalize_ops) op(st);
+    pack_all_kernel<<<dim3((unsigned)e->pack_blocks), 256, 0, st>>>(e->pack_dev, e->pack_ends_dev, (int)nd);
+    CK(cudaGetLastError());
+    for (auto& p : e->params) p.loaded = true;
     API_END
 }
 int sr3_engine_finalize_params(sr3_engine* e, void* stream) {
     API_BEGIN
     REQUIRE(e, "null engine");
     e->check_params();
-    for (auto& op : e->finalize_ops) op(static_cast<cudaStream_t>(stream));
+    for (const PackDesc& d : e->pack_descs)
+        if (d.type == 6) pack_one(d, static_cast<cudaStream_t>(stream));     // src / src2: the engine's copies of the two biases
     API_END
 }
 
@@ -2149,28 +2112,29 @@ int sr3_test_conv_ex(const sr3_test_conv_args* a, sr3_gemm_geometry* geometry, v
     DevAllocs mem;
     const int rows_pad = ((Cout + 127) / 128) * 128;
     ConvArgs c;
+    // the weights are packed by the engine's descriptors (conv_weight_param, the Upsample fold of the layer builder)
+    PackDesc pd{}; pd.Cout = Cout; pd.Cin = Cin; pd.src = a->w;
     if (a->fold_up) {
         fold_up_conv(c, static_cast<const bf16*>(a->x), B, H, W, Cin, PW);
-        const int ldw = PW * c.ktot;
-        bf16* wall = static_cast<bf16*>(mem.alloc((size_t)4 * rows_pad * ldw * sizeof(bf16)));     // [phase][rows_pad][PW * 4C]
-        const long long phase = (long long)rows_pad * ldw;
-        fold_upsample_weight_kernel<<<1024, 256, 0, st>>>(a->w, wall, wall + phase, wall + 2 * phase, wall + 3 * phase, Cout, Cin, ldw, PW == 2 ? c.ktot : 0);
-        CK(cudaGetLastError());
-        c.w = wall;
+        pd.type = 5; pd.ld = PW * c.ktot; pd.n = (long long)rows_pad * pd.ld; pd.lo_off = PW == 2 ? c.ktot : 0;
+        bf16* wall = static_cast<bf16*>(mem.alloc((size_t)4 * pd.n * sizeof(bf16)));     // [phase][rows_pad][PW * 4C]
+        pd.dst = wall; c.w = wall;
+        pack_one(pd, st);
     } else {
-        const int ktot = k * k * Cin + (a->x2 ? a->Cin2 : 0), ld = PW * ktot, lo_off = PW == 2 ? ktot : 0;
-        bf16* wp = static_cast<bf16*>(mem.alloc((size_t)rows_pad * ld * sizeof(bf16)));
-        pack_conv_weight_kernel<<<1024, 256, 0, st>>>(a->w, wp, Cout, Cin, k, k, ld, 0, Cin, lo_off);
-        CK(cudaGetLastError());
+        const int ktot = k * k * Cin + (a->x2 ? a->Cin2 : 0);
+        pd.type = 1; pd.k = k; pd.ld = PW * ktot; pd.k_off = 0; pd.tap_stride = Cin; pd.lo_off = PW == 2 ? ktot : 0;
+        bf16* wp = static_cast<bf16*>(mem.alloc((size_t)rows_pad * pd.ld * sizeof(bf16)));
+        pd.dst = wp; c.w = wp;
+        pack_one(pd, st);
         c.a[0] = s == 1 ? nhwc_src(a->x, B, H, W, Cin * PW) : nhwc_stride2_src(a->x, B, H, W, Cin * PW); c.c0 = Cin;
         add_conv_slabs(c.slabs, 0, Cin, k, s, 0, Cin * PW);
         if (a->x2) {      // ResnetBlock block2 + res_conv (add_res_block): the 1x1 shortcut is K columns [k*k*Cin, ktot) of the same GEMM
-            pack_conv_weight_kernel<<<1024, 256, 0, st>>>(a->w2, wp, Cout, a->Cin2, 1, 1, ld, k * k * Cin, a->Cin2, lo_off);
-            CK(cudaGetLastError());
+            pd.src = a->w2; pd.Cin = a->Cin2; pd.k = 1; pd.k_off = k * k * Cin; pd.tap_stride = a->Cin2;
+            pack_one(pd, st);
             c.n_a = 2; c.a[1] = nhwc_src(a->x2, B, H, W, a->Cin2 * PW); c.c1 = a->Cin2;
             add_conv_slabs(c.slabs, 1, a->Cin2, 1, 1, k * k * Cin);
         }
-        c.w = wp; c.ktot = ktot; c.cout = Cout; c.OH = H / s; c.OW = W / s;
+        c.ktot = ktot; c.cout = Cout; c.OH = H / s; c.OW = W / s;
     }
     c.bias = a->bias; c.bias2 = a->bias2; c.bias2_stride = Cout; c.resid = a->resid;
     c.out.p = a->y; c.out.stats = a->stats;

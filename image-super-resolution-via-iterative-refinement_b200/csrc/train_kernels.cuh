@@ -2,71 +2,14 @@
 // everything the backward pass needs that is not the forward tile kernel.
 //
 //   * data gradients of every conv are the forward tile kernel (gemm_wgmma.cuh) on re-packed weights (mirrored taps for 3x3 stride 1,
-//     the four output-parity phases for the stride-2 Downsample conv, a 4x4 stride-2 kernel for nearest-2x + conv3x3): the packers are here;
+//     the four output-parity phases for the stride-2 Downsample conv, a 4x4 stride-2 kernel for nearest-2x + conv3x3), packed by pack_entry
+//     (the end of this file), which also packs every forward weight;
 //   * weight gradients are a wgmma GEMM that contracts over PIXELS with both operands MN-major (wgrad_kernel);
 //   * GroupNorm + SiLU (+ Dropout) backward, bias / FiLM / noise-MLP gradients, attention backward, loss gradient, Adam.
 #pragma once
 #include "aux_kernels.cuh"
 
 namespace sr3 {
-
-// ------------------------------------------------------------------------------------------------ weight packers for the data gradients
-// dgrad of conv (stride 1, k in {1,3}): dX = conv(dY, W') with W'[ci][((k-1-r)*k + (k-1-s)) * cout_pad + co] = W[co][ci][r][s].
-// One thread per (c, o), o fastest: the k*k taps of a pair are contiguous in src, and for a fixed tap the warp's o are contiguous in dst.
-__global__ void __launch_bounds__(256) pack_dgrad_weight_kernel(const float* __restrict__ src, __nv_bfloat16* __restrict__ dst, int Cout, int Cin, int k,
-                                                                int cout_pad, int ld) {
-    const long long total = static_cast<long long>(Cout) * Cin;
-    const int taps = k * k;
-    for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total; i += static_cast<long long>(gridDim.x) * blockDim.x) {
-        const int o = static_cast<int>(i % Cout);
-        const int c = static_cast<int>(i / Cout);
-        const float* sp = src + (static_cast<long long>(o) * Cin + c) * taps;
-        __nv_bfloat16* dp = dst + static_cast<long long>(c) * ld + o;
-        for (int t = 0; t < taps; ++t) dp[(taps - 1 - t) * cout_pad] = __float2bfloat16_rn(sp[t]);     // (k-1-r)*k + (k-1-s) = k*k-1 - (r*k+s)
-    }
-}
-// dgrad of the stride-2 Downsample conv (unet.py:68-74) as four output-parity phases on the low-resolution dY grid (the same op shape as the
-// folded Upsample forward): input pixel (2i+py, 2j+px) receives, through tap offset (py-1+a, px-1+b) of dY, kernel row R(py,a), column R(px,b)
-// with R(0,0) = none, R(0,1) = 1, R(1,0) = 2, R(1,1) = 0.   dst[phase][ci][(a*2+b)*Cout + co]
-__global__ void __launch_bounds__(256) pack_down_dgrad_weight_kernel(const float* __restrict__ src, __nv_bfloat16* __restrict__ dst, int Cout, int Cin, int rows_pad) {
-    const long long total = 4LL * Cin * 4 * Cout;
-    for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total; i += static_cast<long long>(gridDim.x) * blockDim.x) {
-        long long r = i;
-        const int o = static_cast<int>(r % Cout); r /= Cout;
-        const int ab = static_cast<int>(r % 4); r /= 4;
-        const int c = static_cast<int>(r % Cin);
-        const int ph = static_cast<int>(r / Cin);
-        const int py = ph >> 1, px = ph & 1, a = ab >> 1, b = ab & 1;
-        const int rr = py == 0 ? (a == 1 ? 1 : -1) : (a == 0 ? 2 : 0);
-        const int ss = px == 0 ? (b == 1 ? 1 : -1) : (b == 0 ? 2 : 0);
-        const float v = (rr < 0 || ss < 0) ? 0.f : src[((static_cast<long long>(o) * Cin + c) * 3 + rr) * 3 + ss];
-        dst[(static_cast<long long>(ph) * rows_pad + c) * (4LL * Cout) + ab * Cout + o] = __float2bfloat16_rn(v);
-    }
-}
-// dgrad of Upsample (nearest 2x -> conv3x3, unet.py:58-65): dX[i][j] = sum_{u,v in 0..3} K[u][v] dY[2i-1+u][2j-1+v],
-// K[u][v][ci][co] = sum over (e, r): e + 2 - r = u, (f, s): f + 2 - s = v of W[co][ci][r][s]  (e, f in {0,1}: the 2x2 replicated pixels).
-// dst[ci][(u*4+v)*Cout + co]
-__global__ void __launch_bounds__(256) pack_up_dgrad_weight_kernel(const float* __restrict__ src, __nv_bfloat16* __restrict__ dst, int Cout, int Cin) {
-    const long long total = static_cast<long long>(Cin) * 16 * Cout;
-    for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total; i += static_cast<long long>(gridDim.x) * blockDim.x) {
-        long long r = i;
-        const int o = static_cast<int>(r % Cout); r /= Cout;
-        const int uv = static_cast<int>(r % 16);
-        const int c = static_cast<int>(r / 16);
-        const int u = uv >> 2, v = uv & 3;
-        float acc = 0.f;
-        for (int e = 0; e < 2; ++e) {
-            const int rr = e + 2 - u;
-            if (rr < 0 || rr > 2) continue;
-            for (int f = 0; f < 2; ++f) {
-                const int ss = f + 2 - v;
-                if (ss < 0 || ss > 2) continue;
-                acc += src[((static_cast<long long>(o) * Cin + c) * 3 + rr) * 3 + ss];
-            }
-        }
-        dst[static_cast<long long>(c) * (16LL * Cout) + uv * Cout + o] = __float2bfloat16_rn(acc);
-    }
-}
 
 // ------------------------------------------------------------------------------------------------ weight gradient (wgmma, MN-major operands)
 //     dW[co][tap][ci] = sum over pixels p of  dY[p][co] * X[p + tap][ci]
@@ -749,15 +692,18 @@ __global__ void __launch_bounds__(256) adam_kernel(const AdamTensor* __restrict_
     }
 }
 
-// ------------------------------------------------------------------------------------------------ one launch for the whole re-pack
-// After every optimizer step all packed copies of the fp32 parameters are refreshed (forward K-major weights, data-gradient weights, folded
-// Upsample phases, Downsample / Upsample data-gradient kernels, plain fp32 copies of the GroupNorm / bias / Linear parameters, fused bias
-// vectors).  As separate launches that is ~470 tiny stream operations per step; this kernel walks a device table instead: blockIdx.y = entry,
-// blockIdx.x / gridDim.x stride over the entry's elements.
+// ------------------------------------------------------------------------------------------------ weight packing
+// Every packed copy of an fp32 parameter is one PackDesc, and pack_entry is the only code that writes one: the forward K-major conv weights,
+// the folded Upsample phases, the data-gradient weights of the training plan, plain fp32 copies of the GroupNorm / bias / Linear parameters
+// and the fused block2 + res_conv bias.  pack_all_kernel walks the whole table in one launch (the training loop's re-pack after every
+// optimizer step: ~470 copies); pack_one_kernel packs one entry (loading a single parameter, sr3_test_conv_ex).
+// One thread per work item, grid-strided; the item order keeps both the reads and the writes of a warp coalesced.
 struct PackDesc {
     int type;                 // 0 fp32 copy, 1 forward conv weight, 2 stride-1 data-gradient weight, 3 Downsample data-gradient phases,
                               // 4 Upsample data-gradient 4x4 kernel, 5 folded Upsample forward phases, 6 dst = src + src2 (fused bias)
-    int Cout, Cin, k, ld, k_off, cin_pad, rows_pad;
+    int Cout, Cin, k, ld, k_off, rows_pad;
+    int tap_stride;           // types 1, 2: columns between consecutive taps of a dst row (cin_pad / cout_pad)
+    int lo_off;               // types 1, 5, precise mode: the low halves bf16(v - bf16(v)) sit lo_off elements after the high halves; else 0
     const float* src; const float* src2;
     void* dst;
     long long n;              // type 0 / 6: elements;  type 5: element stride between the four phase matrices
@@ -768,27 +714,38 @@ __device__ __forceinline__ void pack_entry(const PackDesc& d, long long i0, long
     case 0: { float* o = static_cast<float*>(d.dst); for (long long i = i0; i < d.n; i += stride) o[i] = d.src[i]; break; }
     case 6: { float* o = static_cast<float*>(d.dst); for (long long i = i0; i < d.n; i += stride) o[i] = d.src[i] + d.src2[i]; break; }
     case 1: {
+        // OIHW -> K-major: dst[o][k_off + (r*k+s)*tap_stride + c]; one item per (o, c), c fastest
         const int taps = d.k * d.k;
         const long long total = static_cast<long long>(d.Cout) * d.Cin;
         for (long long i = i0; i < total; i += stride) {
             const int c = static_cast<int>(i % d.Cin), o = static_cast<int>(i / d.Cin);
             const float* sp = d.src + i * taps;
-            for (int t = 0; t < taps; ++t) db[static_cast<long long>(o) * d.ld + d.k_off + t * d.cin_pad + c] = __float2bfloat16_rn(sp[t]);
+            for (int t = 0; t < taps; ++t) {
+                const float v = sp[t];
+                const long long di = static_cast<long long>(o) * d.ld + d.k_off + t * d.tap_stride + c;
+                db[di] = __float2bfloat16_rn(v);
+                if (d.lo_off) db[di + d.lo_off] = __float2bfloat16_rn(bf16_residual(v));
+            }
         }
         break;
     }
     case 2: {
+        // data gradient of a stride-1 conv: dX = conv(dY, W') with W'[ci][((k-1-r)*k + (k-1-s)) * tap_stride + co] = W[co][ci][r][s];
+        // one item per (c, o), o fastest
         const int taps = d.k * d.k;
         const long long total = static_cast<long long>(d.Cout) * d.Cin;
         for (long long i = i0; i < total; i += stride) {
             const int o = static_cast<int>(i % d.Cout), c = static_cast<int>(i / d.Cout);
             const float* sp = d.src + (static_cast<long long>(o) * d.Cin + c) * taps;
             __nv_bfloat16* dp = db + static_cast<long long>(c) * d.ld + o;
-            for (int t = 0; t < taps; ++t) dp[(taps - 1 - t) * d.cin_pad] = __float2bfloat16_rn(sp[t]);      // cin_pad holds cout_pad here
+            for (int t = 0; t < taps; ++t) dp[(taps - 1 - t) * d.tap_stride] = __float2bfloat16_rn(sp[t]);     // (k-1-r)*k + (k-1-s) = k*k-1 - (r*k+s)
         }
         break;
     }
     case 3: {
+        // data gradient of the stride-2 Downsample conv (unet.py:68-74) as four output-parity phases on the low-resolution dY grid: input
+        // pixel (2i+py, 2j+px) receives, through tap offset (py-1+a, px-1+b) of dY, kernel row R(py,a), column R(px,b) with R(0,0) = none,
+        // R(0,1) = 1, R(1,0) = 2, R(1,1) = 0.   dst[phase][ci][(a*2+b)*Cout + co], phases rows_pad rows apart
         const long long total = 4LL * d.Cin * 4 * d.Cout;
         for (long long i = i0; i < total; i += stride) {
             long long r = i;
@@ -805,6 +762,9 @@ __device__ __forceinline__ void pack_entry(const PackDesc& d, long long i0, long
         break;
     }
     case 4: {
+        // data gradient of Upsample (nearest 2x -> conv3x3, unet.py:58-65): dX[i][j] = sum_{u,v in 0..3} K[u][v] dY[2i-1+u][2j-1+v],
+        // K[u][v][ci][co] = sum over (e, r): e + 2 - r = u, (f, s): f + 2 - s = v of W[co][ci][r][s]  (e, f in {0,1}: the 2x2 replicated
+        // pixels).   dst[ci][(u*4+v)*Cout + co]
         const long long total = static_cast<long long>(d.Cin) * 16 * d.Cout;
         for (long long i = i0; i < total; i += stride) {
             long long r = i;
@@ -827,6 +787,8 @@ __device__ __forceinline__ void pack_entry(const PackDesc& d, long long i0, long
         break;
     }
     case 5: {
+        // the four phase convs of a folded nearest-2x -> conv3x3: for output parity py the kernel rows that land on low-res row offset a are
+        // R(0,0)={0}, R(0,1)={1,2}, R(1,0)={0,1}, R(1,1)={2} (same for columns); summed in fp32, rounded once.   dst[phase][o][(a*2+b)*Cin + c]
         const long long total = 4LL * d.Cout * d.Cin * 4;
         for (long long i = i0; i < total; i += stride) {
             long long r = i;
@@ -840,19 +802,36 @@ __device__ __forceinline__ void pack_entry(const PackDesc& d, long long i0, long
             float acc = 0.f;
             for (int rr = r0; rr <= r1; ++rr)
                 for (int ss = s0; ss <= s1; ++ss) acc += d.src[((static_cast<long long>(o) * d.Cin + c) * 3 + rr) * 3 + ss];
-            db[ph * d.n + static_cast<long long>(o) * d.ld + ab * d.Cin + c] = __float2bfloat16_rn(acc);
+            const long long di = ph * d.n + static_cast<long long>(o) * d.ld + ab * d.Cin + c;
+            db[di] = __float2bfloat16_rn(acc);
+            if (d.lo_off) db[di + d.lo_off] = __float2bfloat16_rn(bf16_residual(acc));
         }
         break;
     }
     default: break;
     }
 }
-// block_ends[e] = one past the last block of entry e (blocks are dealt in proportion to the entries' work)
+// 256-thread blocks for one entry, in proportion to its work: ~8 (o, c) pairs (x k*k taps) or 32 plain elements per thread
+inline int pack_entry_blocks(const PackDesc& d) {
+    long long items;
+    switch (d.type) {
+        case 0: case 6: items = (d.n + 3) / 4; break;
+        case 1: case 2: items = 1LL * d.Cout * d.Cin; break;
+        case 3: items = 2LL * d.Cin * d.Cout; break;
+        default: items = 4LL * d.Cin * d.Cout; break;
+    }
+    const long long nb = (items + 256 * 8 - 1) / (256 * 8);
+    return static_cast<int>(nb < 1 ? 1 : (nb > 4096 ? 4096 : nb));
+}
+// block_ends[e] = one past the last block of entry e (pack_entry_blocks(tab[e]) blocks each)
 __global__ void __launch_bounds__(256) pack_all_kernel(const PackDesc* __restrict__ tab, const int* __restrict__ block_ends, int n_entries) {
     const int e = find_entry(block_ends, n_entries, blockIdx.x);
     const int b0 = e == 0 ? 0 : __ldg(&block_ends[e - 1]), nb = __ldg(&block_ends[e]) - b0;
     const PackDesc d = tab[e];
     pack_entry(d, (blockIdx.x - b0) * static_cast<long long>(blockDim.x) + threadIdx.x, static_cast<long long>(nb) * blockDim.x);
+}
+__global__ void __launch_bounds__(256) pack_one_kernel(const __grid_constant__ PackDesc d) {
+    pack_entry(d, blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x, static_cast<long long>(gridDim.x) * blockDim.x);
 }
 
 }  // namespace sr3

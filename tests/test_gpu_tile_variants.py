@@ -229,7 +229,7 @@ FOLD_ROWS = {(0, 0): (0, 0), (0, 1): (1, 2), (1, 0): (0, 1), (1, 1): (2, 2)}    
 
 
 def fold_weights(w):
-    """The four 2x2 phase kernels of nearest-2x -> conv3x3, as fold_upsample_weight_kernel forms them: the aliased taps summed in fp32 in
+    """The four 2x2 phase kernels of nearest-2x -> conv3x3, as `pack_entry` type 5 forms them: the aliased taps summed in fp32 in
     row-then-column order, rounded once to bf16.  Returns [4][Cout][Cin][2][2] (fp32 holding bf16 values), phase = 2 py + px."""
     out = torch.zeros(4, w.shape[0], w.shape[1], 2, 2)
     for py in range(2):

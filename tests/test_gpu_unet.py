@@ -179,6 +179,71 @@ def test_state_dict_roundtrip_and_reload():
     assert torch.equal(e3, e1)         # same weights, same inputs -> same bits (order-independent statistics)
 
 
+def _engine_loaded_by(route, unet, batch, precision="bf16", train_dropout=None):
+    """A fresh engine for `unet`'s weights, loaded through one of the two parameter entry points: "table" = load_params_fast (every packed
+    copy in one launch: UNet.engine() and the training loop's re-pack), "per_name" = Engine.load_state_dict (sr3_engine_load_param for
+    every name, then sr3_engine_finalize_params for the fused biases)."""
+    from sr3_b200 import _native
+    cfg = dict(unet.arch, channels=3, conditional=True, precision=precision)
+    eng = _native.Engine(cfg, batch, torch.device("cuda", torch.cuda.current_device()), train_dropout=train_dropout)
+    eng.set_schedule(*unet._schedule)
+    if route == "table":
+        by_name = dict(unet.named_parameters())
+        eng.load_params_fast([by_name[n].detach() for n, _ in eng.param_table()])
+    else:
+        eng.load_state_dict(unet.state_dict())
+    return eng
+
+
+@pytest.mark.parametrize("precision", ["bf16", "fp32"])
+def test_load_routes_pack_identical_weights(precision):
+    """Both parameter entry points pack the same bytes (forward weights, folded Upsample phases, fused block2 + res_conv bias, and in
+    precise mode their low halves): eps and one seeded p_sample are bit-identical."""
+    net = build(TINY_UNET, 32, 3, precision=precision)
+    gen = torch.Generator().manual_seed(6)
+    cond = (torch.rand(2, 3, 32, 32, generator=gen) * 2 - 1).cuda()
+    x = torch.randn(2, 3, 32, 32, generator=gen).cuda()
+    nl = torch.tensor([[0.3], [0.8]]).cuda()
+    outs = {}
+    for route in ("table", "per_name"):
+        eng = _engine_loaded_by(route, net.denoise_fn, 2, precision)
+        eps = eng.unet_forward(torch.cat([cond, x], 1), nl)
+        xs = eng.p_sample(x, 700, condition_x=cond, seed=21)
+        outs[route] = (eps.cpu(), xs.cpu())
+        del eng
+    assert torch.isfinite(outs["table"][0]).all() and torch.isfinite(outs["table"][1]).all()
+    assert torch.equal(outs["table"][0], outs["per_name"][0])
+    assert torch.equal(outs["table"][1], outs["per_name"][1])
+
+
+def test_load_routes_give_the_same_training_step():
+    """The training plan (no dropout) loaded through either entry point: the loss bit for bit (the forward is bit-reproducible), and every
+    gradient, which also goes through the data-gradient weight copies, within what two backward runs of one engine agree to (the backward
+    accumulates with fp32 atomics)."""
+    import _train_util as tu
+    net = build(TINY_UNET, 32, 3)
+    hr, sr, noise = tu.batch(2, 32, 17)
+    gamma = tu.draw_gamma(2, 9)
+    runs = {}
+    for route in ("table", "per_name"):
+        eng = _engine_loaded_by(route, net.denoise_fn, 2, train_dropout=0.0)
+        table = eng.param_table()
+        for rep in range(2):
+            loss = eng.train_forward(hr, sr, gamma, noise, "l1", 0)
+            grads = [torch.empty(shape, device="cuda") for _, shape in table]
+            eng.train_backward(1.0 / hr.numel(), grads)
+            runs[route, rep] = (loss, {n: g.cpu() for (n, _), g in zip(table, grads)})
+        del eng
+    assert runs["table", 0][0] == runs["table", 1][0] == runs["per_name", 0][0] == runs["per_name", 1][0]
+
+    def worst(a, b):
+        return max(tu.rel(runs[a][1][k], runs[b][1][k]) for k in runs[a][1])
+    same = max(worst(("table", 0), ("table", 1)), worst(("per_name", 0), ("per_name", 1)))
+    cross = worst(("table", 0), ("per_name", 0))
+    print(f"worst gradient rel diff: same route {same:.2e}, across routes {cross:.2e}")
+    assert cross <= max(2 * same, 1e-6), (cross, same)
+
+
 def test_tiny_unconditional_loop_matches_oracle():
     """sample() path (diffusion.py:180-187, 202-206): unconditional UNet (in_channel=3), seeded loop with injected noise."""
     sched = {"schedule": "linear", "n_timestep": 6, "linear_start": 1e-4, "linear_end": 2e-2}

@@ -109,7 +109,7 @@ def test_dgrad_identity_used_by_the_gpu_test():
 def test_downsample_dgrad_is_four_parity_phase_convs():
     """The data gradient of the stride-2 Downsample conv (unet.py:68-74) written as four 2x2-tap convolutions on the low-res dY grid, one per
     input-pixel parity (py, px) -- the op shape csrc/train_plan.inc `bwd_downsample` hands to the forward tile kernel, with the kernel-row
-    table of pack_down_dgrad_weight_kernel: R(0,0) = none, R(0,1) = 1, R(1,0) = 2, R(1,1) = 0."""
+    table of `pack_entry` type 3 (csrc/train_kernels.cuh): R(0,0) = none, R(0,1) = 1, R(1,0) = 2, R(1,1) = 0."""
     import torch.nn.functional as F
     g = torch.Generator().manual_seed(0)
     x = torch.randn(2, 5, 8, 12, generator=g, requires_grad=True)
@@ -137,7 +137,7 @@ def test_downsample_dgrad_is_four_parity_phase_convs():
 def test_upsample_dgrad_is_one_4x4_stride2_conv():
     """nearest-2x -> conv3x3 (unet.py:58-65): its data gradient (conv-transpose, then the 2x2 sum of the replicated pixels) equals ONE 4x4
     stride-2 convolution over dY, dX[i][j] = sum_{u,v} K[u][v] dY[2i-1+u][2j-1+v], K[u][v] = sum over (e, r): e+2-r = u, (f, s): f+2-s = v of
-    W[r][s] -- the kernel pack_up_dgrad_weight_kernel builds and `bwd_upsample` runs through the parity view."""
+    W[r][s] -- the kernel `pack_entry` type 4 builds and `bwd_upsample` runs through the parity view."""
     import torch.nn.functional as F
     g = torch.Generator().manual_seed(1)
     x = torch.randn(2, 4, 5, 6, generator=g, requires_grad=True)
