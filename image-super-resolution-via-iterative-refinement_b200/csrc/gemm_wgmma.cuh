@@ -25,6 +25,7 @@
 //   (model/sr3_modules/diffusion.py:141-174 of the reference) and writes x_{t-1} straight into the next step's input.
 #pragma once
 #include <cuda.h>
+#include <type_traits>
 #include "ptx.cuh"
 
 namespace sr3 {
@@ -289,33 +290,76 @@ __device__ __forceinline__ void gemm_stage_setup(const GemmParams& p, const Gemm
     }
 }
 
-// Accumulator chunk -> rows: this warp's 32 rows x CW columns of chunk `cl` of the warpgroup accumulator go through the warp's 4 KB
+// Accumulator chunk -> rows: this warp's 32 rows x CW columns of chunk CL of the warpgroup accumulator go through the warp's 4 KB
 // staging buffer (float4 index XOR-swizzled with the row: conflict-free both ways) and come back as lane = row, v[j] = column j.
-template <int WN, int CW>
-__device__ __forceinline__ void acc_chunk_rows(const float (&acc)[2][WN / 2], const int cl, float* buf, uint32_t (&v)[CW]) {
+// CL is a template argument so that only chunk CL's registers are read: the chunk is dead afterwards.
+template <int WN, int CW, int CL>
+__device__ __forceinline__ void acc_chunk_rows(const float (&acc)[2][WN / 2], float* buf, float (&v)[32]) {
+    static_assert(CW <= 32 && (CL + 1) * CW <= WN, "accumulator chunk");
     const int lane = static_cast<int>(lane_id());
     __syncwarp();
 #pragma unroll
-    for (int c = 0; c < WN / CW; ++c) {
-        if (c != cl) continue;
+    for (int i = 0; i < 2; ++i) {
 #pragma unroll
-        for (int i = 0; i < 2; ++i) {
-#pragma unroll
-            for (int j = (c * CW) / 2; j < ((c + 1) * CW) / 2; j += 2) {
-                const int r = (lane >> 2) + 8 * i + 16 * ((j >> 1) & 1);
-                const int cc = 8 * (j >> 2) - c * CW + 2 * (lane & 3);
-                *reinterpret_cast<float2*>(buf + r * 32 + (cc ^ ((r & 7) << 2))) = make_float2(acc[i][j], acc[i][j + 1]);
-            }
+        for (int j = (CL * CW) / 2; j < ((CL + 1) * CW) / 2; j += 2) {
+            const int r = (lane >> 2) + 8 * i + 16 * ((j >> 1) & 1);
+            const int cc = 8 * (j >> 2) - CL * CW + 2 * (lane & 3);
+            *reinterpret_cast<float2*>(buf + r * 32 + (cc ^ ((r & 7) << 2))) = make_float2(acc[i][j], acc[i][j + 1]);
         }
     }
     __syncwarp();
 #pragma unroll
     for (int c4 = 0; c4 < CW / 4; ++c4) {
         const float4 x = *reinterpret_cast<const float4*>(buf + lane * 32 + ((4 * c4) ^ ((lane & 7) << 2)));
-        v[4 * c4] = __float_as_uint(x.x); v[4 * c4 + 1] = __float_as_uint(x.y);
-        v[4 * c4 + 2] = __float_as_uint(x.z); v[4 * c4 + 3] = __float_as_uint(x.w);
+        v[4 * c4] = x.x; v[4 * c4 + 1] = x.y; v[4 * c4 + 2] = x.z; v[4 * c4 + 3] = x.w;
     }
 }
+
+// f(std::integral_constant<int, I>{}) for I = 0 .. N-1: the body sees its index as a compile-time constant.
+template <int N, int I = 0, typename F>
+__device__ __forceinline__ void static_for(F&& f) {
+    if constexpr (I < N) {
+        f(std::integral_constant<int, I>{});
+        static_for<N, I + 1>(f);
+    }
+}
+
+// One lane's fp64 GroupNorm running sums over N 32-column chunks of one image: chunk c is column n0 + (ch0 + c) * 32 + lane.
+// stats_quantize rounds a sum once per flush, so where a run ends is part of the result: a run ends when the image or the column
+// block changes, and at the end of the op.
+template <int N>
+struct StatRun {
+    double sum[N], sq[N];
+    int img = -1, n0 = -1;
+    __device__ __forceinline__ StatRun() { clear(); }
+    __device__ __forceinline__ void clear() {
+#pragma unroll
+        for (int c = 0; c < N; ++c) { sum[c] = 0.0; sq[c] = 0.0; }
+    }
+    __device__ __forceinline__ void flush(const GemmParams& p, const int ch0, const int lane) {
+        if (img >= 0 && img < p.OB) {
+#pragma unroll
+            for (int c = 0; c < N; ++c) {
+                const int n = n0 + (ch0 + c) * 32 + lane;
+                if (n < p.n_valid) {
+                    double* st = p.stats + (static_cast<long long>(img) * p.stats_C + p.stats_coff + n) * 2;
+                    red_add_f64_global(st, stats_quantize(sum[c]));
+                    red_add_f64_global(st + 1, stats_quantize(sq[c]));
+                }
+            }
+        }
+        clear();
+    }
+    // the next contributions belong to image `im`, column block `nb0`
+    __device__ __forceinline__ void start(const GemmParams& p, const int im, const int nb0, const int ch0, const int lane) {
+        if (im != img || nb0 != n0) { flush(p, ch0, lane); img = im; n0 = nb0; }
+    }
+    __device__ __forceinline__ void add(const int c, const double s, const double q) {
+#pragma unroll
+        for (int cc = 0; cc < N; ++cc)
+            if (cc == c) { sum[cc] += s; sq[cc] += q; }
+    }
+};
 
 // Persistent, warp-specialised tile loop (see the file header).  Two callers:
 //   MEGA = false: gemm_tile_kernel, one launch per layer; `p` lives in the kernel parameter space, barriers are set up here.
@@ -445,9 +489,9 @@ __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmPa
         const int g = warp >> 2;
         const int q = warp & 3;
         const int ew = warp;                                                // 0..7
-        const bool mma_wg = !SINGLE || g == 0;
-        const int own0 = SINGLE ? 0 : g * OWN;                              // items [own0, own1) are in this warpgroup's accumulator
-        const int own1 = SINGLE ? (g == 0 ? 1 : 0) : own0 + OWN;
+        const bool mma_wg = !SINGLE || g == 0;                              // (the warpgroups that hold items)
+        const int own0 = SINGLE ? 0 : g * OWN;                              // items [own0, own0 + OWN) are in this warpgroup's accumulator
+        const int ch0 = own0 % NCH;                                         // item own0 + ii = accumulator chunk ii = tile chunk ch0 + ii
         const int acc_half = MH == 2 ? g : 0;
         const int acc_c0 = (MH == 1 && !SINGLE) ? g * WN : 0;               // first accumulator column inside the tile
         const uint32_t out_smem = epi_base + ew * epi_warp_bytes;           // 4 KB
@@ -462,27 +506,9 @@ __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmPa
         float acc[2][WN / 2];
         int s = 0;                     // stage ring position
         uint32_t ph = 0;
-        // GroupNorm partial sums of this lane's column, kept in registers across tiles of the same (image, column block)
-        constexpr int NCHS = BLOCK_N >= 32 ? BLOCK_N / 32 : 1;
-        double st_sum[NCHS], st_sq[NCHS];
-#pragma unroll
-        for (int c = 0; c < NCHS; ++c) { st_sum[c] = 0.0; st_sq[c] = 0.0; }
-        int st_img = -1, st_n0 = -1;
-        auto flush_stats = [&]() {
-            if (st_img >= 0 && st_img < p.OB) {
-#pragma unroll
-                for (int c = 0; c < NCHS; ++c) {
-                    const int n = st_n0 + c * 32 + lane;
-                    if (n < p.n_valid) {
-                        double* st = p.stats + (static_cast<long long>(st_img) * p.stats_C + p.stats_coff + n) * 2;
-                        red_add_f64_global(st, stats_quantize(st_sum[c]));
-                        red_add_f64_global(st + 1, stats_quantize(st_sq[c]));
-                    }
-                }
-            }
-#pragma unroll
-            for (int c = 0; c < NCHS; ++c) { st_sum[c] = 0.0; st_sq[c] = 0.0; }
-        };
+        // GroupNorm partial sums of this lane's column in the warp's OWN chunks, kept across the tiles of one (image, column block).
+        // (All items of a warp's share of a tile lie in one image: a warp's 32 rows never straddle images.)
+        StatRun<OWN> st_own;
         for (int tile = tile_begin; tile < tile_end; ++tile) {
             int w0, h0, b0, n0, z;
             decode(tile, w0, h0, b0, n0, z);
@@ -502,27 +528,32 @@ __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmPa
                 mbar_arrive_expect_tx(res_bar(ew, b), 4096);
                 tma_load_5d(res_smem + b * 4096, &pm->res_map, res_bar(ew, b), n0 + ch * 32, w0 + sw, 0, h0 + sh, c4);
             };
-            const bool has_work = own0 < own1;
-            if (use_res_tma && has_work && lane == 0) request_resid(own0);     // overlaps the main loop
-            // bias (+ per-image FiLM bias) of this lane's column for every work item of this warp: fetched now (there is no L1, an
-            // L2 round trip per item would sit on the critical path), broadcast through smem when the item is processed
-            float bvs[OWN];
+            // bias (+ per-image FiLM bias) of this lane's column of an item
+            auto item_bias = [&](int item, int qq) {
+                float bv = 0.f;
+                const int half = item / NCH, ch = item % NCH;
+                const int img = b0 + ((half * 128 + qq * 32) >> (p.w_shift + p.h_shift));
+                const int n = n0 + ch * 32 + lane;
+                if (n < p.n_valid) {
+                    if (p.bias) bv += __ldg(&p.bias[n]);
+                    if (p.bias2) bv += __ldcg(&p.bias2[static_cast<long long>(img < p.OB ? img : 0) * p.bias2_stride + n]);   // written earlier in the same launch (step kernel): L2 only
+                }
+                return bv;
+            };
+            // where a (half, chunk) unit's rows sit in a split-K partial tile: laid out [chunk][j][row] so that the 32 lanes (consecutive
+            // rows) of one store / load instruction touch 512 contiguous bytes; WJ = float4 stride between the j-th and (j+1)-th quad of a row
+            constexpr int WJ = MH * 128;
+            auto ws_row = [&](int item, int qq) {
+                return (static_cast<long long>(item % NCH) * 8 * WJ + (item / NCH) * 128 + qq * 32 + lane) * 4;
+            };
+            if (use_res_tma && mma_wg && lane == 0) request_resid(own0);     // overlaps the main loop
+            // the bias of every item of this warp is fetched now (there is no L1, an L2 round trip per item would sit on the critical
+            // path) and broadcast through smem when the item is processed
+            float bvs[OWN] = {};
             if constexpr (BLOCK_N != 16) {
+                if (mma_wg) {
 #pragma unroll
-                for (int ii = 0; ii < OWN; ++ii) {
-                    const int item = own0 + ii;
-                    float bv = 0.f;
-                    if (item < own1) {
-                        const int half = item / NCH, ch = item % NCH;
-                        const int bb = (half * 128 + q * 32) >> (p.w_shift + p.h_shift);
-                        const int img = b0 + bb;
-                        const int n = n0 + ch * 32 + lane;
-                        if (n < p.n_valid) {
-                            if (p.bias) bv += __ldg(&p.bias[n]);
-                            if (p.bias2) bv += __ldcg(&p.bias2[static_cast<long long>(img < p.OB ? img : 0) * p.bias2_stride + n]);   // written earlier in the same launch (step kernel): L2 only
-                        }
-                    }
-                    bvs[ii] = bv;
+                    for (int ii = 0; ii < OWN; ++ii) bvs[ii] = item_bias(own0 + ii, q);
                 }
             }
             const int sp = tile % ksplit;
@@ -605,100 +636,37 @@ __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmPa
                 __syncwarp();
                 asm volatile("bar.sync 1, 256;" ::: "memory");
             }
-            const bool from_ws = (pass == 1);
             const bool to_ws = (ksplit > 1 && pass == 0);
-            // iteration space: pass 0 / no split -- this warpgroup's items, in this warp's quadrant;
-            // pass 1 -- units u = item * 4 + quadrant with u % ksplit == sp, dealt round-robin to the eight warps
-            const int it0 = from_ws ? sp + ksplit * ew : own0;
-            const int itn = from_ws ? NITEMS * 4 : own1;
-            const int its = from_ws ? ksplit * GEMM_EPI_WARPS : 1;
-#pragma unroll 1
-            for (int it = it0; it < itn; it += its) {
-                const int item = from_ws ? (it >> 2) : it;
-                const int qq = from_ws ? (it & 3) : q;
+            // the epilogue of one item (half, chunk) in quadrant qq: `fetch(v)` brings this lane's row of the item's 32x32 chunk (lane = row,
+            // v[j] = column j), which is then finished in place; `add_stats(cs, cq)` takes the GroupNorm sums of this lane's column
+            auto epi_item = [&](const int item, const int qq, const float bv, const bool last, auto&& fetch, auto&& add_stats) {
                 int half, ch, sw, sh, c4;
                 item_geom(item, qq, half, ch, sw, sh, c4);
-                const bool last_item = !from_ws && (item + 1 >= own1);
                 const int row = half * 128 + qq * 32 + lane;
                 const int w = row & (p.w_box - 1);
                 const int h = (row >> p.w_shift) & (p.h_box - 1);
                 const int bb = row >> (p.w_shift + p.h_shift);
                 const int ow = w0 + w, oh = h0 + h, img = b0 + bb;
                 const bool row_ok = (ow < p.OW) && (oh < p.OH) && (img < p.OB);
-                if (p.stats && !to_ws) {
-                    const int img0 = __shfl_sync(0xffffffffu, img, 0);      // all rows of a warp belong to one image
-                    if (img0 != st_img || n0 != st_n0) { flush_stats(); st_img = img0; st_n0 = n0; }
-                }
-                if (!from_ws && out_pending) {                 // the staging buffer is about to be overwritten by the transposition
-                    if (lane == 0) tma_store_wait_read<0>();
-                    __syncwarp();
-                }
-
+                float v[32];
                 if constexpr (BLOCK_N == 16) {
-                    uint32_t v[CW];
-                    acc_chunk_rows<WN, CW>(acc, 0, reinterpret_cast<float*>(out_ptr), v);
+                    fetch(v);
                     if (row_ok) {
                         float eps[4] = {0.f, 0.f, 0.f, 0.f};
-                        for (int c = 0; c < p.post.C; ++c) eps[c] = __uint_as_float(v[c]) + __ldg(&p.bias[c]);
+                        for (int c = 0; c < p.post.C; ++c) eps[c] = v[c] + __ldg(&p.bias[c]);
                         final_epilogue(p, eps, img, oh, ow);
                     }
                 } else {
                     const int nb = n0 + ch * 32;
-                    float bv = 0.f;
-                    if (from_ws) {
-                        const int n = nb + lane;
-                        if (n < p.n_valid) {
-                            if (p.bias) bv += __ldg(&p.bias[n]);
-                            if (p.bias2) {
-                                const int img0 = b0 + ((half * 128 + qq * 32) >> (p.w_shift + p.h_shift));
-                                bv += __ldcg(&p.bias2[static_cast<long long>(img0 < p.OB ? img0 : 0) * p.bias2_stride + n]);
-                            }
-                        }
-                    } else {
-#pragma unroll
-                        for (int ii = 0; ii < OWN; ++ii)
-                            if (item == own0 + ii) bv = bvs[ii];
-                    }
                     float* bs = bias_s + (ew * 2 + (bias_slot++ & 1u)) * 32;
                     bs[lane] = bv;
                     __syncwarp();
                     if (use_res_tma) {
                         ++res_count;                             // this item is residual request number res_count
-                        if (!last_item && lane == 0) request_resid(item + 1);   // other buffer: freed one item ago
+                        if (!last && lane == 0) request_resid(item + 1);   // other buffer: freed one item ago
                     }
-                    uint32_t v[32];
-                    // this thread's eight float4 inside a partial tile: laid out [chunk][j][row] so that the 32 lanes (consecutive rows)
-                    // of one store / load instruction touch 512 contiguous bytes
-                    const long long wrow = (static_cast<long long>(ch) * 8 * (MH * 128) + row) * 4;
-                    constexpr int WJ = MH * 128;                  // float4 stride between the j-th and (j+1)-th quad of a row
-                    if (!from_ws) {
-                        acc_chunk_rows<WN, CW>(acc, ch - acc_c0 / 32, reinterpret_cast<float*>(out_ptr), v);
-                        if (to_ws) {                             // split-K: park the partial sums
-                            float4* dst = reinterpret_cast<float4*>(p.ws + static_cast<long long>(tile) * SLICE + wrow);
-#pragma unroll
-                            for (int j = 0; j < 8; ++j)
-                                __stcg(dst + j * WJ, make_float4(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1]), __uint_as_float(v[4 * j + 2]),
-                                                            __uint_as_float(v[4 * j + 3])));
-                            continue;
-                        }
-                    } else {                                     // sum the ksplit partial tiles (L2 resident), split 0 first
-                        float acc_f[32];
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) acc_f[j] = 0.f;
-                        const float* src0 = p.ws + static_cast<long long>(tile - sp) * SLICE + wrow;
-                        for (int s2 = 0; s2 < ksplit; ++s2) {
-                            const float4* src = reinterpret_cast<const float4*>(src0 + s2 * SLICE);
-#pragma unroll
-                            for (int j = 0; j < 8; ++j) {
-                                const float4 r = __ldcg(src + j * WJ);
-                                acc_f[4 * j] += r.x; acc_f[4 * j + 1] += r.y; acc_f[4 * j + 2] += r.z; acc_f[4 * j + 3] += r.w;
-                            }
-                        }
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(acc_f[j]);
-                    }
+                    fetch(v);
                     const float ep_scale = p.scale;
-                    float f[32];
                     const bool full = (nb + 32 <= p.n_valid);
 #pragma unroll
                     for (int j4 = 0; j4 < 8; ++j4) {               // bias broadcast: 8 x LDS.128 (the slot is 128 B aligned)
@@ -707,9 +675,9 @@ __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmPa
 #pragma unroll
                         for (int jj = 0; jj < 4; ++jj) {
                             const int j = 4 * j4 + jj;
-                            float x = __uint_as_float(v[j]) * ep_scale + bb4[jj];
+                            float x = v[j] * ep_scale + bb4[jj];
                             if (!full && nb + j >= p.n_valid) x = 0.f;
-                            f[j] = x;
+                            v[j] = x;
                         }
                     }
                     if (use_res_tma) {
@@ -720,13 +688,13 @@ __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmPa
 #pragma unroll
                         for (int j = 0; j < 8; ++j) {
                             const float4 r = *reinterpret_cast<const float4*>(rp + ((j ^ (lane & 7)) << 4));
-                            f[4 * j] += r.x; f[4 * j + 1] += r.y; f[4 * j + 2] += r.z; f[4 * j + 3] += r.w;
+                            v[4 * j] += r.x; v[4 * j + 1] += r.y; v[4 * j + 2] += r.z; v[4 * j + 3] += r.w;
                         }
                         __syncwarp();                            // everyone is done with the buffer before it is re-requested
                     } else if (row_ok && p.resid) {
                         const long long ro = out_index(p.rs, z, img, oh, ow);
                         for (int j = 0; j < 32; ++j)
-                            if (nb + j < p.n_valid) f[j] += __ldcg(&p.resid[ro + nb + j]);
+                            if (nb + j < p.n_valid) v[j] += __ldcg(&p.resid[ro + nb + j]);
                     }
                     if (use_out_tma) {
                         if (out_pending) {                       // the previous bulk store must have finished reading the staging buffer
@@ -736,7 +704,7 @@ __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmPa
                         uint8_t* op = out_ptr + lane * 128;
 #pragma unroll
                         for (int j = 0; j < 8; ++j)
-                            *reinterpret_cast<float4*>(op + ((j ^ (lane & 7)) << 4)) = make_float4(f[4 * j], f[4 * j + 1], f[4 * j + 2], f[4 * j + 3]);
+                            *reinterpret_cast<float4*>(op + ((j ^ (lane & 7)) << 4)) = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
                         fence_proxy_async_smem();
                         __syncwarp();
                         if (lane == 0) {
@@ -750,10 +718,10 @@ __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmPa
                         if (full) {
                             float4* o4 = reinterpret_cast<float4*>(p.out_f32 + oo + nb);
 #pragma unroll
-                            for (int j = 0; j < 8; ++j) o4[j] = make_float4(f[4 * j], f[4 * j + 1], f[4 * j + 2], f[4 * j + 3]);
+                            for (int j = 0; j < 8; ++j) o4[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
                         } else {
                             for (int j = 0; j < 32; ++j)
-                                if (nb + j < p.n_valid) p.out_f32[oo + nb + j] = f[j];
+                                if (nb + j < p.n_valid) p.out_f32[oo + nb + j] = v[j];
                         }
                     }
                     if (p.out_t && nb >= p.t_col0) {
@@ -762,9 +730,9 @@ __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmPa
                                                 (img % p.t_per) * (p.OH * p.OW) + oh * p.OW + ow;
 #pragma unroll
                             for (int j = 0; j < 32; ++j) {                                                              // lanes = consecutive tokens
-                                const __nv_bfloat16 hi = __float2bfloat16_rn(f[j]);
+                                const __nv_bfloat16 hi = __float2bfloat16_rn(v[j]);
                                 tp[static_cast<long long>(j) * p.t_ld] = hi;
-                                if (p.lo_t_off) tp[static_cast<long long>(j) * p.t_ld + p.lo_t_off] = __float2bfloat16_rn(f[j] - __bfloat162float(hi));
+                                if (p.lo_t_off) tp[static_cast<long long>(j) * p.t_ld + p.lo_t_off] = __float2bfloat16_rn(v[j] - __bfloat162float(hi));
                             }
                         }
                     } else if (row_ok && p.out_bf16) {
@@ -773,10 +741,10 @@ __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmPa
                             uint4* o4 = reinterpret_cast<uint4*>(p.out_bf16 + ho + nb);
 #pragma unroll
                             for (int j = 0; j < 4; ++j) {
-                                __nv_bfloat162 h0v = __floats2bfloat162_rn(f[8 * j], f[8 * j + 1]);
-                                __nv_bfloat162 h1v = __floats2bfloat162_rn(f[8 * j + 2], f[8 * j + 3]);
-                                __nv_bfloat162 h2v = __floats2bfloat162_rn(f[8 * j + 4], f[8 * j + 5]);
-                                __nv_bfloat162 h3v = __floats2bfloat162_rn(f[8 * j + 6], f[8 * j + 7]);
+                                __nv_bfloat162 h0v = __floats2bfloat162_rn(v[8 * j], v[8 * j + 1]);
+                                __nv_bfloat162 h1v = __floats2bfloat162_rn(v[8 * j + 2], v[8 * j + 3]);
+                                __nv_bfloat162 h2v = __floats2bfloat162_rn(v[8 * j + 4], v[8 * j + 5]);
+                                __nv_bfloat162 h3v = __floats2bfloat162_rn(v[8 * j + 6], v[8 * j + 7]);
                                 uint4 uu;
                                 uu.x = *reinterpret_cast<uint32_t*>(&h0v); uu.y = *reinterpret_cast<uint32_t*>(&h1v);
                                 uu.z = *reinterpret_cast<uint32_t*>(&h2v); uu.w = *reinterpret_cast<uint32_t*>(&h3v);
@@ -784,7 +752,7 @@ __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmPa
                             }
                         } else {
                             for (int j = 0; j < 32; ++j)
-                                if (nb + j < p.n_valid) p.out_bf16[ho + nb + j] = __float2bfloat16_rn(f[j]);
+                                if (nb + j < p.n_valid) p.out_bf16[ho + nb + j] = __float2bfloat16_rn(v[j]);
                         }
                         if (p.lo_out_off) {                       // precise mode: low halves
                             __nv_bfloat16* lp = p.out_bf16 + ho + nb + p.lo_out_off;
@@ -794,7 +762,7 @@ __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmPa
                                 for (int j = 0; j < 4; ++j) {
                                     float r[8];
 #pragma unroll
-                                    for (int u = 0; u < 8; ++u) r[u] = f[8 * j + u] - __bfloat162float(__float2bfloat16_rn(f[8 * j + u]));
+                                    for (int u = 0; u < 8; ++u) r[u] = v[8 * j + u] - __bfloat162float(__float2bfloat16_rn(v[8 * j + u]));
                                     __nv_bfloat162 h0v = __floats2bfloat162_rn(r[0], r[1]), h1v = __floats2bfloat162_rn(r[2], r[3]);
                                     __nv_bfloat162 h2v = __floats2bfloat162_rn(r[4], r[5]), h3v = __floats2bfloat162_rn(r[6], r[7]);
                                     uint4 uu;
@@ -804,13 +772,11 @@ __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmPa
                                 }
                             } else {
                                 for (int j = 0; j < 32; ++j)
-                                    if (nb + j < p.n_valid) lp[j] = __float2bfloat16_rn(f[j] - __bfloat162float(__float2bfloat16_rn(f[j])));
+                                    if (nb + j < p.n_valid) lp[j] = __float2bfloat16_rn(v[j] - __bfloat162float(__float2bfloat16_rn(v[j])));
                             }
                         }
                     }
-                    // `!to_ws` always holds here (a split partial tile took the `continue` above); stating it saves ptxas one spilled
-                    // register in gemm_tile_kernel<64, 1>
-                    if (p.stats && !to_ws) {
+                    if (p.stats) {
                         double cs, cq;
                         if (use_out_tma) {
                             // the 32x32 tile sits in the (swizzled) staging buffer: lane c walks down column c -- conflict free, and a
@@ -849,21 +815,68 @@ __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmPa
                             float s2[32];
 #pragma unroll
                             for (int j = 0; j < 32; ++j) {
-                                const float x = row_ok ? f[j] : 0.f;
-                                f[j] = x; s2[j] = x * x;
+                                const float x = row_ok ? v[j] : 0.f;
+                                v[j] = x; s2[j] = x * x;
                             }
-                            cs = static_cast<double>(warp_column_sums(f));
+                            cs = static_cast<double>(warp_column_sums(v));
                             cq = static_cast<double>(warp_column_sums(s2));
                         }
-#pragma unroll
-                        for (int c = 0; c < NCHS; ++c)
-                            if (c == ch) { st_sum[c] += cs; st_sq[c] += cq; }
+                        add_stats(cs, cq);
                     }
                 }
-            }       // items
+            };
+            if (pass == 0) {
+                if (mma_wg) {
+                    if (p.stats && !to_ws) st_own.start(p, b0 + ((acc_half * 128 + q * 32) >> (p.w_shift + p.h_shift)), n0, ch0, lane);
+                    static_for<OWN>([&](auto ii_c) {             // compile-time ii: accumulator chunk ii is dead once it has been staged
+                        constexpr int ii = decltype(ii_c)::value;
+                        auto stage_acc = [&](float (&v)[32]) {
+                            if (out_pending) {                   // the staging buffer is about to be overwritten by the transposition
+                                if (lane == 0) tma_store_wait_read<0>();
+                                __syncwarp();
+                            }
+                            acc_chunk_rows<WN, CW, ii>(acc, reinterpret_cast<float*>(out_ptr), v);
+                        };
+                        if (to_ws) {                             // split-K: park the partial sums
+                            float v[32];
+                            stage_acc(v);
+                            float4* dst = reinterpret_cast<float4*>(p.ws + static_cast<long long>(tile) * SLICE + ws_row(own0 + ii, q));
+#pragma unroll
+                            for (int j = 0; j < 8; ++j) __stcg(dst + j * WJ, make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]));
+                        } else {
+                            epi_item(own0 + ii, q, bvs[ii], ii + 1 == OWN, stage_acc, [&](double cs, double cq) { st_own.add(ii, cs, cq); });
+                        }
+                    });
+                }
+            } else {
+                // units u = item * 4 + quadrant with u % ksplit == sp, dealt round-robin to the eight warps.  A split-K CTA owns exactly one
+                // (tile, split) pair, so the statistics run of its units ends with the tile.
+                StatRun<NCH> st_ws;
+#pragma unroll 1
+                for (int it = sp + ksplit * ew; it < NITEMS * 4; it += ksplit * GEMM_EPI_WARPS) {
+                    const int item = it >> 2, qq = it & 3;
+                    if (p.stats) st_ws.start(p, b0 + (((item / NCH) * 128 + qq * 32) >> (p.w_shift + p.h_shift)), n0, 0, lane);
+                    epi_item(item, qq, BLOCK_N != 16 ? item_bias(item, qq) : 0.f, true,
+                             [&](float (&v)[32]) {               // sum the ksplit partial tiles (L2 resident), split 0 first
+                                 const float* src0 = p.ws + static_cast<long long>(tile - sp) * SLICE + ws_row(item, qq);
+#pragma unroll
+                                 for (int j = 0; j < 32; ++j) v[j] = 0.f;
+                                 for (int s2 = 0; s2 < ksplit; ++s2) {
+                                     const float4* src = reinterpret_cast<const float4*>(src0 + s2 * SLICE);
+#pragma unroll
+                                     for (int j = 0; j < 8; ++j) {
+                                         const float4 r = __ldcg(src + j * WJ);
+                                         v[4 * j] += r.x; v[4 * j + 1] += r.y; v[4 * j + 2] += r.z; v[4 * j + 3] += r.w;
+                                     }
+                                 }
+                             },
+                             [&](double cs, double cq) { st_ws.add(item % NCH, cs, cq); });
+                }
+                if (p.stats) st_ws.flush(p, 0, lane);
+            }
             }       // pass
         }           // tiles
-        if (p.stats) flush_stats();
+        if (p.stats) st_own.flush(p, ch0, lane);
         if constexpr (MEGA) {
             // the consumer is a later op of the SAME launch (other CTAs, after a grid barrier): the bulk stores must be complete in
             // global memory, not merely done reading shared memory
