@@ -128,6 +128,7 @@ struct GemmDesc {
     long long lo_out_off = 0, lo_t_off = 0;
     // epilogue
     int mode = 0, OW = 0, OH = 1, OB = 1, n_valid = 0;
+    int out_imgs = 0;                             // images the fp32 output / residual tensors hold (0: at least every image the tiles cover)
     float scale = 1.f;
     const float* bias = nullptr; const float* bias2 = nullptr; int bias2_stride = 0;
     const float* resid = nullptr; OutSpec rs{};
@@ -383,7 +384,7 @@ Op make_gemm_op(const GemmDesc& d, DevAllocs& mem, sr3_gemm_geometry* geo = null
         auto mk = [&](const float* ptr, const OutSpec& o, bool& c4z) {
             c4z = (o.sB == 0 && o.sZ != 0);
             const long long s4 = c4z ? o.sZ : o.sB;
-            const uint64_t n4 = c4z ? (uint64_t)d.nz : (uint64_t)(d.tiles_b * d.b_box > d.OB ? d.tiles_b * d.b_box : d.OB);
+            const uint64_t n4 = c4z ? (uint64_t)d.nz : d.out_imgs ? (uint64_t)d.out_imgs : (uint64_t)(d.tiles_b * d.b_box > d.OB ? d.tiles_b * d.b_box : d.OB);
             uint64_t dims[5] = {(uint64_t)d.n_valid, (uint64_t)d.OW, 1ull, (uint64_t)d.OH, n4};
             uint64_t str[4];
             str[0] = (uint64_t)o.sW * 4;
@@ -504,11 +505,12 @@ int pick_block_n(int cout);
 // The tile shape (rows x BLOCK_N) and the split-K factor are chosen by a byte model of the per-CTA critical path: a CTA ingests
 // stages x (A box + B boxes) through TMA at a fixed rate, runs ceil(tiles * split / SMs) waves, and a split tile costs an extra
 // partial-tile store + reload + a grid-level handshake (tools/gpu_splitk_sweep.py sweeps the choices on a device).
-void conv_geometry(GemmDesc& d, int OW, int OH, int Bp, int cout, bool has_resid = false, int nz = 1) {
+// Bt: images the tiles must cover (tiles_b = ceil(Bt / b_box); images past the A tensor's batch load as zeros).
+void conv_geometry(GemmDesc& d, int OW, int OH, int Bt, int cout, bool has_resid = false, int nz = 1) {
     const int npass = d.passes > 1 ? d.passes : 1;
     bool tall_ok = OW >= 8 && OH >= 16, has3 = false;
     for (const KSlab& k : d.slabs) { if (k.p != 0) tall_ok = false; if (k.dh != 0) has3 = true; }
-    tall_ok = tall_ok && has3 && (OH >= 32 || Bp % 2 == 0);
+    tall_ok = tall_ok && has3 && (OH >= 32 || Bt % 2 == 0);
     const int sms = num_sms();
     // cost in bytes of the slowest CTA; `split` returns the factor the cost was computed for
     auto model = [&](long long tiles, int nstage, long long stage_bytes, int rows, int bn, int& split) -> double {
@@ -555,7 +557,7 @@ void conv_geometry(GemmDesc& d, int OW, int OH, int Bp, int cout, bool has_resid
                 const Cand& c = cands[i];
                 if (cout % c.bn != 0) continue;
                 int hb, bb; geom(c.mh, hb, bb);
-                const long long tiles = (long long)(OW / 8) * (OH / hb) * (Bp / bb) * (cout / c.bn) * nz;
+                const long long tiles = (long long)(OW / 8) * (OH / hb) * ((Bt + bb - 1) / bb) * (cout / c.bn) * nz;
                 const long long stage_bytes = (c.mh == 2 ? 36864 : 18432) + 3ll * c.bn * 128;
                 int sp = 1;
                 const double cost = model(tiles, nstage * npass, stage_bytes, c.mh * 128, c.bn, sp);
@@ -577,7 +579,7 @@ void conv_geometry(GemmDesc& d, int OW, int OH, int Bp, int cout, bool has_resid
         d.tall = 0; d.mh = 1;
         pick_image_box(OW, OH, d.w_box, d.h_box, d.b_box);
         d.block_n = pick_block_n(cout);
-        const long long mt = (long long)(OW / d.w_box) * (OH / d.h_box) * (Bp / d.b_box) * nz;
+        const long long mt = (long long)(OW / d.w_box) * ((OH + d.h_box - 1) / d.h_box) * ((Bt + d.b_box - 1) / d.b_box) * nz;
         if (getenv("SR3_BLOCK_N") == nullptr && cout % 32 == 0) {
             // generic stages group up to three K slabs (one A box + one B box each)
             const int nstage = (((int)d.slabs.size() + 2) / 3) * npass;
@@ -592,13 +594,16 @@ void conv_geometry(GemmDesc& d, int OW, int OH, int Bp, int cout, bool has_resid
         }
     }
     if (const char* e = getenv("SR3_KSPLIT")) d.ksplit_max = atoi(e);
-    d.tiles_w = OW / d.w_box; d.tiles_h = OH / d.h_box; d.tiles_b = Bp / d.b_box;
+    d.tiles_w = OW / d.w_box; d.tiles_h = (OH + d.h_box - 1) / d.h_box; d.tiles_b = (Bt + d.b_box - 1) / d.b_box;
 }
 
+// An image of fewer than 32 pixels (4x4) gets a patch padded to 32 rows (4 x 8: rows 4..7 lie outside the image, TMA loads them as zeros
+// and the epilogue masks them), so that a warp's 32 rows still hold one image: its FiLM bias, GroupNorm run and TMA boxes stay per image.
 void pick_image_box(int W, int H, int& w_box, int& h_box, int& b_box) {
     w_box = W < 16 ? W : 16;
     h_box = 128 / w_box;
     if (h_box > H) h_box = H;
+    if (w_box * h_box < 32) h_box = 32 / w_box;
     b_box = 128 / (w_box * h_box);
 }
 
@@ -668,9 +673,9 @@ struct ConvArgs {
     int c0 = 0, c1 = 0;               // channels of the A sources (precise mode: where their low halves start)
 };
 
-// Tile-kernel descriptor of an image conv over B images (Bp allocated, B <= Bp); PW = 2 in precise mode ([hi | lo] operand pairs).
-// The engine's layer builders and the stand-alone test hook both go through here.
-GemmDesc conv_desc(const ConvArgs& c, int B, int Bp, int PW) {
+// Tile-kernel descriptor of an image conv over B images whose tiles cover Bt >= B images (conv_geometry); PW = 2 in precise mode
+// ([hi | lo] operand pairs).  The engine's layer builders and the stand-alone test hook both go through here.
+GemmDesc conv_desc(const ConvArgs& c, int B, int Bt, int PW) {
     GemmDesc d;
     d.n_a = c.n_a; d.a[0] = c.a[0]; d.a[1] = c.a[1];
     d.slabs = c.slabs;
@@ -678,7 +683,7 @@ GemmDesc conv_desc(const ConvArgs& c, int B, int Bp, int PW) {
     // the bf16 store addresses plain NHWC rows: it has no phase offsets (z_off_*) and no custom output map
     REQUIRE(!(c.raw_out && c.custom_os), "a bf16 copy of a phase-addressed (folded upsample) output is not supported");
     if (PW == 2) set_precise_fields(d, c.c0, c.c1, c.ktot);
-    conv_geometry(d, c.OW, c.OH, Bp, c.cout, c.resid != nullptr, c.nz);
+    conv_geometry(d, c.OW, c.OH, Bt, c.cout, c.resid != nullptr, c.nz);
     d.b_ptr = c.w; d.b_K = PW * c.ktot; d.b_rows = (long long)c.nz * (((c.cout + 127) / 128) * 128);      // weights are padded to 128 rows (new_weight)
     d.b_is_param = true;
     d.n_tiles = (c.cout + d.block_n - 1) / d.block_n; d.nz = c.nz; d.a_zstep = 0; d.b_zrows = c.b_zrows;
@@ -732,8 +737,11 @@ struct WgradOut { float* ptr = nullptr; long long slice_stride = 0, row_stride =
 
 // Grid of the weight gradient of one conv: x = (co_pad / 128) * (Cin / 64) output tiles, y = groups of <= 3 taps, z = slices of the
 // nbatch * (OH/8) * (OW/8) pixel patches.  slices = 0: the default (one wave of CTAs); raw: one slice per batch.
+// A 4x4 image is one patch: its other 48 pixels lie outside dY and load as zeros, so they add nothing.
 struct WgradShape { int co_pad = 0, tpc = 0, nx = 0, ny = 0, patches = 0, slices = 0; };
+int wgrad_grid(int extent) { return extent == 4 ? 8 : extent; }      // pixels of the patch grid along one side
 WgradShape wgrad_shape(int CY, int OHh, int OWw, int nbatch, int Cin, int ntaps, int slices, const WgradOut* raw) {
+    OHh = wgrad_grid(OHh); OWw = wgrad_grid(OWw);
     REQUIRE(OHh % 8 == 0 && OWw % 8 == 0 && Cin % 64 == 0 && CY % 64 == 0, "wgrad geometry %dx%d Cin=%d CY=%d", OHh, OWw, Cin, CY);
     REQUIRE(ntaps >= 1 && ntaps <= WGRAD_MAX_TAPS, "too many taps");
     WgradShape s;
@@ -777,7 +785,7 @@ WgradParams wgrad_params(const WgradShape& s, const bf16* dy, int CY, int OHh, i
     }
     p.ws = ws; p.Cin = Cin; p.co_pad = s.co_pad; p.cout_valid = cout_valid;
     p.ws_slice_stride = raw ? raw->slice_stride : (long long)s.co_pad * ntaps * Cin; p.ws_row_stride = raw ? raw->row_stride : (long long)ntaps * Cin;
-    p.OH = OHh; p.OW = OWw; p.B = nbatch; p.ntaps = ntaps; p.taps_per_cta = s.tpc; p.patches = s.patches; p.slices = s.slices;
+    p.OH = wgrad_grid(OHh); p.OW = wgrad_grid(OWw); p.B = nbatch; p.ntaps = ntaps; p.taps_per_cta = s.tpc; p.patches = s.patches; p.slices = s.slices;
     for (int i = 0; i < ntaps; ++i) p.taps[i] = taps[i];
     return p;
 }
@@ -803,7 +811,9 @@ void init_wgrad_attrs() {
 
 struct sr3_engine {
     sr3_unet_config cfg{};
-    int B = 0, Bp = 0, dev = 0;
+    // Bp: images allocated per activation.  Bt: images the tile-kernel launches cover (Bp, or B when Bp was padded to 8 for a 4x4 level:
+    // the high-resolution layers then do not compute the padded images).
+    int B = 0, Bp = 0, Bt = 0, dev = 0;
     int H = 0, W = 0, inner = 0, cond_c = 0, in_C = 64;
     bool precise = false; int PW = 1;       // precise mode: every bf16 operand tensor is PW = 2 times as wide ([hi | lo] per pixel / row)
     DevAllocs mem;
@@ -1035,7 +1045,7 @@ struct sr3_engine {
 
     void add_conv(const ConvArgs& c) {
         if (dry) return;
-        push_gemm(conv_desc(c, B, Bp, PW));
+        push_gemm(conv_desc(c, B, Bt, PW));
     }
 
     // ResnetBlock (+ optional SelfAttention): reference unet.py:94-158
@@ -1121,11 +1131,11 @@ struct sr3_engine {
     Act add_attention(const LayerSpec& L, const Act& x, bf16* raw_out = nullptr) {
         const int C = x.C, Hh = x.H, Ww = x.W, HW = Hh * Ww, G = cfg.norm_groups;
         const std::string p = L.name + ".attn";
-        const int Lt = HW >= 128 ? HW : 128;            // tokens per attention batch (two 8x8 images share one)
+        const int Lt = HW >= 128 ? HW : 128;            // tokens per attention batch (two 8x8 or eight 4x4 images share one)
         const int per = Lt / HW;                         // images per attention batch
         REQUIRE(Lt % 128 == 0 && (Bp % per) == 0, "attention geometry HW=%d", HW);
         REQUIRE(C % 128 == 0, "%s: self-attention over %d channels is not supported (the q/k/v and P.v tiles are 128 columns wide; C must be a multiple of 128)", L.name.c_str(), C);
-        const int nz = Bp / per;
+        const int nz = (Bt + per - 1) / per;
         float* gn_w = f32_param(p + ".norm.weight", {C});
         float* gn_b = f32_param(p + ".norm.bias", {C});
         bf16* wqkv = new_weight(3 * C, C);
@@ -1153,7 +1163,7 @@ struct sr3_engine {
             const int ncol = 3 * C;
             d.block_n = 128; d.b_ptr = wqkv; d.b_K = C * PW; d.b_rows = ncol; d.b_is_param = true;
             pick_image_box(Ww, Hh, d.w_box, d.h_box, d.b_box);
-            d.tiles_w = Ww / d.w_box; d.tiles_h = Hh / d.h_box; d.tiles_b = Bp / d.b_box; d.n_tiles = ncol / 128;
+            d.tiles_w = Ww / d.w_box; d.tiles_h = (Hh + d.h_box - 1) / d.h_box; d.tiles_b = (Bt + d.b_box - 1) / d.b_box; d.n_tiles = ncol / 128;
             d.OW = Ww; d.OH = Hh; d.OB = Bp; d.n_valid = ncol;
             d.out_bf16 = qk; d.hs = nhwc_out(Hh, Ww, 2 * C * PW); d.lo_out_off = precise ? 2 * C : 0;      // rows [q_hi | k_hi | q_lo | k_lo]
             d.out_t = vT; d.t_col0 = 2 * C; d.t_rows = C; d.t_ld = Lt * PW; d.t_per = per; d.lo_t_off = precise ? Lt : 0;
@@ -1245,9 +1255,6 @@ struct sr3_engine {
         int F_total = 0;
         for (auto* v : {&downs, &mid, &ups}) for (auto& L : *v) if (L.kind == 1) F_total += L.cout;
         F = F_total;
-        int min_res = cfg.image_size;
-        for (int i = 1; i < cfg.n_mults; ++i) min_res /= 2;
-        REQUIRE(min_res >= 8, "lowest UNet resolution %d < 8 is not supported", min_res);
         if (train) {
             fin_bias_sum = new_zero(4); dfilm = new_zero((size_t)Bp * F); dtau = new_zero((size_t)Bp * inner);
             if (!dry) {
@@ -1376,7 +1383,7 @@ struct sr3_engine {
                 GemmDesc d; d.n_a = 1; d.a[0] = nhwc_src(a, Bp, H, W, C * PW);
                 add_conv_slabs(d.slabs, 0, C, 3, 1, 0);
                 set_precise(d, C, 0, 9 * C);
-                conv_geometry(d, W, H, Bp, 16);
+                conv_geometry(d, W, H, Bt, 16);
                 d.block_n = 16; d.b_ptr = w; d.b_K = 9 * C * PW; d.b_rows = 128; d.n_tiles = 1; d.b_is_param = true;
                 d.mode = 1; d.OW = W; d.OH = H; d.OB = B; d.n_valid = co; d.bias = b; d.ctl = ctl_dev;
                 d.post.tab = post_tab; d.post.T = T_cap; d.post.H = H; d.post.W = W; d.post.C = co;
@@ -1406,7 +1413,14 @@ struct sr3_engine {
         REQUIRE(cfg.precision == 0 || cfg.precision == 1, "precision must be 0 (bf16) or 1 (precise)");
         precise = cfg.precision == 1; PW = precise ? 2 : 1;
         cond_c = cfg.conditional ? cfg.in_channel - cfg.channels : 0;
-        Bp = (B + 1) & ~1;                         // 8x8 levels tile two images per CTA
+        int min_res = cfg.image_size;
+        for (int i = 1; i < cfg.n_mults; ++i) min_res /= 2;
+        REQUIRE(min_res >= 4, "lowest UNet resolution %d < 4 is not supported", min_res);
+        // 8x8 levels tile two images per CTA.  A 4x4 level tiles four, and its attention batches hold eight 16-token images, which
+        // read (P = 0 makes them inert, but they must be finite) every image slot of their batch: Bp is a multiple of 8, and the
+        // slots no layer writes hold the zeros of the allocation (or, in shared scratch, another layer's finite values).
+        Bp = min_res == 4 ? (B + 7) & ~7 : (B + 1) & ~1;
+        Bt = min_res == 4 ? B : Bp;
         T_cap = 4096;
         REQUIRE(!(train && precise), "the training plan supports the bf16 precision only");
         // pass 1: sizes
@@ -2139,8 +2153,8 @@ int sr3_test_conv_ex(const sr3_test_conv_args* a, sr3_gemm_geometry* geometry, v
     c.bias = a->bias; c.bias2 = a->bias2; c.bias2_stride = Cout; c.resid = a->resid;
     c.out.p = a->y; c.out.stats = a->stats;
     c.raw_out = static_cast<bf16*>(a->y_bf16);
-    const GemmDesc d = conv_desc(c, B, B, PW);
-    REQUIRE(B % d.b_box == 0, "batch must be a multiple of %d at this resolution", d.b_box);
+    GemmDesc d = conv_desc(c, B, B, PW);
+    d.out_imgs = B;          // the last tile may cover images past B: they load as zeros and are not stored
     Op op = make_gemm_op(d, mem, geometry);
     op(st);
     CK(cudaStreamSynchronize(st));

@@ -33,7 +33,7 @@ struct WgradParams {
     CUtensorMap x_map;       // 5-D bf16 view of X, box {64, 8, 1, 8, 1}
     float* ws;               // partial tiles: ws[slice * ws_slice_stride + co * ws_row_stride + tap * Cin + ci]  (default [slices][co_pad][ntaps][Cin])
     long long ws_slice_stride, ws_row_stride;
-    int Cin, co_pad, cout_valid, OH, OW, B;
+    int Cin, co_pad, cout_valid, OH, OW, B;   // OH, OW: the patch grid in pixels (8 for a 4x4 output: one patch, zero outside the image)
     int ntaps, taps_per_cta;
     int patches;             // B * (OH/8) * (OW/8)
     int slices;

@@ -49,6 +49,8 @@ int sr3_abi_version(void);
 
 /* UNet.__init__ (model/sr3_modules/unet.py:161-233) + GaussianDiffusion.__init__ (diffusion.py:64-82):
  * builds the layer plan, allocates activations / packed weights on `device` for a fixed batch size.
+ * The lowest UNet level (image_size / 2^(n_mults - 1)) must be at least 4x4; a net with a 4x4 level allocates its activations for the batch
+ * rounded up to 8 images, but launches the work of the real images only.
  * Threading: calls on one engine must be serialised by the caller.  Kernels whose CTAs wait for partners are safe next to other work on the
  * device: the split-K partners of a tile are one thread-block cluster (gang-scheduled by the hardware), the persistent step kernel (SR3_MEGA=1)
  * is a cooperative launch -- engines driven concurrently from different streams of one device cannot deadlock each other. */
