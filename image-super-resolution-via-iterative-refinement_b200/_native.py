@@ -91,6 +91,7 @@ _SIGS = {
     "sr3_test_conv": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
                               c_void_p]),
     "sr3_test_conv_ex": (c_int, [POINTER(TestConvArgsC), POINTER(GemmGeometryC), c_void_p]),
+    "sr3_tile_schedule": (c_int, [c_void_p, c_int, POINTER(GemmGeometryC), POINTER(c_int), POINTER(c_int)]),
     "sr3_test_wgrad": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float,
                                c_int, POINTER(c_int), c_void_p]),
 }
@@ -398,6 +399,11 @@ class Engine:
             _check(lib().sr3_engine_profile_step(self._h, int(t), int(reps), cap, kinds, ms, fl, by, ctypes.byref(n), _stream()))
         return [(kinds[i], ms[i], fl[i], by[i]) for i in range(n.value)]
 
+    def tile_schedules(self):
+        """Per op of the eager step (the order of profile_step): None for an op that is not a tile-kernel launch, else its geometry dict
+        plus "schedule" ("cooperative" / "pingpong") and "out_hwc" (output rows, columns, channels)."""
+        return [_tile_schedule(self._h, i) for i in range(lib().sr3_engine_num_ops_per_step(self._h))]
+
     def launches_per_step(self):
         return lib().sr3_engine_num_launches_per_step(self._h)
 
@@ -487,6 +493,25 @@ def test_conv_ex(x, w, ksize=3, stride=1, bias=None, bias2=None, resid=None, x2=
     geo = GemmGeometryC()
     _check(lib().sr3_test_conv_ex(ctypes.byref(a), ctypes.byref(geo), _stream()))
     return y, yb, stats, {n: getattr(geo, n) for n, _ in GemmGeometryC._fields_}
+
+
+SCHEDULES = {0: "cooperative", 1: "pingpong"}
+
+
+def _tile_schedule(handle, op):
+    geo, sch, hwc = GemmGeometryC(), c_int(), (c_int * 3)()
+    _check(lib().sr3_tile_schedule(handle, int(op), ctypes.byref(geo), ctypes.byref(sch), hwc))
+    if sch.value < 0:
+        return None
+    d = {n: getattr(geo, n) for n, _ in GemmGeometryC._fields_}
+    d["schedule"] = SCHEDULES[sch.value]
+    d["out_hwc"] = tuple(hwc)
+    return d
+
+
+def last_test_conv_schedule():
+    """Geometry dict + "schedule" + "out_hwc" of the most recent test_conv_ex call on this thread."""
+    return _tile_schedule(None, 0)
 
 
 def test_wgrad(dy, x, ksize, stride=1, cout_valid=None, cin_valid=None, slices=0, gscale=1.0, raw=False):

@@ -116,6 +116,7 @@ struct GemmDesc {
     int block_n = 128;
     int w_box = 16, h_box = 8, b_box = 1;         // output pixel patch of one tile (mh * 128 rows)
     int mh = 1;                                   // 128-row accumulator halves per tile
+    int pingpong = 0;                             // 1: ping-pong schedule (each consumer warpgroup owns whole tiles; never split)
     int tall = 0;                                 // 3x3 stride-1 "tall halo" mode: A box = 8 x (rows + 2) pixels, vertical taps share it
     int a_box_w = 0, a_box_h = 0, a_box_b = 0;    // TMA box of the A operand (0: same as the tile patch)
     int a_half_off = 0;
@@ -191,9 +192,10 @@ void launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cuda
 // by construction -- no assumption about what else occupies the device (other engines / streams, NCCL, library kernels), inside or outside
 // graph capture, and the launch keeps its programmatic-dependent-launch edge.
 constexpr int MAX_CLUSTER_SPLIT = 8;               // portable cluster size limit
-template <int BN, int MH>
+template <int BN, int MH, bool PP = false>
 void launch_gemm_bn(const GemmParams& p, dim3 grid, int smem, cudaStream_t st) {
-    if (p.ksplit == 1) { launch_k(gemm_tile_kernel<BN, MH>, grid, dim3(GEMM_THREADS), (size_t)smem, st, p); return; }
+    if (p.ksplit == 1) { launch_k(gemm_tile_kernel<BN, MH, PP>, grid, dim3(GEMM_THREADS), (size_t)smem, st, p); return; }
+    REQUIRE(!PP, "a ping-pong tile launch cannot be split");
     REQUIRE(p.ksplit <= MAX_CLUSTER_SPLIT && grid.x % p.ksplit == 0, "split-K factor %d does not form clusters of grid %u", p.ksplit, grid.x);
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = grid; cfg.blockDim = dim3(GEMM_THREADS); cfg.dynamicSmemBytes = (size_t)smem; cfg.stream = st;
@@ -216,6 +218,9 @@ void init_gemm_attrs() {
     CK(cudaFuncSetAttribute(gemm_tile_kernel<128, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT));
     CK(cudaFuncSetAttribute(gemm_tile_kernel<128, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT));
     CK(cudaFuncSetAttribute(gemm_tile_kernel<256, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT));
+    CK(cudaFuncSetAttribute(gemm_tile_kernel<64, 2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT));
+    CK(cudaFuncSetAttribute(gemm_tile_kernel<64, 1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT));
+    CK(cudaFuncSetAttribute(gemm_tile_kernel<128, 1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT));
 }
 
 // How many clusters of `c` tile-kernel CTAs (one CTA per SM: they use the whole shared memory) the device holds at once; a cluster lives
@@ -279,10 +284,13 @@ void mega_record(int type, const T& params) {
     g_mega_registry->push_back(std::move(r));
 }
 static thread_local std::vector<GemmHandle>* g_gemm_registry = nullptr;   // set by the engine while it builds its plan
+// what the most recent sr3_test_conv_ex of this thread launched (sr3_tile_schedule with no engine)
+struct LastTestConv { sr3_gemm_geometry geo{}; int schedule = -1; int out_hwc[3] = {0, 0, 0}; };
+static thread_local LastTestConv g_last_test_conv;
 
-// Turns a GemmDesc into a launchable op (encodes the TMA maps, uploads the K-slab table).  `geo` (optional) receives the variant and
-// launch shape that were actually chosen, after every host-side override and cap.
-Op make_gemm_op(const GemmDesc& d, DevAllocs& mem, sr3_gemm_geometry* geo = nullptr) {
+// Turns a GemmDesc into a launchable op (encodes the TMA maps, uploads the K-slab table).  `geo` / `schedule` (optional) receive the variant,
+// launch shape and schedule (0 cooperative, 1 ping-pong) that were actually chosen, after every host-side override and cap.
+Op make_gemm_op(const GemmDesc& d, DevAllocs& mem, sr3_gemm_geometry* geo = nullptr, int* schedule = nullptr) {
     REQUIRE(d.w_box * d.h_box * d.b_box == 128 * d.mh, "tile box must cover %d rows", 128 * d.mh);
     REQUIRE(!d.slabs.empty(), "gemm without K slabs");
     GemmParams p;
@@ -416,7 +424,7 @@ Op make_gemm_op(const GemmDesc& d, DevAllocs& mem, sr3_gemm_geometry* geo = null
     {
         const int tiles = d.tiles_w * d.tiles_h * d.tiles_b * d.n_tiles * d.nz;
         const int ks = d.ksplit_max;
-        if (ks > 1 && d.mode == 0 && d.out_f32 && d.block_n >= 32 && d.n_valid % 32 == 0) {
+        if (ks > 1 && !d.pingpong && d.mode == 0 && d.out_f32 && d.block_n >= 32 && d.n_valid % 32 == 0) {
             int want = num_sms() / tiles;                  // CTAs per tile that still fit one wave
             if (want > ks) want = ks;
             if (want > p.num_k * d.passes / 2) want = p.num_k * d.passes / 2;    // at least two stages per slice
@@ -444,21 +452,30 @@ Op make_gemm_op(const GemmDesc& d, DevAllocs& mem, sr3_gemm_geometry* geo = null
     REQUIRE(smem <= SMEM_LIMIT, "gemm shared memory %d exceeds the limit", smem);
     init_gemm_attrs();
     REQUIRE((bn == 16 || bn == 32 || bn == 64 || bn == 128 || bn == 256) && (mh == 1 || (mh == 2 && bn <= 128 && bn != 32)), "unsupported tile %dx%d", 128 * mh, bn);
+    const bool pp = d.pingpong != 0;
+    REQUIRE(!pp || (gemm_pingpong_ok(bn, mh) && p.ksplit == 1 && d.mode == 0), "no ping-pong form of tile %dx%d (split %d)", 128 * mh, bn, p.ksplit);
     if (geo) {
         geo->tall = d.tall; geo->mh = mh; geo->block_n = bn; geo->h_box = d.h_box; geo->b_box = d.b_box;
         geo->ksplit = p.ksplit; geo->stages = p.stages; geo->ctas = ctas; geo->tiles = total_tiles / p.ksplit; geo->res_smem = res_smem ? 1 : 0;
     }
+    if (schedule) *schedule = pp ? 1 : 0;
     std::shared_ptr<GemmParams> sp = std::make_shared<GemmParams>(p);
     if (g_gemm_registry) {
         GemmHandle h; h.p = sp; h.w_ptr = d.b_ptr; h.w_bytes = 2LL * d.b_rows * d.b_K; h.w_is_param = d.b_is_param; h.bn = bn; h.mh = mh;
         g_gemm_registry->push_back(h);
     }
     if (g_mega_registry) {
-        MegaRec r; r.type = MOP_GEMM; r.variant = bn | (mh << 16); r.gp = sp;
+        MegaRec r; r.type = MOP_GEMM; r.variant = bn | (mh << 16) | (pp ? MEGA_VARIANT_PP : 0); r.gp = sp;
         g_mega_registry->push_back(std::move(r));
     }
-    return [sp, grid, bn, mh, smem](cudaStream_t st) {
+    return [sp, grid, bn, mh, pp, smem](cudaStream_t st) {
         const GemmParams& p = *sp;
+        if (pp) {
+            if (mh == 2) launch_gemm_bn<64, 2, true>(p, grid, smem, st);
+            else if (bn == 64) launch_gemm_bn<64, 1, true>(p, grid, smem, st);
+            else launch_gemm_bn<128, 1, true>(p, grid, smem, st);
+            return;
+        }
         switch (bn) {
             case 16: if (mh == 2) launch_gemm_bn<16, 2>(p, grid, smem, st); else launch_gemm_bn<16, 1>(p, grid, smem, st); break;
             case 32: launch_gemm_bn<32, 1>(p, grid, smem, st); break;
@@ -500,6 +517,11 @@ Op make_attn_op(const bf16* qk, const bf16* vT, bf16* out, int nz, int Lt, int H
 
 void pick_image_box(int W, int H, int& w_box, int& h_box, int& b_box);
 int pick_block_n(int cout);
+// SR3_PINGPONG: -1 unset (the byte model chooses the schedule), 0 cooperative only, 1 ping-pong wherever the tile shape has that form
+int pingpong_knob() {
+    const char* e = getenv("SR3_PINGPONG");
+    return e ? (atoi(e) != 0 ? 1 : 0) : -1;
+}
 
 // Geometry of an image conv: the "tall halo" form for 3x3 stride-1 convs at >= 16x16, else a plain 128-pixel patch per tap.
 // The tile shape (rows x BLOCK_N) and the split-K factor are chosen by a byte model of the per-CTA critical path: a CTA ingests
@@ -512,8 +534,41 @@ void conv_geometry(GemmDesc& d, int OW, int OH, int Bt, int cout, bool has_resid
     for (const KSlab& k : d.slabs) { if (k.p != 0) tall_ok = false; if (k.dh != 0) has3 = true; }
     tall_ok = tall_ok && has3 && (OH >= 32 || Bt % 2 == 0);
     const int sms = num_sms();
-    // cost in bytes of the slowest CTA; `split` returns the factor the cost was computed for
-    auto model = [&](long long tiles, int nstage, long long stage_bytes, int rows, int bn, int& split) -> double {
+    // Schedule.  SR3_PINGPONG (tests / A-B timing): 1 = ping-pong wherever the tile shape has that form (the model ranks the ping-pong
+    // shapes), 0 = cooperative everywhere; a tile forced by SR3_TALL_BN / SR3_TALL_MH / SR3_BLOCK_N keeps the forced shape and, unless
+    // SR3_PINGPONG=1, the cooperative form.  Unset: the best cooperative tile, charged its exposed epilogue (coop_epi), against the 128x64
+    // ping-pong tile.  That is the only ping-pong shape the model offers: its whole-tile accumulator is 64 registers, while the 256x64 and
+    // 128x128 forms hold 128 registers through the epilogue under the 168-register cap of 288 threads, spill ~15x more and measured slower
+    // than cooperative at every shape of the 16->128 step (DESIGN.md section 8).
+    const int pp_knob = pingpong_knob();
+    const bool pp_force = pp_knob == 1, pp_auto = pp_knob < 0;
+    const bool shape_forced = getenv("SR3_TALL_BN") || getenv("SR3_TALL_MH") || getenv("SR3_BLOCK_N");
+    // Epilogue of one 32x32 output item of a warp (transposition, bias / FiLM, residual, TMA store, bf16 copy, GroupNorm sums) in bytes of
+    // TMA ingest at the ~47 B/clk/SM of the model (~3200 clocks) with two epilogue warps per SM sub-partition (cooperative); a ping-pong
+    // warpgroup's four warps have a sub-partition each and take half that per item.  Calibrated with tools/gpu_layer_profile.py on the
+    // 16->128 step at B = 16 (H100, DESIGN.md section 8): the 128x64 ping-pong tile, with twice the weight ingest per row of a 256-row tile,
+    // was faster on the 3x3 convs at 128x128 (15.5 tiles per CTA against cooperative 256x64 at 7.8) and 64x64 (7.8 tiles against 256x128
+    // at 1.9 and 256x64 at 3.9) and slower on the 32x32 convs with a residual (3.9 tiles against 256x64 at 1.9): the model orders those
+    // cases the same way for 137 K < EPI_ITEM_BYTES < 168 K.  So the epilogue, not TMA ingest, bounds these tiles.
+    constexpr double EPI_ITEM_BYTES = 150000.0;
+    // cost in bytes of the slowest CTA; `split` returns the factor the cost was computed for.  pp: the ping-pong schedule (never split):
+    // a warpgroup's epilogue (all MH x NCH items of the tile on its 4 warps) runs under the other warpgroup's MMAs, so only the last one is
+    // exposed, unless the epilogue is longer than the MMA phase it hides behind.  The cooperative cost leaves its epilogue out (so the shape
+    // choice among cooperative tiles is what it was before the ping-pong form existed); coop_epi adds it where the two schedules compete.
+    auto items_of = [](int rows, int bn) { return (double)(rows / 128) * (bn >= 32 ? bn / 32 : 1); };   // 32x32 items per warp quadrant
+    auto coop_epi = [&](long long tiles, int rows, int bn, int split) {   // the 8 consumer warps (4: single-warpgroup tile) share the items
+        const double warps = gemm_single_wg(bn, rows / 128) ? 4.0 : 8.0;
+        const long long waves = (tiles * split + sms - 1) / sms;
+        return (double)waves * items_of(rows, bn) * 4.0 / (warps * split) * EPI_ITEM_BYTES;
+    };
+    auto model = [&](long long tiles, int nstage, long long stage_bytes, int rows, int bn, int& split, bool pp = false) -> double {
+        if (pp) {
+            split = 1;
+            const long long t = (tiles + sms - 1) / sms;               // tiles of the busiest CTA
+            const double mma = (double)nstage * stage_bytes, epi = items_of(rows, bn) * EPI_ITEM_BYTES * 0.5;
+            const double serial = (double)t * mma + epi, paired = (double)((t + 1) / 2) * (mma + epi);
+            return serial > paired ? serial : paired;
+        }
         int smax = 1;
         if (bn >= 32 && cout % 32 == 0) {
             smax = (int)(sms / tiles);
@@ -550,9 +605,10 @@ void conv_geometry(GemmDesc& d, int OW, int OH, int Bt, int cout, bool has_resid
                 if (d.slabs[j].a_sel == d.slabs[i].a_sel && d.slabs[j].a_chan == d.slabs[i].a_chan && d.slabs[j].dw == d.slabs[i].dw) { first = false; break; }
             if (first) ++nstage;
         }
-        int mh = 2, bn = 16, split = 1;               // Cout = 3 (final conv) keeps the 16-wide tile
+        int mh = 2, bn = 16, split = 1, pp = 0;       // Cout = 3 (final conv) keeps the 16-wide tile
         if (cout % 32 == 0) {
-            double best = 1e300;
+            double best = 1e300, best_epi = 0.0, best_pp = 1e300, pp128x64 = 1e300;
+            int pp_mh = 0, pp_bn = 0;
             for (int i = 0; i < 4; ++i) {
                 const Cand& c = cands[i];
                 if (cout % c.bn != 0) continue;
@@ -561,15 +617,27 @@ void conv_geometry(GemmDesc& d, int OW, int OH, int Bt, int cout, bool has_resid
                 const long long stage_bytes = (c.mh == 2 ? 36864 : 18432) + 3ll * c.bn * 128;
                 int sp = 1;
                 const double cost = model(tiles, nstage * npass, stage_bytes, c.mh * 128, c.bn, sp);
+                if (gemm_pingpong_ok(c.bn, c.mh)) {
+                    int sp1 = 1;
+                    const double cpp = model(tiles, nstage * npass, stage_bytes, c.mh * 128, c.bn, sp1, true);
+                    if (cpp < best_pp) { best_pp = cpp; pp_mh = c.mh; pp_bn = c.bn; }
+                    if (c.mh == 1 && c.bn == 64) pp128x64 = cpp;
+                }
                 // the residual is staged through smem (8 warps x 8 KB) unless the tile is split: a 256x128 tile would be left with one stage
                 if (c.bn == 128 && has_resid && sp <= 1) continue;
-                if (cost < best) { best = cost; mh = c.mh; bn = c.bn; split = sp; }
+                if (cost < best) { best = cost; best_epi = coop_epi(tiles, c.mh * 128, c.bn, sp); mh = c.mh; bn = c.bn; split = sp; }
+            }
+            if (!shape_forced) {
+                if (pp_force && pp_bn) { mh = pp_mh; bn = pp_bn; split = 1; pp = 1; }
+                else if (pp_auto && pp128x64 < best + best_epi) { mh = 1; bn = 64; split = 1; pp = 1; }
             }
         }
         if (const char* e = getenv("SR3_TALL_BN")) { int v = atoi(e); if ((v == 32 || v == 64 || v == 128) && cout % v == 0) { bn = v; split = 16; } }
         if (const char* e = getenv("SR3_TALL_MH")) { int v = atoi(e); if (v == 1 || v == 2) { mh = v; split = 16; } }
         if (mh == 2 && bn == 32) bn = 64;
-        d.mh = mh; d.block_n = bn; d.ksplit_max = split;
+        if (shape_forced) pp = (pp_force && gemm_pingpong_ok(bn, mh)) ? 1 : 0;
+        if (pp) split = 1;
+        d.mh = mh; d.block_n = bn; d.ksplit_max = split; d.pingpong = pp;
         geom(mh, d.h_box, d.b_box);
         d.a_box_w = 8; d.a_box_b = d.b_box;
         if (mh == 2 && d.b_box == 1) { d.a_box_h = 34; d.a_half_off = 16 * 1024; }
@@ -583,16 +651,28 @@ void conv_geometry(GemmDesc& d, int OW, int OH, int Bt, int cout, bool has_resid
         if (getenv("SR3_BLOCK_N") == nullptr && cout % 32 == 0) {
             // generic stages group up to three K slabs (one A box + one B box each)
             const int nstage = (((int)d.slabs.size() + 2) / 3) * npass;
-            double best = 1e300;
+            double best = 1e300, best_pp = 1e300;
+            int pp_bn = 0;
             for (int bn = 128; bn >= 32; bn >>= 1) {
                 if (cout % bn != 0) continue;
                 int sp = 1;
-                const double cost = model(mt * (cout / bn), nstage, 3ll * (16384 + bn * 128), 128, bn, sp);
+                const long long tiles = mt * (cout / bn);
+                const double cost = model(tiles, nstage, 3ll * (16384 + bn * 128), 128, bn, sp);
+                // ping-pong needs two stages in flight: one warpgroup holds a stage while the other waits for the next
+                if (gemm_pingpong_ok(bn, 1) && gemm_smem_bytes(bn, 3 * 16384, 3, 2, has_resid, nstage / npass) <= SMEM_LIMIT) {
+                    int sp1 = 1;
+                    const double cpp = model(tiles, nstage, 3ll * (16384 + bn * 128), 128, bn, sp1, true);
+                    if (cpp < best_pp) { best_pp = cpp; pp_bn = bn; }
+                }
                 if (bn == 128 && sp > 1) continue;      // 96 KB stages leave a 2-deep pipeline: measured slower than 64-wide split tiles
                 if (cost < best) { best = cost; d.block_n = bn; d.ksplit_max = sp; }
             }
+            if (pp_force && pp_bn) { d.block_n = pp_bn; d.ksplit_max = 1; d.pingpong = 1; }
+        } else if (pp_force && gemm_pingpong_ok(d.block_n, 1)) {
+            d.pingpong = 1;
         }
     }
+    if (d.pingpong) d.ksplit_max = 1;
     if (const char* e = getenv("SR3_KSPLIT")) d.ksplit_max = atoi(e);
     d.tiles_w = OW / d.w_box; d.tiles_h = (OH + d.h_box - 1) / d.h_box; d.tiles_b = (Bt + d.b_box - 1) / d.b_box;
 }
@@ -821,7 +901,9 @@ struct sr3_engine {
     std::map<std::string, int> pindex;
     std::vector<Op> ops;
     std::vector<GemmHandle> gemms;          // tile-kernel launches of the step, in order (for next-layer weight prefetch)
-    struct OpInfo { int kind; double flops; double bytes; };   // kind: 0 gemm, 1 groupnorm-apply, 2 cast/upsample, 3 softmax, 4 other
+    // kind: 0 gemm, 1 groupnorm-apply, 2 cast/upsample, 3 softmax, 4 other.  Tile ops also keep the variant they launch (sr3_tile_schedule):
+    // geometry, schedule (0 cooperative, 1 ping-pong; -1 not a tile op) and output rows x columns x channels.
+    struct OpInfo { int kind; double flops; double bytes; sr3_gemm_geometry geo; int schedule; int out_hwc[3]; };
     std::vector<OpInfo> op_info;
     std::map<std::string, Act> taps;
     std::map<std::string, size_t> role_max;
@@ -969,7 +1051,7 @@ struct sr3_engine {
         if (dry) return;
         if (bwd_sink) { bwd_sink->push_back(std::move(op)); bwd_kinds.back().push_back(kind); return; }
         ops.push_back(std::move(op));
-        op_info.push_back({kind, flops, bytes});
+        op_info.push_back({kind, flops, bytes, sr3_gemm_geometry{}, -1, {0, 0, 0}});
     }
     // executed work of a gemm op: 2*M*N*K flops; bytes = A read once per tap set + B once + outputs
     void push_gemm(const GemmDesc& d) {
@@ -983,7 +1065,15 @@ struct sr3_engine {
         double a_elems = 0;
         for (int i = 0; i < d.n_a; ++i) a_elems += (double)d.a[i].C * d.a[i].W * d.a[i].P * d.a[i].H * d.a[i].Bn;
         bytes += a_elems * 2;
-        push(make_gemm_op(d, mem), 0, 2.0 * M * N * K, bytes);
+        sr3_gemm_geometry geo{};
+        int schedule = 0;
+        push(make_gemm_op(d, mem, &geo, &schedule), 0, 2.0 * M * N * K, bytes);
+        if (!dry && !bwd_sink) {
+            OpInfo& info = op_info.back();
+            info.geo = geo; info.schedule = schedule;
+            // output rows x columns (a folded upsample's four phases land at twice the resolution) x channels
+            info.out_hwc[0] = d.OH * (d.z_phase ? 2 : 1); info.out_hwc[1] = d.OW * (d.z_phase ? 2 : 1); info.out_hwc[2] = d.n_valid;
+        }
     }
 
     // ---- layer builders -------------------------------------------------------------------------
@@ -1167,6 +1257,7 @@ struct sr3_engine {
             d.OW = Ww; d.OH = Hh; d.OB = Bp; d.n_valid = ncol;
             d.out_bf16 = qk; d.hs = nhwc_out(Hh, Ww, 2 * C * PW); d.lo_out_off = precise ? 2 * C : 0;      // rows [q_hi | k_hi | q_lo | k_lo]
             d.out_t = vT; d.t_col0 = 2 * C; d.t_rows = C; d.t_ld = Lt * PW; d.t_per = per; d.lo_t_off = precise ? Lt : 0;
+            d.pingpong = pingpong_knob() == 1 ? 1 : 0;         // (fixed 128x128 shape: the byte model is not consulted)
             push_gemm(d);
         }
         if (attn_fusable(Lt, C) && !precise && !train) {
@@ -1481,7 +1572,7 @@ struct sr3_engine {
             MegaOp o{}; o.type = r.type; o.variant = r.variant;
             const uint8_t* src = r.raw.data(); size_t n = r.raw.size();
             if (r.type == MOP_GEMM) {
-                const int bn = r.variant & 0xffff, mh = r.variant >> 16;
+                const int bn = r.variant & 0xffff, mh = (r.variant >> 16) & 0xff;
                 if (!((bn == 16 || bn == 32 || bn == 64 || bn == 128) && (mh == 1 || mh == 2) && !(bn == 32 && mh == 2))) { use_mega = false; return; }
                 src = reinterpret_cast<const uint8_t*>(r.gp.get()); n = sizeof(GemmParams);
             }
@@ -2155,9 +2246,33 @@ int sr3_test_conv_ex(const sr3_test_conv_args* a, sr3_gemm_geometry* geometry, v
     c.raw_out = static_cast<bf16*>(a->y_bf16);
     GemmDesc d = conv_desc(c, B, B, PW);
     d.out_imgs = B;          // the last tile may cover images past B: they load as zeros and are not stored
-    Op op = make_gemm_op(d, mem, geometry);
+    g_last_test_conv = LastTestConv{};
+    Op op = make_gemm_op(d, mem, &g_last_test_conv.geo, &g_last_test_conv.schedule);
+    g_last_test_conv.out_hwc[0] = d.OH * (d.z_phase ? 2 : 1); g_last_test_conv.out_hwc[1] = d.OW * (d.z_phase ? 2 : 1); g_last_test_conv.out_hwc[2] = d.n_valid;
+    if (geometry) *geometry = g_last_test_conv.geo;
     op(st);
     CK(cudaStreamSynchronize(st));
+    API_END
+}
+
+int sr3_tile_schedule(const sr3_engine* e, int op, sr3_gemm_geometry* geometry, int* schedule, int* out_hwc) {
+    API_BEGIN
+    REQUIRE(schedule, "null argument");
+    sr3_gemm_geometry geo{};
+    int sch = -1, hwc[3] = {0, 0, 0};
+    if (e == nullptr) {
+        REQUIRE(g_last_test_conv.schedule >= 0, "no sr3_test_conv_ex call on this thread yet");
+        geo = g_last_test_conv.geo; sch = g_last_test_conv.schedule;
+        for (int i = 0; i < 3; ++i) hwc[i] = g_last_test_conv.out_hwc[i];
+    } else {
+        REQUIRE(op >= 0 && op < (int)e->op_info.size(), "op %d out of range (%d ops per step)", op, (int)e->op_info.size());
+        const sr3_engine::OpInfo& info = e->op_info[op];
+        geo = info.geo; sch = info.schedule;
+        for (int i = 0; i < 3; ++i) hwc[i] = info.out_hwc[i];
+    }
+    if (geometry) *geometry = geo;
+    *schedule = sch;
+    if (out_hwc) for (int i = 0; i < 3; ++i) out_hwc[i] = hwc[i];
     API_END
 }
 

@@ -18,6 +18,8 @@
 //   32 columns: warpgroup 0 alone) and then run the epilogue on it: accumulator -> per-warp 32 x 32 transposition in shared memory ->
 //   bias / FiLM -> residual (TMA prefetched into smem) -> fp32 tile staged in swizzled smem and written by TMA store (and/or bf16
 //   direct stores) -> per-(image, channel) GroupNorm partial sums, accumulated in registers across tiles.
+//   Ping-pong schedule (PP, 256x64 / 128x128 / 128x64 tiles): instead each warpgroup owns every other tile of the CTA's range and the two
+//   take turns at the MMAs (named barriers 2 and 3), so the epilogue of one tile runs while the tensor cores work on the next.
 // * A warpgroup's m64 wgmma pair covers 128 rows with the 8-row groups interleaved (instruction i reads groups 2g + i at a 2048 B group
 //   stride), so that warp q of the group holds exactly rows [32 q, 32 q + 32): the 32-row unit of the epilogue, of its TMA boxes and of
 //   the statistics.
@@ -154,6 +156,12 @@ constexpr int HDR_PARAMS = 768;
 constexpr int HDR_NUM_BARS = 64;
 // Tiles of at most 32 columns (MH = 1) are computed by warpgroup 0 alone; every other tile is shared by both consumer warpgroups.
 __host__ __device__ constexpr bool gemm_single_wg(int block_n, int mh) { return mh == 1 && block_n <= 32; }
+// Ping-pong schedule: each consumer warpgroup owns whole tiles (local tiles g, g + 2, ... of the CTA's range), their MMA phases take
+// turns through two named barriers, so one warpgroup's epilogue runs while the other one feeds the tensor cores.  Shapes it exists for:
+__host__ __device__ constexpr bool gemm_pingpong_ok(int block_n, int mh) { return (mh == 2 && block_n == 64) || (mh == 1 && (block_n == 64 || block_n == 128)); }
+constexpr int GEMM_ORDER_BAR = 2;            // named barriers 2 (warpgroup 0's turn) and 3 (warpgroup 1's turn); 1 is the split-K pass
+// arrivals that release a pipeline stage: one per warpgroup that reads it
+__host__ __device__ constexpr int gemm_stage_readers(int block_n, int mh, bool pp) { return (pp || gemm_single_wg(block_n, mh)) ? 1 : 2; }
 __host__ __device__ constexpr int gemm_aux_bytes(int num_k) {
     return GEMM_HDR_BYTES + ((num_k * 96 + 127) / 128) * 128 /*stage table*/ + GEMM_EPI_WARPS * 2 * 32 * 4 /*per-warp bias staging*/;
 }
@@ -260,7 +268,7 @@ static_assert(sizeof(GemmParams) <= GEMM_HDR_BYTES - HDR_PARAMS, "GemmParams mus
 // depends on data produced by other CTAs, so the persistent step kernel runs it BEFORE waiting at the grid barrier in front of the op.
 // Must be followed by a block-wide barrier.
 __device__ __forceinline__ void gemm_stage_setup(const GemmParams& p, const GemmParams* pm, const uint32_t base, uint8_t* base_ptr, const int block_n,
-                                                 const int mh, const bool recycle) {
+                                                 const int mh, const bool pp, const bool recycle) {
     const int stages = p.stages;
     const int stage_bytes = p.a_stage_bytes + p.b_taps * block_n * 128;
     const bool use_res_tma = p.tma_epi && p.resid != nullptr && p.ksplit <= 1;
@@ -280,10 +288,10 @@ __device__ __forceinline__ void gemm_stage_setup(const GemmParams& p, const Gemm
         if (recycle) {                           // the previous op's barriers (all quiescent: see the end of gemm_tile_body) are recycled
             for (int i = 0; i < HDR_NUM_BARS; ++i) mbar_inval(bar_base + 8u * i);
         }
-        const uint32_t consumers = gemm_single_wg(block_n, mh) ? 1 : 2;
+        const uint32_t consumers = gemm_stage_readers(block_n, mh, pp);
         for (int s = 0; s < stages; ++s) {
             mbar_init(bar_base + 8u * s, 1);                                     // full
-            mbar_init(bar_base + 8u * (GEMM_MAX_STAGES + s), consumers);         // empty: one arrive per consumer warpgroup
+            mbar_init(bar_base + 8u * (GEMM_MAX_STAGES + s), consumers);         // empty: one arrive per consumer warpgroup that reads it
         }
         for (int w = 0; w < 2 * GEMM_EPI_WARPS; ++w) mbar_init(bar_base + 8u * (2 * GEMM_MAX_STAGES + w), 1);   // residual tiles
         fence_mbar_init();
@@ -367,17 +375,23 @@ struct StatRun {
 //                 of the op's parameter block, `pm` its global-memory original (TMA descriptors must not live in shared memory),
 //                 `cta / ncta` replace blockIdx / gridDim.
 // `base` / `base_ptr`: 1024-aligned start of the CTA's dynamic shared memory (header first).
-template <int BLOCK_N, int MH, bool MEGA>
+// PP = false: cooperative schedule, both warpgroups share every tile.  PP = true: ping-pong schedule (gemm_pingpong_ok shapes, no split-K):
+// warpgroup g owns the CTA's local tiles g, g + 2, ... with an accumulator of the whole tile, and the warpgroups issue their MMAs in
+// turn (order barrier GEMM_ORDER_BAR + g), so the stage ring is consumed strictly in order, one warpgroup per stage.
+template <int BLOCK_N, int MH, bool MEGA, bool PP = false>
 __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmParams* pm, const uint32_t base, uint8_t* base_ptr,
                                                const int cta, const int ncta) {
+    static_assert(!PP || gemm_pingpong_ok(BLOCK_N, MH), "ping-pong tile shape");
     constexpr int B_BYTES = BLOCK_N * 128;
-    constexpr bool SINGLE = gemm_single_wg(BLOCK_N, MH);
-    constexpr int WN = (SINGLE || MH == 2) ? BLOCK_N : BLOCK_N / 2;     // accumulator columns of one warpgroup
+    constexpr bool SINGLE = !PP && gemm_single_wg(BLOCK_N, MH);
+    constexpr int WN = (PP || SINGLE || MH == 2) ? BLOCK_N : BLOCK_N / 2;   // accumulator columns of one warpgroup
+    constexpr int AH = PP ? MH : 1;                                     // 128-row halves in one warpgroup's accumulator
     constexpr int CW = WN < 32 ? WN : 32;                               // columns of one epilogue chunk
     constexpr int NCH = BLOCK_N >= 32 ? BLOCK_N / 32 : 1;               // 32-column chunks per 128-row half
     constexpr int NITEMS = MH * NCH;                                    // work items (half, chunk) per tile
-    constexpr int OWN = SINGLE ? 1 : NITEMS / 2;                        // items held by one warpgroup's accumulator
-    static_assert(WN % CW == 0 && WN <= 128, "accumulator shape");
+    constexpr int OWN = PP ? NITEMS : SINGLE ? 1 : NITEMS / 2;          // items held by one warpgroup's accumulator
+    constexpr int NSTAT = PP ? NCH : OWN;                               // chunks of one GroupNorm run (ping-pong: one run per half)
+    static_assert(WN % CW == 0 && AH * WN <= 128, "accumulator shape");
 
     const int stages = p.stages;
     const int stage_bytes = p.a_stage_bytes + p.b_taps * B_BYTES;            // multiple of 1024
@@ -404,7 +418,7 @@ __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmPa
     const int total_tiles = tiles_m * p.n_tiles * p.nz * ksplit;      // split index fastest: the CTAs of one output tile run together
     const int num_kt = p.num_k * (p.passes > 1 ? p.passes : 1);       // stages per tile (precise mode: three passes over the table)
     if constexpr (!MEGA) {
-        gemm_stage_setup(p, pm, base, base_ptr, BLOCK_N, MH, false);  // (the step kernel did this before its grid barrier)
+        gemm_stage_setup(p, pm, base, base_ptr, BLOCK_N, MH, PP, false);  // (the step kernel did this before its grid barrier)
         __syncthreads();
     }
     if (warp == 2 && lane == 0 && p.pf_bytes > 0) {                   // L2 prefetch of this CTA's slice of the next layer's weights
@@ -490,10 +504,10 @@ __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmPa
         const int q = warp & 3;
         const int ew = warp;                                                // 0..7
         const bool mma_wg = !SINGLE || g == 0;                              // (the warpgroups that hold items)
-        const int own0 = SINGLE ? 0 : g * OWN;                              // items [own0, own0 + OWN) are in this warpgroup's accumulator
-        const int ch0 = own0 % NCH;                                         // item own0 + ii = accumulator chunk ii = tile chunk ch0 + ii
-        const int acc_half = MH == 2 ? g : 0;
-        const int acc_c0 = (MH == 1 && !SINGLE) ? g * WN : 0;               // first accumulator column inside the tile
+        const int own0 = (SINGLE || PP) ? 0 : g * OWN;                      // items [own0, own0 + OWN) are in this warpgroup's accumulator
+        const int ch0 = PP ? 0 : own0 % NCH;                                // item own0 + ii = accumulator chunk ii = tile chunk ch0 + ii
+        const int acc_half = (MH == 2 && !PP) ? g : 0;
+        const int acc_c0 = (MH == 1 && !SINGLE && !PP) ? g * WN : 0;        // first accumulator column inside the tile
         const uint32_t out_smem = epi_base + ew * epi_warp_bytes;           // 4 KB
         const uint32_t res_smem = out_smem + 4096;                          // 2 x 4 KB (layers with a residual only)
         uint8_t* out_ptr = stage_ptr + stages * stage_bytes + ew * epi_warp_bytes;
@@ -503,15 +517,21 @@ __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmPa
         uint32_t res_count = 0;        // residual chunks consumed so far
         uint32_t bias_slot = 0;        // alternating bias staging slot
         bool out_pending = false;      // a bulk store from the staging buffer may still be reading it
-        float acc[2][WN / 2];
+        float acc[AH][2][WN / 2];
         int s = 0;                     // stage ring position
         uint32_t ph = 0;
         // GroupNorm partial sums of this lane's column in the warp's OWN chunks, kept across the tiles of one (image, column block).
-        // (All items of a warp's share of a tile lie in one image: a warp's 32 rows never straddle images.)
-        StatRun<OWN> st_own;
-        for (int tile = tile_begin; tile < tile_end; ++tile) {
+        // (All items of a warp's share of a tile lie in one image: a warp's 32 rows never straddle images.  Ping-pong: the two halves of
+        // a tile may be two images, so a run covers the NCH chunks of one half.)
+        StatRun<NSTAT> st_own;
+        for (int tile = tile_begin + (PP ? g : 0); tile < tile_end; tile += (PP ? 2 : 1)) {
             int w0, h0, b0, n0, z;
             decode(tile, w0, h0, b0, n0, z);
+            if constexpr (PP) {        // every tile of the range streams num_kt stages: this tile's first stage is number li * num_kt
+                const long long pos = static_cast<long long>(tile - tile_begin) * num_kt;
+                s = static_cast<int>(pos % stages);
+                ph = static_cast<uint32_t>((pos / stages) & 1);
+            }
             // geometry of a work item: rows of `half`, columns of `ch`
             auto item_geom = [&](int item, int qq, int& half, int& ch, int& sw, int& sh, int& c4) {
                 half = item / NCH; ch = item % NCH;
@@ -567,6 +587,8 @@ __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmPa
                 }
                 const uint32_t a_base = stage_base + acc_half * p.a_half_off;
                 const uint32_t b_base = stage_base + p.a_stage_bytes + acc_c0 * 128;
+                const int li = tile - tile_begin;                           // (ping-pong) local tile index: li % 2 == g
+                if (PP && li > 0) asm volatile("bar.sync %0, 256;" ::"r"(GEMM_ORDER_BAR + g) : "memory");   // our turn to issue MMAs
                 int prev = -1;
                 for (int k = k0; k < k1; ++k) {
                     mbar_wait(full_bar(s), ph, 2);
@@ -579,9 +601,12 @@ __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmPa
                         for (int kk = 0; kk < 4; ++kk) {   // 4 x K(16) = 64 channels; +32 B inside the 128 B swizzle row
                             const uint64_t bdesc = wgmma_desc_sw128(b_addr + kk * 32, 16, 1024);
 #pragma unroll
-                            for (int i = 0; i < 2; ++i)    // row groups 2 g' + i, g' = 0..7
-                                Wgmma<WN>::template mma<0, 0>(acc[i], wgmma_desc_sw128(a_addr + i * 1024 + kk * 32, 16, 2048), bdesc,
-                                                              ((k - k0) | t | kk) != 0);
+                            for (int hh = 0; hh < AH; ++hh)    // (ping-pong, MH = 2: both 128-row halves share the B slab)
+#pragma unroll
+                                for (int i = 0; i < 2; ++i)    // row groups 2 g' + i, g' = 0..7
+                                    Wgmma<WN>::template mma<0, 0>(acc[hh][i],
+                                                                  wgmma_desc_sw128(a_addr + hh * p.a_half_off + i * 1024 + kk * 32, 16, 2048),
+                                                                  bdesc, ((k - k0) | t | kk) != 0);
                         }
                     }
                     wgmma_commit();
@@ -597,16 +622,21 @@ __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmPa
                     }
                     if (++s == stages) { s = 0; ph ^= 1u; }
                 }
+                // every MMA of the tile is issued: the other warpgroup may issue those of the next tile (if the CTA has one)
+                if (PP && tile + 1 < tile_end) asm volatile("bar.arrive %0, 256;" ::"r"(GEMM_ORDER_BAR + (g ^ 1)) : "memory");
                 wgmma_wait<0>();
-                wgmma_fence_regs(acc[0]);
-                wgmma_fence_regs(acc[1]);
+#pragma unroll
+                for (int hh = 0; hh < AH; ++hh) {
+                    wgmma_fence_regs(acc[hh][0]);
+                    wgmma_fence_regs(acc[hh][1]);
+                }
                 if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(empty_bar(prev));
             }
             // pass 0 reads the accumulator.  With split-K it only stores this CTA's partial tile into its slice of `ws`;
             // once all `ksplit` CTAs of the output tile have arrived at the tile's counter, pass 1 runs in EVERY one of them on a
             // 1/ksplit share of the tile's 32x32 units: sum the partials (fixed order: deterministic) and do the real epilogue.
             // (All CTAs of the grid are resident -- at most one (tile, split) pair per SM -- so the spin wait cannot deadlock.)
-            const int npass = ksplit > 1 ? 2 : 1;
+            const int npass = (!PP && ksplit > 1) ? 2 : 1;                 // (the host never splits a ping-pong launch)
             constexpr long long SLICE = static_cast<long long>(MH) * 128 * BLOCK_N;       // floats per partial tile
 #pragma unroll 1
             for (int pass = 0; pass < npass; ++pass) {
@@ -636,7 +666,7 @@ __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmPa
                 __syncwarp();
                 asm volatile("bar.sync 1, 256;" ::: "memory");
             }
-            const bool to_ws = (ksplit > 1 && pass == 0);
+            const bool to_ws = (!PP && ksplit > 1 && pass == 0);
             // the epilogue of one item (half, chunk) in quadrant qq: `fetch(v)` brings this lane's row of the item's 32x32 chunk (lane = row,
             // v[j] = column j), which is then finished in place; `add_stats(cs, cq)` takes the GroupNorm sums of this lane's column
             auto epi_item = [&](const int item, const int qq, const float bv, const bool last, auto&& fetch, auto&& add_stats) {
@@ -827,15 +857,19 @@ __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmPa
             };
             if (pass == 0) {
                 if (mma_wg) {
-                    if (p.stats && !to_ws) st_own.start(p, b0 + ((acc_half * 128 + q * 32) >> (p.w_shift + p.h_shift)), n0, ch0, lane);
+                    if (!PP && p.stats && !to_ws) st_own.start(p, b0 + ((acc_half * 128 + q * 32) >> (p.w_shift + p.h_shift)), n0, ch0, lane);
                     static_for<OWN>([&](auto ii_c) {             // compile-time ii: accumulator chunk ii is dead once it has been staged
                         constexpr int ii = decltype(ii_c)::value;
+                        constexpr int AHI = PP ? ii / NCH : 0, ACL = PP ? ii % NCH : ii;   // accumulator half and chunk of item ii
+                        if constexpr (PP) {                      // a new half may be a new image: its own GroupNorm run
+                            if (ACL == 0 && p.stats) st_own.start(p, b0 + ((AHI * 128 + q * 32) >> (p.w_shift + p.h_shift)), n0, 0, lane);
+                        }
                         auto stage_acc = [&](float (&v)[32]) {
                             if (out_pending) {                   // the staging buffer is about to be overwritten by the transposition
                                 if (lane == 0) tma_store_wait_read<0>();
                                 __syncwarp();
                             }
-                            acc_chunk_rows<WN, CW, ii>(acc, reinterpret_cast<float*>(out_ptr), v);
+                            acc_chunk_rows<WN, CW, ACL>(acc[AHI], reinterpret_cast<float*>(out_ptr), v);
                         };
                         if (to_ws) {                             // split-K: park the partial sums
                             float v[32];
@@ -844,7 +878,7 @@ __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmPa
 #pragma unroll
                             for (int j = 0; j < 8; ++j) __stcg(dst + j * WJ, make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]));
                         } else {
-                            epi_item(own0 + ii, q, bvs[ii], ii + 1 == OWN, stage_acc, [&](double cs, double cq) { st_own.add(ii, cs, cq); });
+                            epi_item(own0 + ii, q, bvs[ii], ii + 1 == OWN, stage_acc, [&](double cs, double cq) { st_own.add(PP ? ACL : ii, cs, cq); });
                         }
                     });
                 }
@@ -887,12 +921,12 @@ __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmPa
     }
 }
 
-template <int BLOCK_N, int MH>
+template <int BLOCK_N, int MH, bool PP = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tile_kernel(const __grid_constant__ GemmParams p) {
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw = smem_u32(smem_raw);
     const uint32_t base = (raw + 1023u) & ~1023u;
-    gemm_tile_body<BLOCK_N, MH, false>(p, &p, base, smem_raw + (base - raw), blockIdx.x, gridDim.x);
+    gemm_tile_body<BLOCK_N, MH, false, PP>(p, &p, base, smem_raw + (base - raw), blockIdx.x, gridDim.x);
 }
 
 }  // namespace sr3

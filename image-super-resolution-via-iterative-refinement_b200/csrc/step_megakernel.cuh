@@ -20,7 +20,7 @@ enum MegaOpType : int { MOP_GEMM = 0, MOP_PREP = 1, MOP_ATTN = 2, MOP_SOFTMAX = 
 
 struct MegaOp {
     int type;
-    int variant;        // gemm: BLOCK_N | (MH << 16)
+    int variant;        // gemm: BLOCK_N | (MH << 16) | (ping-pong << 24)
     int sync_before;    // 1: grid barrier before this op (it reads what other CTAs wrote in earlier ops)
     int param_bytes;
     long long param_off;    // byte offset of the parameter block inside the blob (128-byte aligned)
@@ -266,9 +266,10 @@ __device__ __noinline__ void embed_film_body(const EmbedFilmParams& p, float* sm
 
 // ---------------------------------------------------------------------------------------------------------------- the step kernel
 // (not inlined: every tile variant / op body gets its own register allocation instead of sharing the step kernel's)
-template <int BN, int MH>
+constexpr int MEGA_VARIANT_PP = 1 << 24;
+template <int BN, int MH, bool PP = false>
 __device__ __noinline__ void mega_gemm(const uint8_t* hdr_params, const uint8_t* gparams, uint32_t base, uint8_t* base_ptr, int cta, int ncta) {
-    gemm_tile_body<BN, MH, true>(*reinterpret_cast<const GemmParams*>(hdr_params), reinterpret_cast<const GemmParams*>(gparams), base, base_ptr,
+    gemm_tile_body<BN, MH, true, PP>(*reinterpret_cast<const GemmParams*>(hdr_params), reinterpret_cast<const GemmParams*>(gparams), base, base_ptr,
                                  cta, ncta);
 }
 
@@ -310,7 +311,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) step_kernel(const __grid_cons
         if (op.type == MOP_GEMM) {
             if (threadIdx.x == 0) reinterpret_cast<GemmParams*>(hdr_params)->t_fixed = t_step;
             gemm_stage_setup(*reinterpret_cast<const GemmParams*>(hdr_params), reinterpret_cast<const GemmParams*>(gparams), base, base_ptr,
-                             op.variant & 0xffff, op.variant >> 16, true);
+                             op.variant & 0xffff, (op.variant >> 16) & 0xff, (op.variant & MEGA_VARIANT_PP) != 0, true);
         }
         if (stamp) mp.prof[4 * i + 1] = globaltimer_ns();
         if (op.sync_before) gb.wait(i); else __syncthreads();
@@ -325,6 +326,9 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) step_kernel(const __grid_cons
                     case 64 | (2 << 16): mega_gemm<64, 2>(hdr_params, gparams, base, base_ptr, cta, ncta); break;
                     case 128 | (1 << 16): mega_gemm<128, 1>(hdr_params, gparams, base, base_ptr, cta, ncta); break;
                     case 128 | (2 << 16): mega_gemm<128, 2>(hdr_params, gparams, base, base_ptr, cta, ncta); break;
+                    case 64 | (2 << 16) | MEGA_VARIANT_PP: mega_gemm<64, 2, true>(hdr_params, gparams, base, base_ptr, cta, ncta); break;
+                    case 64 | (1 << 16) | MEGA_VARIANT_PP: mega_gemm<64, 1, true>(hdr_params, gparams, base, base_ptr, cta, ncta); break;
+                    case 128 | (1 << 16) | MEGA_VARIANT_PP: mega_gemm<128, 1, true>(hdr_params, gparams, base, base_ptr, cta, ncta); break;
                     default: if (threadIdx.x == 0) printf("sr3: step kernel: unsupported tile variant %x\n", op.variant); __trap();
                 }
                 break;

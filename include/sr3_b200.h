@@ -228,6 +228,11 @@ typedef struct sr3_test_conv_args {
     int fold_up, precise;
 } sr3_test_conv_args;
 int sr3_test_conv_ex(const sr3_test_conv_args* args, sr3_gemm_geometry* geometry, void* stream);
+/* Schedule of a tile-kernel launch: *schedule = 0 cooperative (both consumer warpgroups share every tile), 1 ping-pong (each warpgroup owns
+ * whole tiles and its epilogue overlaps the other one's MMAs), -1 op `op` is not a tile-kernel launch.  e = NULL: the most recent
+ * sr3_test_conv_ex call of the calling thread (`op` ignored); otherwise op `op` of e's eager step, indexed as sr3_engine_profile_step
+ * reports them.  geometry and out_hwc (output rows, columns, channels; optional) receive the rest of the launch. */
+int sr3_tile_schedule(const sr3_engine* e, int op, sr3_gemm_geometry* geometry, int* schedule, int* out_hwc);
 /* Weight gradient of one conv through wgrad_kernel + wgrad_reduce_kernel (the training plan's path): dy bf16 NHWC [B][OH][OW][CY], x bf16
  * NHWC [B][OH*stride][OW*stride][Cin]; k = 1 (stride 1) or 3 (stride 1 or 2, padding 1).  grad fp32 OIHW [cout_valid][cin_valid][k][k] =
  * gscale * dW over the first cout_valid / cin_valid channels.  slices = 0: the training plan's slice count; *slices_used (optional) reports it.
