@@ -77,6 +77,9 @@ _SIGS = {
     "sr3_resize_bicubic_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_float, c_void_p]),
     "sr3_tensor2img": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_float, c_void_p]),
     "sr3_ssd_u8": (c_int, [c_void_p, c_void_p, c_int64, POINTER(c_uint64), c_void_p]),
+    "sr3_ssim": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, POINTER(c_double), c_void_p]),
+    "sr3_image_metrics": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_float, c_void_p, c_void_p, POINTER(c_uint64),
+                                  POINTER(c_double), c_void_p]),
     "sr3_engine_num_launches_per_step": (c_int, [c_void_p]),
     "sr3_engine_num_ops_per_step": (c_int, [c_void_p]),
     "sr3_engine_uses_step_kernel": (c_int, [c_void_p]),

@@ -392,9 +392,13 @@ __global__ void __launch_bounds__(256) loss_sum_kernel(const float* __restrict__
 // tensor2img of the reference (core/metrics.py:8-34) on the device: clamp to [lo, hi] -> (x - lo) / (hi - lo) -> * 255 -> round half to even
 // -> uint8, laid out HWC.  `n` images [n][C][H][W] are tiled like torchvision.utils.make_grid(nrow, padding=2, pad_value=0) when n > 1
 // (grid of ncol x nrow cells of (H+2) x (W+2) pixels plus a 2-pixel border); n == 1: plain [H][W][C].
+// Per-image form: n == 1 and gridDim.y images, image blockIdx.y read from src [y][C][H][W] and written to its own dst [y][H][W][C]
+// (what tensor2img(sr[i]) gives for every i of a batch); the grid form launches gridDim.y == 1.
 __global__ void __launch_bounds__(256) tensor2img_kernel(const float* __restrict__ src, unsigned char* __restrict__ dst, int n, int C, int H, int W,
                                                          int ncol, int GH, int GW, float lo, float hi) {
     const long long total = static_cast<long long>(GH) * GW * C;
+    src += blockIdx.y * (static_cast<long long>(C) * H * W);
+    dst += blockIdx.y * total;
     const int pad = n > 1 ? 2 : 0;
     for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total; i += static_cast<long long>(gridDim.x) * blockDim.x) {
         const int c = static_cast<int>(i % C);
@@ -418,9 +422,13 @@ __global__ void __launch_bounds__(256) tensor2img_kernel(const float* __restrict
     }
 }
 
-// sum of squared differences of two uint8 images (calculate_psnr, core/metrics.py:42-50): exact in integers
+// sum of squared differences of two uint8 images (calculate_psnr, core/metrics.py:42-50): exact in integers.
+// Per-pair form: gridDim.y pairs of n elements each, pair blockIdx.y summed into out[blockIdx.y] (integer atomics: order-independent).
 __global__ void __launch_bounds__(256) ssd_u8_kernel(const unsigned char* __restrict__ a, const unsigned char* __restrict__ b, long long n,
                                                      unsigned long long* __restrict__ out) {
+    a += blockIdx.y * n;
+    b += blockIdx.y * n;
+    out += blockIdx.y;
     unsigned long long acc = 0;
     for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n; i += static_cast<long long>(gridDim.x) * blockDim.x) {
         const int d = static_cast<int>(a[i]) - static_cast<int>(b[i]);
@@ -429,6 +437,82 @@ __global__ void __launch_bounds__(256) ssd_u8_kernel(const unsigned char* __rest
 #pragma unroll
     for (int o = 16; o; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
     if ((threadIdx.x & 31) == 0 && acc) atomicAdd(out, acc);
+}
+
+// ssim of the reference (core/metrics.py:52-72), everything in fp64: the 11x11 window outer(g, g) of cv2.getGaussianKernel(11, 1.5), applied
+// as an 11-tap horizontal then an 11-tap vertical pass to the five moments x, y, x^2, y^2, xy, only where the window fits the image
+// (filter2D(...)[5:-5, 5:-5] keeps exactly those pixels); sigma = E[x^2] - mu^2; every channel of an HWC image filtered on its own.
+// Pair blockIdx.z of [n][H][W][C]; a CTA owns an SSIM_TH x SSIM_TW tile of the (H-10) x (W-10) valid region across all channels and writes
+// the sum of its map values to partial[pair][tile]; ssim_finish_kernel adds the tiles in order.  The split depends on (H, W, C) only, so a
+// pair's value does not depend on the batch it is scored in.
+constexpr int SSIM_TH = 16, SSIM_TW = 32, SSIM_THREADS = 256, SSIM_TAPS = 11;
+struct SsimWindow { double g[SSIM_TAPS]; };
+
+template <typename T>
+__global__ void __launch_bounds__(SSIM_THREADS) ssim_kernel(const T* __restrict__ a, const T* __restrict__ b, int H, int W, int C, const SsimWindow win,
+                                                            double* __restrict__ partial) {
+    constexpr int R = SSIM_TH + SSIM_TAPS - 1;                  // input rows a tile's vertical pass reads
+    __shared__ double hs[5][R][SSIM_TW];                        // horizontal pass: the five moments per (input row, output column)
+    __shared__ double ws[SSIM_THREADS / 32];
+    constexpr double C1 = (0.01 * 255) * (0.01 * 255), C2 = (0.03 * 255) * (0.03 * 255);
+    const int Hv = H - (SSIM_TAPS - 1), Wv = W - (SSIM_TAPS - 1);
+    const int x0 = blockIdx.x * SSIM_TW, y0 = blockIdx.y * SSIM_TH;
+    const long long img = blockIdx.z * (static_cast<long long>(H) * W * C);
+    a += img;
+    b += img;
+    double acc = 0.0;
+    for (int c = 0; c < C; ++c) {
+        for (int i = threadIdx.x; i < R * SSIM_TW; i += SSIM_THREADS) {
+            const int r = i / SSIM_TW, j = i % SSIM_TW;
+            double m[5] = {0.0, 0.0, 0.0, 0.0, 0.0};
+            if (y0 + r < H && x0 + j < Wv) {
+                const long long p = (static_cast<long long>(y0 + r) * W + x0 + j) * C + c;
+#pragma unroll
+                for (int k = 0; k < SSIM_TAPS; ++k) {
+                    const double u = static_cast<double>(a[p + k * C]), v = static_cast<double>(b[p + k * C]), w = win.g[k];
+                    m[0] += w * u; m[1] += w * v; m[2] += w * (u * u); m[3] += w * (v * v); m[4] += w * (u * v);
+                }
+            }
+#pragma unroll
+            for (int q = 0; q < 5; ++q) hs[q][r][j] = m[q];
+        }
+        __syncthreads();
+        for (int i = threadIdx.x; i < SSIM_TH * SSIM_TW; i += SSIM_THREADS) {
+            const int r = i / SSIM_TW, j = i % SSIM_TW;
+            if (y0 + r >= Hv || x0 + j >= Wv) continue;
+            double m[5] = {0.0, 0.0, 0.0, 0.0, 0.0};
+#pragma unroll
+            for (int k = 0; k < SSIM_TAPS; ++k) {
+#pragma unroll
+                for (int q = 0; q < 5; ++q) m[q] += win.g[k] * hs[q][r + k][j];
+            }
+            // explicit roundings (no contraction): for x == y both factors of the ratio are bit-identical, so the map is exactly 1
+            const double mu1_sq = __dmul_rn(m[0], m[0]), mu2_sq = __dmul_rn(m[1], m[1]), mu1_mu2 = __dmul_rn(m[0], m[1]);
+            const double s1 = __dsub_rn(m[2], mu1_sq), s2 = __dsub_rn(m[3], mu2_sq), s12 = __dsub_rn(m[4], mu1_mu2);
+            const double num = __dmul_rn(__dadd_rn(__dmul_rn(2.0, mu1_mu2), C1), __dadd_rn(__dmul_rn(2.0, s12), C2));
+            const double den = __dmul_rn(__dadd_rn(__dadd_rn(mu1_sq, mu2_sq), C1), __dadd_rn(__dadd_rn(s1, s2), C2));
+            acc += __ddiv_rn(num, den);
+        }
+        __syncthreads();
+    }
+#pragma unroll
+    for (int o = 16; o; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+    if ((threadIdx.x & 31) == 0) ws[threadIdx.x >> 5] = acc;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double t = 0.0;
+        for (int i = 0; i < SSIM_THREADS / 32; ++i) t += ws[i];
+        partial[(static_cast<long long>(blockIdx.z) * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x] = t;
+    }
+}
+
+// ssim_map.mean() per pair: the pair's `tiles` partial sums added in tile order, over `count` = (H-10) (W-10) C map values
+__global__ void __launch_bounds__(128) ssim_finish_kernel(const double* __restrict__ partial, int tiles, double count, int n, double* __restrict__ out) {
+    const int pair = blockIdx.x * blockDim.x + threadIdx.x;
+    if (pair >= n) return;
+    double t = 0.0;
+    for (int i = 0; i < tiles; ++i) t += partial[static_cast<long long>(pair) * tiles + i];
+    out[pair] = t / count;
 }
 
 // One pass of Pillow's 8-bit resampler (src/libImaging/Resample.c, ImagingResampleHorizontal_8bpc / Vertical_8bpc) with host-built

@@ -9,6 +9,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <functional>
+#include <limits>
 #include <map>
 #include <memory>
 #include <mutex>
@@ -2374,6 +2375,44 @@ void pil_bicubic_tables(int in_size, int out_size, std::vector<int>& bounds, std
         bounds[2 * xx] = xmin; bounds[2 * xx + 1] = xmax;
     }
 }
+
+// cv2.getGaussianKernel(11, 1.5) (core/metrics.py:58): g_i = exp(-(i-5)^2 / (2 * 1.5^2)), normalised to sum 1
+SsimWindow ssim_window() {
+    SsimWindow w;
+    double s = 0.0;
+    for (int i = 0; i < SSIM_TAPS; ++i) {
+        const double x = i - (SSIM_TAPS - 1) / 2;
+        w.g[i] = std::exp(-0.5 / (1.5 * 1.5) * x * x);
+        s += w.g[i];
+    }
+    const double inv = 1.0 / s;
+    for (int i = 0; i < SSIM_TAPS; ++i) w.g[i] *= inv;
+    return w;
+}
+
+// SSIM of n pairs of HWC images (dtype 0 uint8, 1 float64) into out[n] (DEVICE), asynchronously on st.  An image smaller than the window
+// in either direction has an empty valid region: its value is NaN (the reference's mean of an empty crop), written here without a kernel.
+void launch_ssim(const void* a, const void* b, int dtype, int n, int H, int W, int C, double* out, DevAllocs& mem, cudaStream_t st) {
+    const int Hv = H - (SSIM_TAPS - 1), Wv = W - (SSIM_TAPS - 1);
+    if (Hv < 1 || Wv < 1) {
+        const std::vector<double> nan((size_t)n, std::numeric_limits<double>::quiet_NaN());
+        CK(cudaMemcpyAsync(out, nan.data(), (size_t)n * sizeof(double), cudaMemcpyHostToDevice, st));
+        CK(cudaStreamSynchronize(st));           // `nan` is pageable host memory that dies with this call
+        return;
+    }
+    const dim3 grid((Wv + SSIM_TW - 1) / SSIM_TW, (Hv + SSIM_TH - 1) / SSIM_TH, n);
+    const int tiles = (int)(grid.x * grid.y);
+    double* partial = static_cast<double*>(mem.alloc((size_t)n * tiles * sizeof(double), false));
+    const SsimWindow win = ssim_window();
+    if (dtype == 0)
+        ssim_kernel<unsigned char><<<grid, SSIM_THREADS, 0, st>>>(static_cast<const unsigned char*>(a), static_cast<const unsigned char*>(b), H, W, C,
+                                                                   win, partial);
+    else
+        ssim_kernel<double><<<grid, SSIM_THREADS, 0, st>>>(static_cast<const double*>(a), static_cast<const double*>(b), H, W, C, win, partial);
+    CK(cudaGetLastError());
+    ssim_finish_kernel<<<(n + 127) / 128, 128, 0, st>>>(partial, tiles, (double)Hv * Wv * C, n, out);
+    CK(cudaGetLastError());
+}
 }  // namespace
 
 extern "C" {
@@ -2443,6 +2482,50 @@ int sr3_ssd_u8(const unsigned char* a, const unsigned char* b, int64_t n, unsign
     CK(cudaGetLastError());
     CK(cudaMemcpyAsync(ssd_host, d, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
+    API_END
+}
+
+// ssim (core/metrics.py:52-72) of n pairs of DEVICE images [n][H][W][C] (dtype 0 uint8, 1 float64) -> ssim_host[n] (see ssim_kernel).
+int sr3_ssim(const void* a, const void* b, int dtype, int n, int H, int W, int C, double* ssim_host, void* stream) {
+    API_BEGIN
+    REQUIRE(a && b && ssim_host && (dtype == 0 || dtype == 1) && n >= 1 && n <= 65535 && H >= 1 && W >= 1 && C >= 1, "bad ssim arguments");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    DevAllocs mem;
+    double* d = static_cast<double*>(mem.alloc((size_t)n * sizeof(double), false));
+    launch_ssim(a, b, dtype, n, H, W, C, d, mem, st);
+    CK(cudaMemcpyAsync(ssim_host, d, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    API_END
+}
+
+// The evaluation of a sampled batch (sr.py:216-217 for every image): tensor2img of sr[i] and hr[i] (fp32 DEVICE [n][C][H][W]) into uint8 HWC
+// images (sr_u8 / hr_u8: DEVICE [n][H][W][C], or NULL for scratch), then per pair the exact integer SSD (calculate_psnr) and the SSIM of
+// ssim_kernel.  Both results come back in one device-to-host copy.
+int sr3_image_metrics(const float* sr, const float* hr, int n, int C, int H, int W, float min_v, float max_v, unsigned char* sr_u8, unsigned char* hr_u8,
+                      unsigned long long* ssd_host, double* ssim_host, void* stream) {
+    API_BEGIN
+    REQUIRE(sr && hr && ssd_host && ssim_host && n >= 1 && n <= 65535 && C >= 1 && H >= 1 && W >= 1 && max_v > min_v, "bad image_metrics arguments");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    DevAllocs mem;
+    const long long per = 1LL * H * W * C;
+    if (!sr_u8) sr_u8 = static_cast<unsigned char*>(mem.alloc((size_t)(n * per), false));
+    if (!hr_u8) hr_u8 = static_cast<unsigned char*>(mem.alloc((size_t)(n * per), false));
+    // results: n SSDs then n SSIMs (both 8 bytes), one copy back
+    unsigned long long* res = static_cast<unsigned long long*>(mem.alloc((size_t)n * 16, false));
+    CK(cudaMemsetAsync(res, 0, (size_t)n * sizeof(unsigned long long), st));
+    const dim3 grid((unsigned)std::min<long long>((per + 255) / 256, num_sms() * 8LL), n);
+    tensor2img_kernel<<<grid, 256, 0, st>>>(sr, sr_u8, 1, C, H, W, 1, H, W, min_v, max_v);
+    CK(cudaGetLastError());
+    tensor2img_kernel<<<grid, 256, 0, st>>>(hr, hr_u8, 1, C, H, W, 1, H, W, min_v, max_v);
+    CK(cudaGetLastError());
+    ssd_u8_kernel<<<grid, 256, 0, st>>>(sr_u8, hr_u8, per, res);
+    CK(cudaGetLastError());
+    launch_ssim(sr_u8, hr_u8, 0, n, H, W, C, reinterpret_cast<double*>(res + n), mem, st);
+    std::vector<unsigned long long> host((size_t)n * 2);
+    CK(cudaMemcpyAsync(host.data(), res, (size_t)n * 16, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    memcpy(ssd_host, host.data(), (size_t)n * sizeof(unsigned long long));
+    memcpy(ssim_host, host.data() + n, (size_t)n * sizeof(double));
     API_END
 }
 

@@ -162,6 +162,16 @@ int sr3_tensor2img(const float* src, unsigned char* dst_u8, int n, int C, int H,
 /* core/metrics.py:42-50 `calculate_psnr`: exact integer sum of squared differences of two uint8 DEVICE images (n elements) -> *ssd_host;
  * PSNR = 20 log10(255 / sqrt(ssd / n)) is formed by the caller in float64 as the reference does. */
 int sr3_ssd_u8(const unsigned char* a_u8, const unsigned char* b_u8, int64_t n, unsigned long long* ssd_host, void* stream);
+/* core/metrics.py:52-72 `ssim` of n image pairs: a, b DEVICE [n][H][W][C] (HWC; dtype 0 uint8, 1 float64) -> ssim_host[n] (HOST).  fp64
+ * throughout: the 11x11 Gaussian window (sigma 1.5) as two separable passes over x, y, x^2, y^2, xy, valid pixels only, each channel on its
+ * own, mean over every kept pixel of every channel; NaN when H or W is below 11.  The work split depends on (H, W, C) only: a pair scores
+ * bit-identically alone or inside any batch.  calculate_ssim (:75-93) is formed by the caller. */
+int sr3_ssim(const void* a, const void* b, int dtype, int n, int H, int W, int C, double* ssim_host, void* stream);
+/* The evaluation of a sampled batch (sr.py:216-217 for every image): tensor2img (as sr3_tensor2img with n == 1) of each of the n images of
+ * sr_f32 and hr_f32 (DEVICE fp32 [n][C][H][W]) into uint8 [n][H][W][C] (sr_u8 / hr_u8 DEVICE, or NULL: internal scratch), then per pair
+ * the sr3_ssd_u8 sum (ssd_host[n]) and the sr3_ssim value (ssim_host[n]), in one call with one device-to-host copy. */
+int sr3_image_metrics(const float* sr_f32, const float* hr_f32, int n, int C, int H, int W, float min_v, float max_v, unsigned char* sr_u8,
+                      unsigned char* hr_u8, unsigned long long* ssd_host, double* ssim_host, void* stream);
 
 /* Entrance of the path: the conditioning image.  data/prepare_data.py:17-40 `trans_fn.resize(img, size, Image.BICUBIC)` (Pillow's two-pass
  * fixed-point bicubic resampler on uint8) + data/util.py:74-83 `transform_augment` (ToTensor, optional horizontal flip, range mapping).
