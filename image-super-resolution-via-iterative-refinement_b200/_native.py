@@ -36,6 +36,18 @@ class TestConvArgsC(ctypes.Structure):
                [(n, c_int) for n in ("B", "H", "W", "Cin", "Cout", "Cin2", "ksize", "stride", "fold_up", "precise")]
 
 
+class TestGroupNormArgsC(ctypes.Structure):
+    _fields_ = [(n, c_void_p) for n in ("x0", "x1", "st0", "st1", "gamma", "beta", "drop_mask", "dA", "add", "a_bf16", "mr", "dst0", "dst0_b",
+                                         "gsum0", "dst1", "dgamma", "dbeta")] + \
+               [("drop_seed", c_uint64)] + [(n, c_int) for n in ("B", "HW", "C0", "C1", "groups", "silu", "drop", "add_ld", "acc0")] + \
+               [("drop_layer", ctypes.c_uint), ("drop_p", c_float), ("gscale", c_float)]
+
+
+class TestFilmArgsC(ctypes.Structure):
+    _fields_ = [(n, c_void_p) for n in ("wf", "tau", "dfilm", "nl", "w1", "b1", "w2", "dwf", "dbf", "dcb", "dtau", "dw1", "db1", "dw2", "db2")] + \
+               [(n, c_int) for n in ("F", "inner", "B")] + [("gscale", c_float)]
+
+
 _SIGS = {
     "sr3_last_error": (c_char_p, []),
     "sr3_abi_version": (c_int, []),
@@ -97,6 +109,14 @@ _SIGS = {
     "sr3_tile_schedule": (c_int, [c_void_p, c_int, POINTER(GemmGeometryC), POINTER(c_int), POINTER(c_int)]),
     "sr3_test_wgrad": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float,
                                c_int, POINTER(c_int), c_void_p]),
+    "sr3_test_groupnorm_layer": (c_int, [POINTER(TestGroupNormArgsC), c_void_p]),
+    "sr3_test_grad_combine": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_int, c_int, c_int,
+                                      c_void_p]),
+    "sr3_test_dgrad": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    "sr3_test_attention_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
+                                       c_void_p]),
+    "sr3_test_film_embed_bwd": (c_int, [POINTER(TestFilmArgsC), c_void_p]),
+    "sr3_test_loss_grad": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, POINTER(c_double), c_void_p, c_int, c_void_p, c_void_p]),
 }
 EXPORTED_SYMBOLS = tuple(_SIGS.keys())
 
@@ -546,3 +566,104 @@ def test_conv_groupnorm(x_nhwc_bf16, w_oihw, bias, gamma, beta, groups, silu, ks
 def adam_step(table_dev, n_tensors, lr, beta1, beta2, eps, step, grad_scale=1.0):
     """torch.optim.Adam step over a device table of {param, grad, exp_avg, exp_avg_sq, numel} records (int64 [n, 5]) in one launch."""
     _check(lib().sr3_adam_step(_ptr(table_dev), int(n_tensors), float(lr), float(beta1), float(beta2), float(eps), int(step), float(grad_scale), _stream()))
+
+
+# ---- kernel-level hooks of the training backward (CUDA tensors in, CUDA tensors out; see include/sr3_b200.h)
+def test_groupnorm_layer(x0, st0, gamma, beta, groups, silu, dA, x1=None, st1=None, add=None, dst0=None, acc0=False, drop=None, gscale=1.0):
+    """GroupNorm(+SiLU, +Dropout) forward apply then backward, as the training plan pairs them.  x0 / x1 fp32 [B,HW,C0|C1], st fp64 [B,C,2],
+    dA fp32 [B,HW,C], add fp32 [B,HW,>=C], dst0 (initial, accumulated into when acc0) fp32 [B,HW,C0].  drop: None, ("philox", p, seed,
+    layer) or ("mask", p, uint8 [B,C,HW]).  Returns a dict: a (bf16), mr, dst0, dst0_b, gsum0, dst1, dgamma, dbeta."""
+    B, HW, C0 = x0.shape
+    C1 = 0 if x1 is None else x1.shape[2]
+    C = C0 + C1
+    dev = x0.device
+    out = {"a": torch.empty(B, HW, C, device=dev, dtype=torch.bfloat16), "mr": torch.empty(B, groups, 2, device=dev),
+           "dst0": dst0.clone() if dst0 is not None else torch.zeros(B, HW, C0, device=dev),
+           "dst0_b": torch.empty(B, HW, C0, device=dev, dtype=torch.bfloat16), "gsum0": torch.zeros(B, C0, device=dev),
+           "dst1": torch.empty(B, HW, C1, device=dev) if C1 else None, "dgamma": torch.empty(C, device=dev), "dbeta": torch.empty(C, device=dev)}
+    a = TestGroupNormArgsC()
+    for n, t in (("x0", x0), ("x1", x1), ("st0", st0), ("st1", st1), ("gamma", gamma), ("beta", beta), ("dA", dA), ("add", add)):
+        setattr(a, n, t.data_ptr() if t is not None else None)
+    for n in ("a_bf16", "mr", "dst0", "dst0_b", "gsum0", "dst1", "dgamma", "dbeta"):
+        k = "a" if n == "a_bf16" else n
+        setattr(a, n, out[k].data_ptr() if out[k] is not None else None)
+    a.B, a.HW, a.C0, a.C1, a.groups, a.silu = B, HW, C0, C1, groups, int(bool(silu))
+    a.add_ld = add.shape[2] if add is not None else 0
+    a.acc0, a.gscale = int(bool(acc0)), float(gscale)
+    if drop is not None:
+        if drop[0] == "philox":
+            a.drop, a.drop_p, a.drop_seed, a.drop_layer = 1, float(drop[1]), int(drop[2]), int(drop[3])
+        else:
+            a.drop, a.drop_p, a.drop_mask = 2, float(drop[1]), drop[2].data_ptr()
+    _check(lib().sr3_test_groupnorm_layer(ctypes.byref(a), _stream()))
+    return out
+
+
+def test_grad_combine(a, b=None, dst=None, acc=False, want_bf16=True, want_gsum=True, bias_outputs=0, gscale=1.0):
+    """grad_combine_kernel (+ bias_grad_kernel into bias_outputs = 0, 1 or 2 destinations).  a, b, dst fp32 [B,HW,C] (dst is updated in
+    place).  Returns (dst_b, gsum, [bias gradients])."""
+    B, HW, C = a.shape
+    dev = a.device
+    db = torch.empty(B, HW, C, device=dev, dtype=torch.bfloat16) if want_bf16 else None
+    gs = torch.zeros(B, C, device=dev) if want_gsum else None
+    bias = [torch.empty(C, device=dev) for _ in range(bias_outputs)]
+    _check(lib().sr3_test_grad_combine(_ptr(a), _ptr(b), _ptr(dst), int(bool(acc)), _ptr(db), _ptr(gs), _ptr(bias[0] if bias else None),
+                                       _ptr(bias[1] if len(bias) > 1 else None), float(gscale), B, HW, C, _stream()))
+    return db, gs, bias
+
+
+DGRAD_FORMS = {"conv": 0, "down": 1, "up": 2}
+
+
+def test_dgrad(dy, w_oihw, form, H, W):
+    """Data gradient on the tile kernel with the weight packed on the device (sr3_test_dgrad).  dy bf16 NHWC; w fp32 OIHW [Cout,Cin,k,k];
+    H, W: the conv's input size.  Returns dx fp32 [B,H,W,Cin]."""
+    B, CY = dy.shape[0], dy.shape[3]
+    Cout, Cin, k = w_oihw.shape[0], w_oihw.shape[1], w_oihw.shape[2]
+    dx = torch.empty(B, H, W, Cin, device=dy.device)
+    w = _f32c(w_oihw, dy.device)
+    _check(lib().sr3_test_dgrad(_ptr(dy), _ptr(w), _ptr(dx), DGRAD_FORMS[form], B, H, W, CY, Cin, Cout, k, _stream()))
+    return dx
+
+
+def test_attention_bwd(qk, vT, P, dO, nz, Lt, HW, C):
+    """Attention backward from the transposes to the bf16 copy of d(qkv).  Returns (dS fp32 [nz*Lt,Lt], dS bf16, dqkv fp32 [nz*Lt,3C],
+    dqkv bf16)."""
+    dev = qk.device
+    dS = torch.empty(nz * Lt, Lt, device=dev)
+    dSb = torch.empty(nz * Lt, Lt, device=dev, dtype=torch.bfloat16)
+    dqkv = torch.empty(nz * Lt, 3 * C, device=dev)
+    dqkvb = torch.empty(nz * Lt, 3 * C, device=dev, dtype=torch.bfloat16)
+    _check(lib().sr3_test_attention_bwd(_ptr(qk), _ptr(vT), _ptr(P), _ptr(dO), _ptr(dS), _ptr(dSb), _ptr(dqkv), _ptr(dqkvb), nz, Lt, HW, C, _stream()))
+    return dS, dSb, dqkv, dqkvb
+
+
+def test_film_embed_bwd(wf, tau, dfilm, nl, w1, b1, w2, gscale=1.0):
+    """film_bwd_kernel + embed_bwd_kernel.  Returns a dict: dwf, dbf, dcb, dtau, dw1, db1, dw2, db2."""
+    F, inner = wf.shape
+    B = tau.shape[0]
+    dev = wf.device
+    out = {"dwf": torch.empty(F, inner, device=dev), "dbf": torch.empty(F, device=dev), "dcb": torch.empty(F, device=dev),
+           "dtau": torch.empty(B, inner, device=dev), "dw1": torch.empty(4 * inner, inner, device=dev), "db1": torch.empty(4 * inner, device=dev),
+           "dw2": torch.empty(inner, 4 * inner, device=dev), "db2": torch.empty(inner, device=dev)}
+    a = TestFilmArgsC()
+    for n, t in (("wf", wf), ("tau", tau), ("dfilm", dfilm), ("nl", nl), ("w1", w1), ("b1", b1), ("w2", w2)):
+        setattr(a, n, t.data_ptr())
+    for n, t in out.items():
+        setattr(a, n, t.data_ptr())
+    a.F, a.inner, a.B, a.gscale = F, inner, B, float(gscale)
+    _check(lib().sr3_test_film_embed_bwd(ctypes.byref(a), _stream()))
+    return out
+
+
+def test_loss_grad(noise, eps, l2, deps=None, ld=64):
+    """loss_grad_kernel.  noise, eps fp32 NCHW.  deps: bf16 [B,H,W,ld] updated in place (fresh zeros by default).  Returns (loss, deps,
+    bias_sum [C])."""
+    B, C, H, W = noise.shape
+    if deps is None:
+        deps = torch.zeros(B, H, W, ld, device=noise.device, dtype=torch.bfloat16)
+    bias = torch.zeros(C, device=noise.device)
+    loss = c_double()
+    _check(lib().sr3_test_loss_grad(_ptr(noise), _ptr(eps), B, C, H, W, int(bool(l2)), ctypes.byref(loss), _ptr(deps), deps.shape[3], _ptr(bias),
+                                    _stream()))
+    return loss.value, deps, bias

@@ -888,6 +888,224 @@ void init_wgrad_attrs() {
     if (first_use_on_device(seen)) CK(cudaFuncSetAttribute(wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WGRAD_SMEM_BYTES));
 }
 
+// ---- GroupNorm / elementwise launches of the plan, shared by the layer builders and the stand-alone test hooks.  Every thread owns one
+// 4-channel column and walks the pixels of its block kpix at a time; grid = (blocks per image, images).
+struct RowLaunch { int threads = 0, ppb = 0, smem = 0; dim3 grid; };
+// the GroupNorm op a = act(GN(cat(src0, src1))) as prep_kernel and gn_bwd_kernel both see it (no outputs, launch shape or dropout yet)
+PrepParams gn_op(const float* src0, const double* st0, int C0, const float* src1, const double* st1, int C1, const float* gamma, const float* beta,
+                 int groups, int HW, bool silu) {
+    PrepParams p{};
+    p.src0 = src0; p.st0 = st0; p.C0 = C0;
+    p.src1 = src1; p.st1 = st1; p.C1 = C1;
+    p.gamma = gamma; p.beta = beta; p.groups = groups; p.HW = HW; p.silu = silu ? 1 : 0; p.eps = 1e-5f;
+    const int C = C0 + C1;
+    REQUIRE(C % groups == 0 && C % 4 == 0 && C0 % 4 == 0, "bad GroupNorm geometry C=%d groups=%d", C, groups);
+    REQUIRE(C / 4 <= 512, "GroupNorm over %d channels is not supported", C);
+    return p;
+}
+// prep_kernel: ONE wave of blocks.  The kernel uses 64 registers per thread, i.e. 4 resident 256-thread blocks (2 of 512) per SM; a grid
+// sized for 8 per SM (round 1, 32-register version) runs as two waves and pays the statistics set-up twice (24 vs 15 us on the 128x128 level).
+RowLaunch prep_launch(int C, int groups, int HW, int B) {
+    const int vpp = C / 4;
+    const int kpix = vpp >= 256 ? 1 : 256 / vpp;
+    RowLaunch L; L.threads = vpp * kpix;                         // <= 512, every thread owns one 4-channel column
+    const int per_sm = L.threads > 256 ? 2 : 4;
+    int bpi = per_sm * num_sms() / B; if (bpi < 1) bpi = 1;    // blocks per image
+    const int q = kpix * 4;                                    // 4 loads in flight per thread
+    int ppb = (HW + bpi - 1) / bpi;
+    ppb = ((ppb + q - 1) / q) * q;
+    if (ppb < q) ppb = q;
+    if (ppb > HW) ppb = HW;
+    L.ppb = ppb; L.grid = dim3((HW + ppb - 1) / ppb, B); L.smem = (2 * C + 2 * groups) * sizeof(float);
+    return L;
+}
+void launch_prep(const PrepParams& p, const RowLaunch& L, cudaStream_t st) {
+    if (p.drop) launch_k(prep_kernel<true>, L.grid, dim3(L.threads), (size_t)L.smem, st, p);
+    else launch_k(prep_kernel<false>, L.grid, dim3(L.threads), (size_t)L.smem, st, p);
+}
+// gn_bwd_kernel, measured (8 images, 16->128): 64 pixel rows per thread column and ~4 blocks per SM beat 32 / 8 (2.67 -> 2.53 ms) and
+// 128 / 2 (3.06 ms)
+RowLaunch gn_bwd_launch(int C, int groups, int HW, int B) {
+    const int vpp = C / 4;
+    const int kpix = vpp >= 256 ? 1 : 256 / vpp;
+    RowLaunch L; L.threads = vpp * kpix;
+    int ppb = kpix * 64;
+    { const int cap = (int)(((long long)HW * B) / 592); if (ppb > cap) ppb = cap; }
+    if (ppb < kpix * 4) ppb = kpix * 4;
+    if (ppb > HW) ppb = HW;
+    L.ppb = ppb; L.grid = dim3((HW + ppb - 1) / ppb, B); L.smem = gn_bwd_smem_bytes(C, groups);
+    return L;
+}
+// both passes; p.sums must be zero
+void launch_gn_bwd(const GnBwdParams& p, const RowLaunch& L, cudaStream_t st) {
+    launch_k(gn_bwd_kernel<false>, L.grid, dim3(L.threads), (size_t)L.smem, st, p);
+    launch_k(gn_bwd_kernel<true>, L.grid, dim3(L.threads), (size_t)L.smem, st, p);
+}
+RowLaunch combine_launch(int C, int HW, int B) {
+    const int vpp = C / 4;
+    REQUIRE(C % 4 == 0 && vpp <= 256, "combine over %d channels", C);
+    const int kpix = 256 / vpp;
+    RowLaunch L; L.threads = vpp * kpix;
+    int ppb = kpix * 32;
+    { const int cap = (int)(((long long)HW * B) / 1184); if (ppb > cap) ppb = cap; }
+    if (ppb < kpix) ppb = kpix;
+    if (ppb > HW) ppb = HW;
+    L.ppb = ppb; L.grid = dim3((HW + ppb - 1) / ppb, B); L.smem = C * 4;
+    return L;
+}
+void launch_combine(const RowLaunch& L, const float* a, const float* b2, float* dst, int acc, bf16* dst_b, float* gsum, int B, int HW, int C, cudaStream_t st) {
+    launch_k(grad_combine_kernel, L.grid, dim3(L.threads), (size_t)L.smem, st, a, b2, dst, acc, dst_b, gsum, B, HW, C, L.ppb);
+}
+void launch_bias_grad(const float* gsum, int ld, float* d0, float* d1, int B, int C, float gscale, cudaStream_t st) {
+    bias_grad_kernel<<<(C + 255) / 256, 256, 0, st>>>(gsum, ld, d0, d1, B, C, gscale);
+    CK(cudaGetLastError());
+}
+void launch_loss_grad(const float* noise, const float* eps, int B, int C, int H, int W, int l2, double* loss, bf16* deps, int ld, float* bias_sum,
+                      cudaStream_t st) {
+    loss_grad_kernel<<<296, 256, 0, st>>>(noise, eps, B, C, H, W, l2, loss, deps, ld, bias_sum);
+    CK(cudaGetLastError());
+}
+
+// ---- FiLM projections + noise-level MLP backward: one block's shared memory holds every image's embedding (and the MLP's hidden layer)
+constexpr int FILM_BWD_SMEM_MAX = 200 * 1024;
+int film_bwd_smem(int B, int inner) { return 2 * B * inner * 4; }
+int embed_bwd_smem(int B, int inner) { return (2 * B * inner + 2 * B * 4 * inner) * 4; }
+// dtau must be zero
+void launch_film_bwd(const float* wf, const float* tau, const float* dfilm, float* dwf, float* dbf, float* dcb, float* dtau, int F, int inner, int B,
+                     float gscale, cudaStream_t st) {
+    const int smem = film_bwd_smem(B, inner);
+    static std::vector<int> seen;
+    if (first_use_on_device(seen)) CK(cudaFuncSetAttribute(film_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FILM_BWD_SMEM_MAX));
+    REQUIRE(smem <= FILM_BWD_SMEM_MAX, "FiLM backward: batch %d too large for one block's shared memory", B);
+    film_bwd_kernel<<<(F + 63) / 64, 256, smem, st>>>(wf, tau, dfilm, dwf, dbf, dcb, dtau, F, inner, B, gscale);
+    CK(cudaGetLastError());
+}
+void launch_embed_bwd(const float* nl, const float* w1, const float* b1, const float* w2, const float* dtau, float* dw1, float* db1, float* dw2, float* db2,
+                      int inner, int B, float gscale, cudaStream_t st) {
+    const int esm = embed_bwd_smem(B, inner);
+    static std::vector<int> seen;
+    if (first_use_on_device(seen)) CK(cudaFuncSetAttribute(embed_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FILM_BWD_SMEM_MAX));
+    REQUIRE(esm <= FILM_BWD_SMEM_MAX, "noise-level MLP backward: batch %d too large for one block", B);
+    embed_bwd_kernel<<<1, 256, esm, st>>>(nl, w1, b1, w2, dtau, dw1, db1, dw2, db2, inner, B, gscale);
+    CK(cudaGetLastError());
+}
+
+// ---- data gradients on the forward tile kernel
+// the packed weight of a data gradient (pack_entry types 2, 3, 4; the source parameter is filled in when it is packed):
+//   2: stride-1 conv, Cout -> Cin, k x k: rows Cin, k*k*cout_pad columns (mirrored taps, cout_pad = Cout rounded up to 64)
+//   3: Downsample, C -> C: four phase matrices of rows_pad rows x 4C columns
+//   4: Upsample, C -> C: rows C, 16C columns (the 4x4 kernel)
+PackDesc dgrad_pack_desc(int type, void* dst, int Cout, int Cin, int k) {
+    PackDesc d{}; d.type = type; d.dst = dst; d.Cout = Cout; d.Cin = Cin;
+    if (type == 2) {
+        const int cout_pad = ((Cout + 63) / 64) * 64;
+        d.k = k; d.ld = k * k * cout_pad; d.tap_stride = cout_pad;
+    } else if (type == 3) {
+        d.rows_pad = ((Cin + 127) / 128) * 128;
+    }
+    return d;
+}
+// bf16 elements of the packed weight of dgrad_pack_desc (rows padded to 128)
+size_t dgrad_weight_elems(int type, int Cout, int Cin, int k) {
+    const size_t rows_pad = ((Cin + 127) / 128) * 128;
+    if (type == 2) return rows_pad * k * k * (((Cout + 63) / 64) * 64);
+    if (type == 3) return 4 * rows_pad * 4 * Cin;
+    return rows_pad * 16 * Cin;
+}
+// dX = conv_k(dY, W') of a stride-1 conv: A bf16 [Bp][H][W][CA] (CA: dY channels, >= Cout: the final conv reads 3 of 64); out fp32 [Bp][H][W][N]
+ConvArgs dgrad_conv(const bf16* A, int Bp, int CA, int Hh, int Ww, int k, const bf16* w, int N, float* out, bf16* out_b) {
+    ConvArgs c; c.n_a = 1; c.a[0] = nhwc_src(A, Bp, Hh, Ww, CA); c.c0 = CA;
+    add_conv_slabs(c.slabs, 0, CA, k, 1, 0);
+    c.w = w; c.ktot = k * k * CA; c.cout = N; c.OH = Hh; c.OW = Ww;
+    Act o; o.p = out; o.C = N; o.H = Hh; o.W = Ww; c.out = o;
+    c.raw_out = out_b;
+    return c;
+}
+// Downsample (conv3x3 stride 2): four input-parity phases on the low-resolution dY grid (bf16 [Bp][yH][yW][C]) -> out fp32 [Bp][2yH][2yW][C]
+ConvArgs downsample_dgrad_conv(const bf16* dy, int Bp, int yH, int yW, int C, const bf16* w, float* out) {
+    ConvArgs c; c.n_a = 1; c.a[0] = nhwc_src(dy, Bp, yH, yW, C); c.c0 = C;
+    for (int a = 0; a < 2; ++a)
+        for (int bb = 0; bb < 2; ++bb)
+            for (int ch = 0; ch < C; ch += 64) { KSlab k; k.a_sel = 0; k.a_chan = ch; k.dh = -1 + a; k.dw = -1 + bb; k.p = 0; k.b_col = (a * 2 + bb) * C + ch; c.slabs.push_back(k); }
+    c.w = w; c.ktot = 4 * C; c.cout = C; c.OH = yH; c.OW = yW;
+    Act o; o.p = out; o.C = C; o.H = yH; o.W = yW; c.out = o;
+    c.custom_os = true;
+    c.os.sZ = 0; c.os.sB = 4LL * yH * yW * C; c.os.sH = 4LL * yW * C; c.os.sW = 2LL * C; c.os.off = 0;
+    c.nz = 4; c.b_zrows = ((C + 127) / 128) * 128; c.z_phase = 1; c.z_off_hi = 2LL * yW * C; c.z_off_lo = C;
+    return c;
+}
+// Upsample (nearest 2x -> conv3x3): dX[i][j] = sum_{u,v} K[u][v] dY[2i-1+u][2j-1+v], a 4x4 stride-2 conv over dY (bf16 [Bp][yH][yW][C]) in
+// the parity view -> out fp32 [Bp][yH/2][yW/2][C]
+ConvArgs upsample_dgrad_conv(const bf16* dy, int Bp, int yH, int yW, int C, const bf16* w, float* out) {
+    ConvArgs c; c.n_a = 1; c.a[0] = nhwc_stride2_src(dy, Bp, yH, yW, C); c.c0 = C;
+    for (int u = 0; u < 4; ++u)
+        for (int v = 0; v < 4; ++v)
+            for (int ch = 0; ch < C; ch += 64) {
+                KSlab k; k.a_sel = 0; k.b_col = (u * 4 + v) * C + ch;
+                k.dh = (u == 0) ? -1 : (u == 3 ? 1 : 0); k.p = (u == 0 || u == 2) ? 1 : 0;
+                k.dw = (v == 0) ? -1 : (v == 3 ? 1 : 0); k.a_chan = ((v == 0 || v == 2) ? C : 0) + ch;
+                c.slabs.push_back(k);
+            }
+    c.w = w; c.ktot = 16 * C; c.cout = C; c.OH = yH / 2; c.OW = yW / 2;
+    Act o; o.p = out; o.C = C; o.H = yH / 2; o.W = yW / 2; c.out = o;
+    return c;
+}
+
+// ---- attention backward: the four matrix products of nz attention batches of Lt tokens, head dim C
+// dP[z] = dO V^T: rows = queries, N = keys, K = head dim.  dOb bf16 [nz][Lt][C], V bf16 [nz][Lt][C] -> dS fp32 [nz][Lt][Lt]
+GemmDesc attn_bwd_dp_desc(const bf16* dOb, const bf16* v, float* dS, int nz, int Lt, int C) {
+    GemmDesc d; d.n_a = 1; d.a[0] = matrix_src(dOb, nz, Lt, C, C, (long long)Lt * C);
+    for (int ch = 0; ch < C; ch += 64) d.slabs.push_back({0, ch, 0, 0, 0, ch});
+    d.block_n = 128; d.b_ptr = v; d.b_K = C; d.b_rows = (long long)nz * Lt;
+    d.w_box = 128; d.h_box = 1; d.b_box = 1; d.tiles_w = Lt / 128; d.tiles_h = 1; d.tiles_b = 1;
+    d.n_tiles = Lt / 128; d.nz = nz; d.a_zstep = 1; d.b_zrows = Lt;
+    d.OW = Lt; d.OH = 1; d.OB = nz; d.n_valid = Lt;
+    d.out_f32 = dS; d.os = OutSpec{0, (long long)Lt * Lt, 0, Lt, 0};
+    return d;
+}
+// dQ[z] = dS K: rows = queries, N = head dim, K = keys.  dSb bf16 [nz][Lt][Lt], K^T bf16 [nz][C][Lt] -> dqkv[:, 0:C] (rows of 3C floats)
+GemmDesc attn_bwd_dq_desc(const bf16* dSb, const bf16* kT, float* dqkv, int nz, int Lt, int C) {
+    GemmDesc d; d.n_a = 1; d.a[0] = matrix_src(dSb, nz, Lt, Lt, Lt, (long long)Lt * Lt);
+    for (int ch = 0; ch < Lt; ch += 64) d.slabs.push_back({0, ch, 0, 0, 0, ch});
+    d.block_n = 128; d.b_ptr = kT; d.b_K = Lt; d.b_rows = (long long)nz * C;
+    d.w_box = 128; d.h_box = 1; d.b_box = 1; d.tiles_w = Lt / 128; d.tiles_h = 1; d.tiles_b = 1;
+    d.n_tiles = C / 128; d.nz = nz; d.a_zstep = 1; d.b_zrows = C;
+    d.OW = Lt; d.OH = 1; d.OB = nz; d.n_valid = C;
+    d.out_f32 = dqkv; d.os = OutSpec{0, (long long)Lt * 3 * C, 0, (long long)3 * C, 0};
+    return d;
+}
+// dK = dS^T Q and dV = P^T dO contract over the QUERY index: the weight-gradient kernel's batched form with the tokens of an attention batch
+// as a 16-wide "image" of 8x8 patches and the keys as its "output channels".  Q is read inside the q|k rows (2C wide) of qk.
+ASrc attn_bwd_q_view(const bf16* qk, int nz, int Lt, int C) {
+    ASrc q; q.ptr = qk; q.C = C; q.W = 16; q.P = 1; q.H = Lt / 16; q.Bn = nz;
+    q.sW = 2LL * 2 * C; q.sP = 2LL * 16 * 2 * C; q.sH = 2LL * 16 * 2 * C; q.sB = 2LL * Lt * 2 * C;
+    return q;
+}
+void launch_transpose_bf16(const bf16* src, bf16* dst, int R, int Cc, long long src_ld, long long src_z, long long dst_z, int nzb, cudaStream_t st) {
+    launch_k(transpose_bf16_kernel, dim3((Cc + 31) / 32, (R + 31) / 32, nzb), dim3(256), 0, st, src, dst, R, Cc, src_ld, src_z, dst_z);
+}
+// vT[z][d][key] (the forward's) -> V[z][key][d]
+void launch_v_from_vT(const bf16* vT, bf16* v, int nz, int Lt, int C, cudaStream_t st) {
+    launch_transpose_bf16(vT, v, C, Lt, Lt, (long long)C * Lt, (long long)Lt * C, nz, st);
+}
+// K[z][key][d] inside the q|k rows -> K^T[z][d][key]
+void launch_kT_from_qk(const bf16* qk, bf16* kT, int nz, int Lt, int C, cudaStream_t st) {
+    launch_transpose_bf16(qk + C, kT, Lt, C, 2 * C, (long long)Lt * 2 * C, (long long)C * Lt, nz, st);
+}
+// dS = P * (dP - rowsum(P dP)) / sqrt(C) in place on dP = dS fp32 [nz][Lt][Lt], over the seg-token segments of each row; dSb = bf16(dS)
+void launch_softmax_bwd(const bf16* P, float* dS, bf16* dSb, int nz, int Lt, int seg, int C, cudaStream_t st) {
+    const long long rows = (long long)nz * Lt;
+    launch_k(softmax_bwd_kernel, dim3((int)((rows + 7) / 8)), dim3(256), 0, st, P, dS, dSb, rows, Lt, seg, 1.0f / sqrtf((float)C));
+}
+void launch_cast_bf16(const float* src, bf16* dst, long long n4, cudaStream_t st) {
+    launch_k(cast_bf16_kernel, dim3((int)std::min<long long>((n4 + 255) / 256, 2368)), dim3(256), 0, st, src, dst, n4);
+}
+// where such a product lands: columns [col, col + C) of the 3C-wide d(qkv) rows, one slice per attention batch
+WgradOut attn_bwd_qkv_out(float* dqkv, int col, int nz, int Lt, int C) {
+    WgradOut o; o.ptr = dqkv ? dqkv + col : nullptr; o.slice_stride = (long long)Lt * 3 * C; o.row_stride = 3LL * C; o.nb = nz;
+    return o;
+}
+
 }  // namespace
 
 struct sr3_engine {
@@ -1081,35 +1299,14 @@ struct sr3_engine {
     float* last_mr = nullptr;              // training plan: (mean, rstd) buffer written by the most recent add_prep, read by its backward
     void add_prep(const Act& s0, const Act* s1, const float* gamma, const float* beta, int groups, bool silu, bf16* out_a, bf16* out_raw, const DropSpec* drop = nullptr) {
         if (dry) return;
-        PrepParams p{};
+        PrepParams p = gn_op(s0.p, s0.stats, s0.C, s1 ? s1->p : nullptr, s1 ? s1->stats : nullptr, s1 ? s1->C : 0, gamma, beta, groups, s0.H * s0.W, silu);
         p.drop = drop;
         if (train) { last_mr = static_cast<float*>(mem.alloc((size_t)Bp * groups * 2 * sizeof(float))); p.save_mr = last_mr; }
-        p.src0 = s0.p; p.st0 = s0.stats; p.C0 = s0.C;
-        p.src1 = s1 ? s1->p : nullptr; p.st1 = s1 ? s1->stats : nullptr; p.C1 = s1 ? s1->C : 0;
-        p.gamma = gamma; p.beta = beta; p.groups = groups; p.HW = s0.H * s0.W; p.silu = silu ? 1 : 0; p.eps = 1e-5f;
         p.out_a = out_a; p.out_raw = out_raw; p.precise = precise ? 1 : 0;
         const int C = p.C0 + p.C1;
-        REQUIRE(C % groups == 0 && C % 4 == 0 && p.C0 % 4 == 0, "bad GroupNorm geometry C=%d groups=%d", C, groups);
         const int vpp = C / 4;
-        REQUIRE(vpp <= 512, "GroupNorm over %d channels is not supported", C);
-        const int kpix = vpp >= 256 ? 1 : 256 / vpp;
-        const int threads = vpp * kpix;                                // <= 512, every thread owns one 4-channel column
-        // ONE wave of blocks: the kernel uses 64 registers per thread, i.e. 4 resident 256-thread blocks (2 of 512) per SM; a grid sized
-        // for 8 per SM (round 1, 32-register version) runs as two waves and pays the statistics set-up twice (24 vs 15 us on the 128x128
-        // level).
-        int ppb;
-        {
-            const int per_sm = threads > 256 ? 2 : 4;
-            int bpi = per_sm * num_sms() / B; if (bpi < 1) bpi = 1;    // blocks per image
-            const int q = kpix * 4;                                    // 4 loads in flight per thread
-            ppb = (p.HW + bpi - 1) / bpi;
-            ppb = ((ppb + q - 1) / q) * q;
-            if (ppb < q) ppb = q;
-            if (ppb > p.HW) ppb = p.HW;
-        }
-        p.pix_per_block = ppb;
-        const dim3 grid((p.HW + ppb - 1) / ppb, B);
-        const int smem = (2 * C + 2 * groups) * sizeof(float);
+        const RowLaunch L = prep_launch(C, groups, p.HW, B);
+        p.pix_per_block = L.ppb;
         {   // the same op inside the persistent step kernel: B x items_per_image work items dealt contiguously to the CTAs
             PrepParams m = p;
             const int nth = GEMM_THREADS;
@@ -1121,10 +1318,7 @@ struct sr3_engine {
             m.pix_per_block = mp; m.items_per_image = (p.HW + mp - 1) / mp; m.B = B;
             mega_record(MOP_PREP, m);
         }
-        push([p, grid, smem, threads](cudaStream_t st) {
-            if (p.drop) launch_k(prep_kernel<true>, grid, dim3(threads), (size_t)smem, st, p);
-            else launch_k(prep_kernel<false>, grid, dim3(threads), (size_t)smem, st, p);
-        }, 1, 0, (double)B * p.HW * C * (4.0 + 2.0 + (out_raw ? 2.0 : 0.0)));
+        push([p, L](cudaStream_t st) { launch_prep(p, L, st); }, 1, 0, (double)B * p.HW * C * (4.0 + 2.0 + (out_raw ? 2.0 : 0.0)));
     }
     void add_cast(const Act& s, bf16* dst, int up) {
         if (dry) return;
@@ -2540,16 +2734,151 @@ int sr3_test_conv_groupnorm(const void* x, const float* w_oihw, const float* bia
     double* stats = static_cast<double*>(mem.alloc((size_t)B * Cout * 2 * sizeof(double)));
     int rc = sr3_test_conv(x, w_oihw, bias, y, stats, B, H, W, Cin, Cout, ksize, 1, stream);
     if (rc) return rc;
-    PrepParams p{};
-    p.src0 = y; p.st0 = stats; p.C0 = Cout; p.C1 = 0;
-    p.gamma = gamma; p.beta = beta; p.groups = groups; p.HW = H * W; p.silu = silu; p.eps = 1e-5f;
-    p.out_a = static_cast<bf16*>(a_bf16); p.out_raw = nullptr;
-    const int vpp = Cout / 4;
-    REQUIRE(vpp <= 512, "too many channels");
-    const int kpix = vpp >= 256 ? 1 : 256 / vpp;
-    p.pix_per_block = kpix * 4; p.B = B; p.items_per_image = (p.HW + p.pix_per_block - 1) / p.pix_per_block;
-    const dim3 grid((p.HW + p.pix_per_block - 1) / p.pix_per_block, B);
-    launch_k(prep_kernel<false>, grid, dim3(vpp * kpix), (size_t)((2 * Cout + 2 * groups) * sizeof(float)), st, p);
+    PrepParams p = gn_op(y, stats, Cout, nullptr, nullptr, 0, gamma, beta, groups, H * W, silu != 0);
+    p.out_a = static_cast<bf16*>(a_bf16);
+    const RowLaunch L = prep_launch(Cout, groups, p.HW, B);      // the geometry of the engine's add_prep
+    p.pix_per_block = L.ppb;
+    launch_prep(p, L, st);
+    CK(cudaStreamSynchronize(st));
+    API_END
+}
+
+int sr3_test_groupnorm_layer(const sr3_test_groupnorm_args* a, void* stream) {
+    API_BEGIN
+    REQUIRE(a && a->x0 && a->st0 && a->gamma && a->beta && a->dA && a->a_bf16 && a->mr && a->dst0 && a->dgamma && a->dbeta, "null argument");
+    REQUIRE(a->C1 == 0 || (a->x1 && a->st1 && a->dst1), "second source without its statistics or gradient");
+    REQUIRE(a->drop >= 0 && a->drop <= 2 && (a->drop != 2 || a->drop_mask), "bad dropout source");
+    REQUIRE(a->B >= 1 && a->HW >= 1 && (!a->add || a->add_ld >= a->C0 + a->C1), "bad shape");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    DevAllocs mem;
+    const int C = a->C0 + a->C1;
+    DropSpec* drop = nullptr;
+    if (a->drop) {
+        DropSpec ds{}; ds.mask = a->drop == 2 ? a->drop_mask : nullptr; ds.p = a->drop_p; ds.layer = a->drop_layer; ds.seed = a->drop_seed;
+        drop = static_cast<DropSpec*>(mem.alloc(sizeof(DropSpec), false));
+        CK(cudaMemcpyAsync(drop, &ds, sizeof(ds), cudaMemcpyHostToDevice, st));
+    }
+    // forward apply, as add_prep launches it in a training plan
+    PrepParams f = gn_op(a->x0, a->st0, a->C0, a->x1, a->st1, a->C1, a->gamma, a->beta, a->groups, a->HW, a->silu != 0);
+    PrepParams fp = f;
+    fp.drop = drop; fp.save_mr = a->mr; fp.out_a = static_cast<bf16*>(a->a_bf16);
+    const RowLaunch Lf = prep_launch(C, a->groups, a->HW, a->B);
+    fp.pix_per_block = Lf.ppb;
+    launch_prep(fp, Lf, st);
+    // backward, as bwd_groupnorm launches it
+    GnBwdParams p; memset(&p, 0, sizeof(p));
+    p.f = f; p.f.B = a->B;
+    p.dA = a->dA; p.drop = drop; p.sums = static_cast<float*>(mem.alloc((size_t)a->B * C * 2 * sizeof(float))); p.add = a->add; p.add_ld = a->add_ld;
+    p.mr = a->mr;
+    p.dst0 = a->dst0; p.acc0 = a->acc0; p.dst0_b = static_cast<bf16*>(a->dst0_b); p.gsum0 = a->gsum0; p.gsum_ld0 = a->C0;
+    p.dst1 = a->dst1;
+    p.dgamma = a->dgamma; p.dbeta = a->dbeta; p.gscale = a->gscale;
+    const RowLaunch Lb = gn_bwd_launch(C, a->groups, a->HW, a->B);
+    p.f.pix_per_block = Lb.ppb;
+    launch_gn_bwd(p, Lb, st);
+    CK(cudaStreamSynchronize(st));
+    API_END
+}
+
+int sr3_test_grad_combine(const float* a, const float* b, float* dst, int acc, void* dst_b, float* gsum, float* bias0, float* bias1, float gscale,
+                          int B, int HW, int C, void* stream) {
+    API_BEGIN
+    REQUIRE(a && B >= 1 && HW >= 1 && (!bias0 || gsum) && (!acc || dst), "bad arguments");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    launch_combine(combine_launch(C, HW, B), a, b, dst, acc, static_cast<bf16*>(dst_b), gsum, B, HW, C, st);
+    if (bias0) launch_bias_grad(gsum, C, bias0, bias1, B, C, gscale, st);
+    CK(cudaStreamSynchronize(st));
+    API_END
+}
+
+int sr3_test_dgrad(const void* dy_bf16, const float* w_oihw, float* dx, int form, int B, int H, int W, int CY, int Cin, int Cout, int ksize,
+                   void* stream) {
+    API_BEGIN
+    REQUIRE(dy_bf16 && w_oihw && dx && B >= 1, "null argument");
+    REQUIRE((form == 0 && (ksize == 1 || ksize == 3) && CY == ((Cout + 63) / 64) * 64 && Cin % 64 == 0) ||
+            ((form == 1 || form == 2) && ksize == 3 && Cin == Cout && CY == Cin && Cin % 64 == 0), "bad data-gradient shape");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    DevAllocs mem;
+    const int type = form == 0 ? 2 : (form == 1 ? 3 : 4);
+    bf16* w = static_cast<bf16*>(mem.alloc(dgrad_weight_elems(type, Cout, Cin, ksize) * sizeof(bf16)));     // zero padding, as new_weight
+    PackDesc pd = dgrad_pack_desc(type, w, Cout, Cin, ksize);
+    pd.src = w_oihw;
+    pack_one(pd, st);
+    const bf16* dy = static_cast<const bf16*>(dy_bf16);
+    const ConvArgs c = form == 0 ? dgrad_conv(dy, B, CY, H, W, ksize, w, Cin, dx, nullptr)
+                     : form == 1 ? downsample_dgrad_conv(dy, B, H / 2, W / 2, Cin, w, dx)
+                                 : upsample_dgrad_conv(dy, B, 2 * H, 2 * W, Cin, w, dx);
+    GemmDesc d = conv_desc(c, B, B, 1);
+    d.out_imgs = B;
+    Op op = make_gemm_op(d, mem);
+    op(st);
+    CK(cudaStreamSynchronize(st));
+    API_END
+}
+
+int sr3_test_attention_bwd(const void* qk_bf16, const void* vT_bf16, const void* P_bf16, const void* dO_bf16, float* dS, void* dS_bf16, float* dqkv,
+                           void* dqkv_bf16, int nz, int Lt, int HW, int C, void* stream) {
+    API_BEGIN
+    REQUIRE(qk_bf16 && vT_bf16 && P_bf16 && dO_bf16 && dS && dS_bf16 && dqkv && dqkv_bf16, "null argument");
+    REQUIRE(nz >= 1 && Lt % 128 == 0 && C % 128 == 0 && HW >= 1 && Lt % HW == 0, "attention backward geometry Lt=%d HW=%d C=%d", Lt, HW, C);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    DevAllocs mem;
+    const bf16* qk = static_cast<const bf16*>(qk_bf16);
+    const bf16* P = static_cast<const bf16*>(P_bf16);
+    const bf16* dO = static_cast<const bf16*>(dO_bf16);
+    bf16* dSb = static_cast<bf16*>(dS_bf16);
+    bf16* v = static_cast<bf16*>(mem.alloc((size_t)nz * Lt * C * 2, false));
+    bf16* kT = static_cast<bf16*>(mem.alloc((size_t)nz * C * Lt * 2, false));
+    // the sequence of bwd_attention, from the transposes to the bf16 copy of d(qkv)
+    launch_v_from_vT(static_cast<const bf16*>(vT_bf16), v, nz, Lt, C, st);
+    launch_kT_from_qk(qk, kT, nz, Lt, C, st);
+    make_gemm_op(attn_bwd_dp_desc(dO, v, dS, nz, Lt, C), mem)(st);
+    launch_softmax_bwd(P, dS, dSb, nz, Lt, HW, C, st);
+    make_gemm_op(attn_bwd_dq_desc(dSb, kT, dqkv, nz, Lt, C), mem)(st);
+    init_wgrad_attrs();
+    const WgradOut ok = attn_bwd_qkv_out(dqkv, C, nz, Lt, C), ov = attn_bwd_qkv_out(dqkv, 2 * C, nz, Lt, C);
+    const std::vector<WgradTap> taps = taps_1x1();
+    {   // dK = dS^T Q
+        const WgradShape s = wgrad_shape(Lt, Lt / 16, 16, nz, C, 1, 0, &ok);
+        const WgradParams p = wgrad_params(s, dSb, Lt, Lt / 16, 16, nz, nz, attn_bwd_q_view(qk, nz, Lt, C), C, taps, Lt, ok.ptr, &ok);
+        launch_k(wgrad_kernel, dim3(s.nx, s.ny, s.slices), dim3(WGRAD_THREADS), (size_t)WGRAD_SMEM_BYTES, st, p);
+    }
+    {   // dV = P^T dO
+        const WgradShape s = wgrad_shape(Lt, Lt / 16, 16, nz, C, 1, 0, &ov);
+        const WgradParams p = wgrad_params(s, P, Lt, Lt / 16, 16, nz, nz, nhwc_src(dO, nz, Lt / 16, 16, C), C, taps, Lt, ov.ptr, &ov);
+        launch_k(wgrad_kernel, dim3(s.nx, s.ny, s.slices), dim3(WGRAD_THREADS), (size_t)WGRAD_SMEM_BYTES, st, p);
+    }
+    launch_cast_bf16(dqkv, static_cast<bf16*>(dqkv_bf16), (long long)nz * Lt * 3 * C / 4, st);
+    CK(cudaStreamSynchronize(st));
+    API_END
+}
+
+int sr3_test_film_embed_bwd(const sr3_test_film_args* a, void* stream) {
+    API_BEGIN
+    REQUIRE(a && a->wf && a->tau && a->dfilm && a->nl && a->w1 && a->b1 && a->w2 && a->dwf && a->dbf && a->dcb && a->dtau && a->dw1 && a->db1 &&
+            a->dw2 && a->db2, "null argument");
+    REQUIRE(a->F >= 1 && a->inner >= 2 && a->inner % 2 == 0 && a->B >= 1, "bad shape");
+    // both kernels' shared-memory limits before anything is launched
+    REQUIRE(film_bwd_smem(a->B, a->inner) <= FILM_BWD_SMEM_MAX && embed_bwd_smem(a->B, a->inner) <= FILM_BWD_SMEM_MAX,
+            "FiLM / noise-level MLP backward: batch %d too large for one block's shared memory", a->B);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    CK(cudaMemsetAsync(a->dtau, 0, (size_t)a->B * a->inner * sizeof(float), st));
+    launch_film_bwd(a->wf, a->tau, a->dfilm, a->dwf, a->dbf, a->dcb, a->dtau, a->F, a->inner, a->B, a->gscale, st);
+    launch_embed_bwd(a->nl, a->w1, a->b1, a->w2, a->dtau, a->dw1, a->db1, a->dw2, a->db2, a->inner, a->B, a->gscale, st);
+    CK(cudaStreamSynchronize(st));
+    API_END
+}
+
+int sr3_test_loss_grad(const float* noise, const float* eps, int B, int C, int H, int W, int l2, double* loss_host, void* deps_bf16, int ld,
+                       float* bias_sum, void* stream) {
+    API_BEGIN
+    REQUIRE(noise && eps && loss_host && deps_bf16 && bias_sum, "null argument");
+    REQUIRE(B >= 1 && C >= 1 && C <= ld && (H * W) % 32 == 0, "bad loss shape");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    DevAllocs mem;
+    double* loss = static_cast<double*>(mem.alloc(sizeof(double)));
+    launch_loss_grad(noise, eps, B, C, H, W, l2 ? 1 : 0, loss, static_cast<bf16*>(deps_bf16), ld, bias_sum, st);
+    CK(cudaMemcpyAsync(loss_host, loss, sizeof(double), cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     API_END
 }

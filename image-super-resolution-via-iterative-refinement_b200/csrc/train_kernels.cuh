@@ -215,66 +215,32 @@ struct GnBwdParams {
     int add_ld;
     float* dst0; int acc0; __nv_bfloat16* dst0_b; float* gsum0; int gsum_ld0;    // gradient of source 0: [B][HW][C0]; acc: dst += ; gsum[b * ld + c] += column sums
     float* dst1; int acc1; __nv_bfloat16* dst1_b; float* gsum1; int gsum_ld1;    // source 1 (skip connection)
-    const float* mr;         // [B][groups][2] (mean, rstd) saved by the forward's GroupNorm apply
+    const float* mr;         // [B][groups][2] (mean, rstd) saved by the forward's GroupNorm apply (prep_kernel's save_mr)
     float* dgamma; float* dbeta; float gscale;   // pass 2, block (0, 0): dgamma[c] = gscale sum_b S2[b][c], dbeta[c] = gscale sum_b S1[b][c]
 };
 
-// mean / rstd per group into gm / gr (shared), from the fp64 channel sums.  scratch: [C] doubles.  Ends with __syncthreads().
-__device__ __forceinline__ void groupnorm_mean_rstd(const PrepParams& p, int b, double* scratch, float* gm, float* gr) {
-    const int C = p.C0 + p.C1;
-    const int gs = C / p.groups;
-    const double inv = 1.0 / (static_cast<double>(gs) * static_cast<double>(p.HW));
-    for (int c = threadIdx.x; c < C; c += blockDim.x)
-        scratch[c] = (c < p.C0) ? __ldcg(p.st0 + (static_cast<long long>(b) * p.C0 + c) * 2) : __ldcg(p.st1 + (static_cast<long long>(b) * p.C1 + (c - p.C0)) * 2);
-    __syncthreads();
-    double gmean = 0.0;
-    for (int g = threadIdx.x; g < p.groups; g += blockDim.x) {
-        double s = 0.0;
-        for (int j = 0; j < gs; ++j) s += scratch[g * gs + j];
-        gmean = s * inv;
-        gm[g] = static_cast<float>(gmean);
-    }
-    __syncthreads();
-    for (int c = threadIdx.x; c < C; c += blockDim.x)
-        scratch[c] = (c < p.C0) ? __ldcg(p.st0 + (static_cast<long long>(b) * p.C0 + c) * 2 + 1) : __ldcg(p.st1 + (static_cast<long long>(b) * p.C1 + (c - p.C0)) * 2 + 1);
-    __syncthreads();
-    for (int g = threadIdx.x; g < p.groups; g += blockDim.x) {
-        double q = 0.0;
-        for (int j = 0; j < gs; ++j) q += scratch[g * gs + j];
-        double var = q * inv - gmean * gmean;
-        if (var < 0.0) var = 0.0;
-        gr[g] = static_cast<float>(1.0 / sqrt(var + static_cast<double>(p.eps)));
-    }
-    __syncthreads();
-}
-
-// shared memory: [C] doubles scratch | gm[groups] | gr[groups] | m1[groups] | m2[groups] | red[2*C] floats
-__host__ __device__ constexpr int gn_bwd_smem_bytes(int C, int groups) { return C * 8 + 4 * groups * 4 + 2 * C * 4; }
+// shared memory: gm[groups] | gr[groups] | m1[groups] | m2[groups] | red[2*C] floats
+__host__ __device__ constexpr int gn_bwd_smem_bytes(int C, int groups) { return 4 * groups * 4 + 2 * C * 4; }
 
 template <bool APPLY>
 __global__ void __launch_bounds__(512) gn_bwd_kernel(const GnBwdParams p) {
     pdl_launch_dependents();
     pdl_wait();
-    extern __shared__ double smd[];
+    extern __shared__ float smf[];
     const PrepParams& f = p.f;
     const int C = f.C0 + f.C1;
     const int gs = C / f.groups;
-    double* scratch = smd;
-    float* gm = reinterpret_cast<float*>(smd + C);
+    float* gm = smf;
     float* gr = gm + f.groups;
     float* m1 = gr + f.groups;
     float* m2 = m1 + f.groups;
     float* red = m2 + f.groups;                    // [2C]
     const int b = blockIdx.y;
-    if (p.mr != nullptr) {
-        for (int g = threadIdx.x; g < f.groups; g += blockDim.x) {
-            gm[g] = __ldcg(&p.mr[(static_cast<long long>(b) * f.groups + g) * 2]);
-            gr[g] = __ldcg(&p.mr[(static_cast<long long>(b) * f.groups + g) * 2 + 1]);
-        }
-        __syncthreads();
-    } else {
-        groupnorm_mean_rstd(f, b, scratch, gm, gr);
+    for (int g = threadIdx.x; g < f.groups; g += blockDim.x) {
+        gm[g] = __ldcg(&p.mr[(static_cast<long long>(b) * f.groups + g) * 2]);
+        gr[g] = __ldcg(&p.mr[(static_cast<long long>(b) * f.groups + g) * 2 + 1]);
     }
+    __syncthreads();
     if (APPLY) {
         if (blockIdx.x == 0 && blockIdx.y == 0 && (p.dgamma != nullptr || p.dbeta != nullptr)) {
             for (int c = threadIdx.x; c < C; c += blockDim.x) {
@@ -538,57 +504,7 @@ __global__ void __launch_bounds__(256) embed_bwd_kernel(const float* __restrict_
 }
 
 // ------------------------------------------------------------------------------------------------ attention backward (unet.py:129-139)
-// 0.7 % of the FLOPs: plain fp32 CUDA-core batched GEMM  C[z][m][n] = alpha * sum_k A[z](m,k) B[z](n,k)  with arbitrary element strides
-// (covers the four products dP = dO V^T, dQ = dS K, dK = dS^T Q, dV = P^T dO without materialising a transpose).
-template <typename T> __device__ __forceinline__ float ld_as_float(const T* p);
-template <> __device__ __forceinline__ float ld_as_float<float>(const float* p) { return *p; }
-template <> __device__ __forceinline__ float ld_as_float<__nv_bfloat16>(const __nv_bfloat16* p) { return __bfloat162float(*p); }
-struct BgemmParams {
-    const void* A; const void* B; float* C;
-    long long a_m, a_k, a_z, b_n, b_k, b_z, c_m, c_z;    // element strides (C is [m][n] with n contiguous)
-    int M, N, K;
-    float alpha;
-};
-template <typename TA, typename TB>
-__global__ void __launch_bounds__(256) bgemm_kernel(const BgemmParams p) {
-    pdl_launch_dependents();
-    pdl_wait();
-    __shared__ float As[16][64 + 1], Bs[16][64 + 1];
-    const int z = blockIdx.z, m0 = blockIdx.y * 64, n0 = blockIdx.x * 64;
-    const TA* A = static_cast<const TA*>(p.A) + z * p.a_z;
-    const TB* B = static_cast<const TB*>(p.B) + z * p.b_z;
-    const int tx = threadIdx.x % 16, ty = threadIdx.x / 16;
-    float acc[4][4] = {};
-    for (int k0 = 0; k0 < p.K; k0 += 16) {
-        for (int i = threadIdx.x; i < 64 * 16; i += 256) {
-            // pick the loop order that walks the contiguous axis with consecutive threads
-            int mm, kk;
-            if (p.a_k == 1) { kk = i % 16; mm = i / 16; } else { mm = i % 64; kk = i / 64; }
-            As[kk][mm] = (m0 + mm < p.M && k0 + kk < p.K) ? ld_as_float<TA>(A + (m0 + mm) * p.a_m + (k0 + kk) * p.a_k) : 0.f;
-            int nn, k2;
-            if (p.b_k == 1) { k2 = i % 16; nn = i / 16; } else { nn = i % 64; k2 = i / 64; }
-            Bs[k2][nn] = (n0 + nn < p.N && k0 + k2 < p.K) ? ld_as_float<TB>(B + (n0 + nn) * p.b_n + (k0 + k2) * p.b_k) : 0.f;
-        }
-        __syncthreads();
-#pragma unroll
-        for (int kk = 0; kk < 16; ++kk) {
-            float a[4], b[4];
-#pragma unroll
-            for (int i = 0; i < 4; ++i) { a[i] = As[kk][ty * 4 + i]; b[i] = Bs[kk][tx * 4 + i]; }
-#pragma unroll
-            for (int i = 0; i < 4; ++i)
-#pragma unroll
-                for (int j = 0; j < 4; ++j) acc[i][j] += a[i] * b[j];
-        }
-        __syncthreads();
-    }
-    float* C = p.C + z * p.c_z;
-    for (int i = 0; i < 4; ++i)
-        for (int j = 0; j < 4; ++j) {
-            const int m = m0 + ty * 4 + i, n = n0 + tx * 4 + j;
-            if (m < p.M && n < p.N) C[m * p.c_m + n] = p.alpha * acc[i][j];
-        }
-}
+// The four matrix products run on the tensor cores (train_plan.inc, bwd_attention); these are the small kernels between them.
 // softmax backward, in place on dP: dS = P * (dP - sum_k P dP) * scale; rows / segments as softmax_kernel
 __global__ void __launch_bounds__(256) softmax_bwd_kernel(const __nv_bfloat16* __restrict__ P, float* __restrict__ dP, __nv_bfloat16* __restrict__ dS_b, long long rows, int L, int seg,
                                                           float scale) {

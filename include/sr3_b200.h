@@ -256,6 +256,58 @@ int sr3_test_wgrad(const void* dy_bf16, const void* x_bf16, float* grad, int B, 
 int sr3_test_conv_groupnorm(const void* x_bf16, const float* w_oihw, const float* bias, const float* gamma, const float* beta, int groups,
                             int silu, float* y, void* a_bf16, int B, int H, int W, int Cin, int Cout, int ksize, void* stream);
 
+/* ---- kernel-level hooks of the training backward: each builds its launches with the training plan's own helpers (csrc/train_plan.inc).
+ * Every pointer is DEVICE memory; tensors are NHWC with HW = H * W pixels per image. */
+
+/* One GroupNorm (+SiLU, +Dropout) layer of a ResnetBlock / attention / final Block as the plan pairs its forward and backward:
+ * prep_kernel (a = drop(silu(GN(cat(x0, x1)))) as bf16, saving (mean, rstd)), then both passes of gn_bwd_kernel given dA.
+ *   x0 fp32 [B][HW][C0], x1 (optional) fp32 [B][HW][C1]; st0 / st1 fp64 [B][C][2] (channel sum, sum of squares);
+ *   drop: 0 none, 1 Philox keyed by (drop_seed; vector index, drop_layer), 2 the uint8 keep-mask drop_mask [B][C0+C1][HW] (NCHW);
+ *   dA fp32 [B][HW][C0+C1]; add (optional) fp32 [B][HW][add_ld] (its first C0 + C1 channels are added to the input gradient);
+ *   outputs: a_bf16 [B][HW][C0+C1], mr [B][groups][2], dst0 fp32 [B][HW][C0] (acc0: added to what it holds), dst0_b (optional) bf16(dst0),
+ *   gsum0 (optional, zeroed by the caller) [B][C0] += per-image channel sums of dst0, dst1 (optional) fp32 [B][HW][C1] (stored),
+ *   dgamma / dbeta [C0+C1] = gscale * the parameter gradients. */
+typedef struct sr3_test_groupnorm_args {
+    const float* x0; const float* x1; const double* st0; const double* st1; const float* gamma; const float* beta;
+    const unsigned char* drop_mask; const float* dA; const float* add;
+    void* a_bf16; float* mr; float* dst0; void* dst0_b; float* gsum0; float* dst1; float* dgamma; float* dbeta;
+    uint64_t drop_seed;
+    int B, HW, C0, C1, groups, silu, drop, add_ld, acc0;
+    unsigned int drop_layer;
+    float drop_p, gscale;
+} sr3_test_groupnorm_args;
+int sr3_test_groupnorm_layer(const sr3_test_groupnorm_args* args, void* stream);
+/* grad_combine_kernel: out = a (+ b) fp32 [B][HW][C]; dst (optional) = out, or += out when acc; dst_b (optional) = bf16 of it; gsum (optional,
+ * zeroed by the caller) [B][C] += its per-image channel sums.  Then, when bias0 is given, bias_grad_kernel: bias0 (and bias1) [C] =
+ * gscale * sum over images of gsum. */
+int sr3_test_grad_combine(const float* a, const float* b, float* dst, int acc, void* dst_b, float* gsum, float* bias0, float* bias1, float gscale,
+                          int B, int HW, int C, void* stream);
+/* Data gradient of a conv on the tile kernel, its weight packed on the device from w (fp32 OIHW) as the plan packs it.  dx fp32
+ * [B][H][W][Cin] (H, W: the conv's input size).  form 0: stride-1 k x k conv Cin -> Cout, dy bf16 [B][H][W][CY] (CY = Cout rounded up to a multiple
+ * of 64: the final conv's 3 channels sit in a 64-channel buffer); form 1: Downsample (3x3 stride 2, C -> C), dy bf16 [B][H/2][W/2][C];
+ * form 2: Upsample (nearest 2x then 3x3, C -> C), dy bf16 [B][2H][2W][C]. */
+int sr3_test_dgrad(const void* dy_bf16, const float* w_oihw, float* dx, int form, int B, int H, int W, int CY, int Cin, int Cout, int ksize,
+                   void* stream);
+/* Attention backward from the transposes to the bf16 copy of d(qkv), nz batches of Lt tokens (HW per image), head dim C:
+ * qk bf16 [nz*Lt][2C] (q | k), vT bf16 [nz*C][Lt], P bf16 [nz*Lt][Lt] (the forward's softmax), dO bf16 [nz*Lt][C] ->
+ * dS fp32 [nz*Lt][Lt], dS_b bf16 [nz*Lt][Lt], dqkv fp32 [nz*Lt][3C] (dQ | dK | dV), dqkv_b bf16 of it. */
+int sr3_test_attention_bwd(const void* qk_bf16, const void* vT_bf16, const void* P_bf16, const void* dO_bf16, float* dS, void* dS_bf16, float* dqkv,
+                           void* dqkv_bf16, int nz, int Lt, int HW, int C, void* stream);
+/* FiLM projections + noise-level MLP backward (film_bwd_kernel into a zeroed dtau, then embed_bwd_kernel): film = W_f tau(nl) + b_f + cb,
+ * tau(nl) = W2 swish(W1 PE(nl) + b1) + b2, inner = tau's width, hidden 4 inner.  wf [F][inner], tau [B][inner], dfilm [B][F], nl [B],
+ * w1 [4 inner][inner], b1 [4 inner], w2 [inner][4 inner] -> dwf, dbf, dcb, dtau [B][inner], dw1, db1, dw2, db2 (all but dtau times gscale). */
+typedef struct sr3_test_film_args {
+    const float* wf; const float* tau; const float* dfilm; const float* nl; const float* w1; const float* b1; const float* w2;
+    float* dwf; float* dbf; float* dcb; float* dtau; float* dw1; float* db1; float* dw2; float* db2;
+    int F, inner, B;
+    float gscale;
+} sr3_test_film_args;
+int sr3_test_film_embed_bwd(const sr3_test_film_args* args, void* stream);
+/* loss_grad_kernel: noise, eps fp32 NCHW [B][C][H][W] (H * W a multiple of 32) -> *loss_host = sum |eps - noise| (l2 = 0) or
+ * sum (eps - noise)^2 (l2 = 1); deps bf16 [B][H][W][ld] channels 0..C-1 = sign(d) or 2 d (the rest untouched); bias_sum [C] += its sums. */
+int sr3_test_loss_grad(const float* noise, const float* eps, int B, int C, int H, int W, int l2, double* loss_host, void* deps_bf16, int ld,
+                       float* bias_sum, void* stream);
+
 /* Timing harness for one conv shape on zero-filled buffers (kernel-tuning experiments): average ms over `reps` launches. */
 int sr3_bench_conv(int B, int H, int W, int Cin, int Cout, int ksize, int stride, int with_resid, int with_stats, int reps, float* ms_out);
 

@@ -9,7 +9,9 @@ import numpy as np
 import pytest
 import torch
 
+import _philox
 import _train_util as tu
+from _lowres_inputs import TINY4
 from oracle import sr3_oracle as orc
 
 pytestmark = pytest.mark.gpu
@@ -126,7 +128,69 @@ def test_dropout_masks_of_the_reference(train_golden):
     assert abs(ev - lo) / lo > 1e-4
 
 
-def test_philox_dropout_is_deterministic_and_has_the_right_rate():
+def dropout_shapes(unet, R, B):
+    """{"downs.1.res_block.block2": (B, C, H, W), ...}: the activation each ResnetBlock's nn.Dropout masks (unet.py:86,100-101)."""
+    downs, mid, ups = orc.unet_topology(tu.oracle_cfg(unet, R))
+    return {s.name + ".res_block.block2": (B, s.cout, s.res, s.res) for s in downs + mid + ups if s.kind == "res"}
+
+
+def check_dropout_gradients(net, unet, R, hr, sr, gamma, noise, masks, dropout_seed=0):
+    lo, go = tu.ours_loss_and_grads(net, hr, sr, gamma, noise, train_mode=True, dropout_seed=dropout_seed)
+    lr_, gr = tu.oracle_loss_and_grads(net, unet, R, hr, sr, gamma, noise, "l2", dropout_masks=masks)
+    assert abs(lo - lr_) / abs(lr_) < 1e-2, (lo, lr_)
+    assert set(go) == set(gr)
+    for n, e, c, _ in tu.compare(go, gr):
+        assert e < GRAD_TOL, (n, e, c)
+    return lo
+
+
+@pytest.mark.parametrize("name,unet,R,B", [("tiny", TINY, 32, 2), ("tiny_4x4", TINY4, 16, 3)])
+def test_dropout_gradients_match_oracle_on_injected_masks(name, unet, R, B):
+    """Random keep-masks (p = 0.2) injected into every block2 Dropout: every gradient tensor against the oracle's fp32 autograd with the
+    same masks.  A backward that evaluated a different mask from the forward's fails here (the gradient norms alone would barely move)."""
+    p = 0.2
+    unet = dict(unet, dropout=p)
+    net = tu.build_train_net(unet, R, 5, "l2")
+    hr, sr, noise = tu.batch(B, R, 1000)
+    gamma = tu.draw_gamma(B, 7)
+    net.train(True)
+    eng = net.denoise_fn.engine(B, conditional=True, channels=3, train_dropout=p)
+    shapes = dropout_shapes(unet, R, B)
+    assert sorted(eng.dropout_layers()) == sorted(shapes)
+    g = torch.Generator().manual_seed(21)
+    masks = {}
+    for k, shape in shapes.items():
+        keep = (torch.rand(shape, generator=g) >= p).to(torch.uint8)
+        eng.set_dropout_mask(k, keep.cuda().contiguous())
+        masks[k] = _philox.scale_mask(keep, p)
+    try:
+        check_dropout_gradients(net, unet, R, hr, sr, gamma, noise, masks)
+    finally:
+        for k in shapes:
+            eng.set_dropout_mask(k, None)
+
+
+def test_dropout_gradients_match_oracle_on_philox_masks():
+    """The device's own Philox masks (dropout_seed), reproduced bit for bit by the numpy restatement of drop_scale4 (tests/_philox.py): the
+    layer index of a Dropout is its position in eng.dropout_layers() (the order the plan numbers them in, DropSpec.layer).  Every gradient
+    tensor against the oracle's fp32 autograd on those masks."""
+    p, B, R, seed = 0.2, 2, 32, 0x5EED0000C0FFEE
+    unet = dict(TINY, dropout=p)
+    net = tu.build_train_net(unet, R, 5, "l2")
+    hr, sr, noise = tu.batch(B, R, 1000)
+    gamma = tu.draw_gamma(B, 7)
+    net.train(True)
+    eng = net.denoise_fn.engine(B, conditional=True, channels=3, train_dropout=p)
+    shapes = dropout_shapes(unet, R, B)
+    masks = {}
+    for layer, k in enumerate(eng.dropout_layers()):
+        b, c, h, w = shapes[k]
+        keep = _philox.keep_mask(b, c, h * w, p, seed, layer).reshape(b, c, h, w)
+        masks[k] = _philox.scale_mask(keep, p)
+    check_dropout_gradients(net, unet, R, hr, sr, gamma, noise, masks, dropout_seed=seed)
+
+
+def test_philox_dropout_is_deterministic():
     unet = dict(TINY, dropout=0.2)
     net = tu.build_train_net(unet, 32, 5, "l2")
     hr, sr, noise = tu.batch(2, 32, 1000)
