@@ -72,7 +72,7 @@ __device__ __forceinline__ void attn_unit_t(const AttnParams& p, const AttnParam
         int s = 0;
         uint32_t ph = 0;
         for (int it = 0; it < kc1 + kc3; ++it) {
-            mbar_wait(empty_bar(s), ph ^ 1u, 11);
+            mbar_wait(empty_bar(s), ph ^ 1u);
             if (elect_one_sync()) {
                 const uint32_t dst = base + s * ATTN_STAGE_BYTES;
                 if (it < kc1) {
@@ -92,7 +92,7 @@ __device__ __forceinline__ void attn_unit_t(const AttnParams& p, const AttnParam
         if constexpr (MEGA) {        // tail: no arrival may be in flight when the barriers are recycled
             const int total = kc1 + kc3, n_wait = total < ATTN_STAGES ? total : ATTN_STAGES;
             for (int i = 0; i < n_wait; ++i) {
-                mbar_wait(empty_bar(s), ph ^ 1u, 16);
+                mbar_wait(empty_bar(s), ph ^ 1u);
                 if (++s == ATTN_STAGES) { s = 0; ph ^= 1u; }
             }
         }
@@ -106,14 +106,14 @@ __device__ __forceinline__ void attn_unit_t(const AttnParams& p, const AttnParam
         auto release_prev = [&]() {                        // the stage before the one just committed has been read
             if (prev >= 0) {
                 wgmma_wait<1>();
-                if (leader) mbar_arrive(empty_bar(prev));
+                mbar_arrive_if(empty_bar(prev), leader);
             }
             prev = s;
             if (++s == ATTN_STAGES) { s = 0; ph ^= 1u; }
         };
         float sacc[LT / 2];
         for (int it = 0; it < kc1; ++it) {
-            mbar_wait(full_bar(s), ph, 13);
+            mbar_wait(full_bar(s), ph);
             wgmma_fence();
             const uint32_t st = base + s * ATTN_STAGE_BYTES;
 #pragma unroll
@@ -165,7 +165,7 @@ __device__ __forceinline__ void attn_unit_t(const AttnParams& p, const AttnParam
 
         float oacc[DN / 2];
         for (int kc = 0; kc < kc3; ++kc) {
-            mbar_wait(full_bar(s), ph, 13);
+            mbar_wait(full_bar(s), ph);
             wgmma_fence();
             const uint32_t st = base + s * ATTN_STAGE_BYTES;
             const uint32_t pa = p_base + kc * 16384 + g * 8192;
@@ -178,7 +178,7 @@ __device__ __forceinline__ void attn_unit_t(const AttnParams& p, const AttnParam
         }
         wgmma_wait<0>();
         wgmma_fence_regs(oacc);
-        if (prev >= 0 && leader) mbar_arrive(empty_bar(prev));
+        if (prev >= 0) mbar_arrive_if(empty_bar(prev), leader);
         const float inv[2] = {1.0f / sum[0], 1.0f / sum[1]};
 #pragma unroll
         for (int j = 0; j < DN / 2; j += 2) {

@@ -465,7 +465,7 @@ __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmPa
             const int sp = tile % ksplit;
             const int k0 = (num_kt * sp) / ksplit, k1 = (num_kt * (sp + 1)) / ksplit;
             for (int k = k0; k < k1; ++k) {
-                mbar_wait(empty_bar(s), ph ^ 1u, 1);
+                mbar_wait(empty_bar(s), ph ^ 1u);
                 if (elect_one_sync()) {
                     const int pass = k / p.num_k;
                     const StageDesc& e = ktab_s[k - pass * p.num_k];
@@ -493,7 +493,7 @@ __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmPa
             }
             const int n_wait = filled < stages ? filled : stages;
             for (int i = 0; i < n_wait; ++i) {
-                mbar_wait(empty_bar(s), ph ^ 1u, 6);
+                mbar_wait(empty_bar(s), ph ^ 1u);
                 if (++s == stages) { s = 0; ph ^= 1u; }
             }
         }
@@ -517,7 +517,6 @@ __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmPa
         uint32_t res_count = 0;        // residual chunks consumed so far
         uint32_t bias_slot = 0;        // alternating bias staging slot
         bool out_pending = false;      // a bulk store from the staging buffer may still be reading it
-        float acc[AH][2][WN / 2];
         int s = 0;                     // stage ring position
         uint32_t ph = 0;
         // GroupNorm partial sums of this lane's column in the warp's OWN chunks, kept across the tiles of one (image, column block).
@@ -525,6 +524,7 @@ __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmPa
         // a tile may be two images, so a run covers the NCH chunks of one half.)
         StatRun<NSTAT> st_own;
         for (int tile = tile_begin + (PP ? g : 0); tile < tile_end; tile += (PP ? 2 : 1)) {
+            float acc[AH][2][WN / 2];
             int w0, h0, b0, n0, z;
             decode(tile, w0, h0, b0, n0, z);
             if constexpr (PP) {        // every tile of the range streams num_kt stages: this tile's first stage is number li * num_kt
@@ -591,32 +591,42 @@ __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmPa
                 if (PP && li > 0) asm volatile("bar.sync %0, 256;" ::"r"(GEMM_ORDER_BAR + g) : "memory");   // our turn to issue MMAs
                 int prev = -1;
                 for (int k = k0; k < k1; ++k) {
-                    mbar_wait(full_bar(s), ph, 2);
+                    mbar_wait(full_bar(s), ph);
                     const StageDesc& e = ktab_s[k % p.num_k];
-                    wgmma_fence();
-                    for (int t = 0; t < e.ntaps; ++t) {
-                        const uint32_t a_addr = a_base + s * stage_bytes + e.tap[t].a_off + (e.a_multi ? 0 : zrow_off);
-                        const uint32_t b_addr = b_base + s * stage_bytes + t * B_BYTES;
+                    // The MMAs of a stage are one branch-free chain with a compile-time tap count: a branch between two wgmma (a loop
+                    // over a count read from shared memory) makes ptxas re-fence before every tap or serialise them.  The count is
+                    // broadcast from lane 0 so that ptxas knows the switch below is warp-uniform.
+                    const int ntaps = __shfl_sync(0xffffffffu, e.ntaps, 0);
+                    auto issue = [&](auto nt_c) {
+                        wgmma_fence();
 #pragma unroll
-                        for (int kk = 0; kk < 4; ++kk) {   // 4 x K(16) = 64 channels; +32 B inside the 128 B swizzle row
-                            const uint64_t bdesc = wgmma_desc_sw128(b_addr + kk * 32, 16, 1024);
+                        for (int t = 0; t < decltype(nt_c)::value; ++t) {
+                            const uint32_t a_addr = a_base + s * stage_bytes + e.tap[t].a_off + (e.a_multi ? 0 : zrow_off);
+                            const uint32_t b_addr = b_base + s * stage_bytes + t * B_BYTES;
 #pragma unroll
-                            for (int hh = 0; hh < AH; ++hh)    // (ping-pong, MH = 2: both 128-row halves share the B slab)
+                            for (int kk = 0; kk < 4; ++kk) {   // 4 x K(16) = 64 channels; +32 B inside the 128 B swizzle row
+                                const uint64_t bdesc = wgmma_desc_sw128(b_addr + kk * 32, 16, 1024);
 #pragma unroll
-                                for (int i = 0; i < 2; ++i)    // row groups 2 g' + i, g' = 0..7
-                                    Wgmma<WN>::template mma<0, 0>(acc[hh][i],
-                                                                  wgmma_desc_sw128(a_addr + hh * p.a_half_off + i * 1024 + kk * 32, 16, 2048),
-                                                                  bdesc, ((k - k0) | t | kk) != 0);
+                                for (int hh = 0; hh < AH; ++hh)    // (ping-pong, MH = 2: both 128-row halves share the B slab)
+#pragma unroll
+                                    for (int i = 0; i < 2; ++i)    // row groups 2 g' + i, g' = 0..7
+                                        Wgmma<WN>::template mma<0, 0>(acc[hh][i],
+                                                                      wgmma_desc_sw128(a_addr + hh * p.a_half_off + i * 1024 + kk * 32, 16, 2048),
+                                                                      bdesc, ((k - k0) | t | kk) != 0);
+                            }
                         }
-                    }
-                    wgmma_commit();
+                        wgmma_commit();
+                    };
+                    if (ntaps == 3) issue(std::integral_constant<int, 3>{});
+                    else if (ntaps == 2) issue(std::integral_constant<int, 2>{});
+                    else issue(std::integral_constant<int, 1>{});
                     if (stages == 1) {                                      // nothing can be loaded ahead: free the only stage now
                         wgmma_wait<0>();
-                        if ((threadIdx.x & 127) == 0) mbar_arrive(empty_bar(s));
+                        mbar_arrive_if(empty_bar(s), (threadIdx.x & 127) == 0);
                     } else {
                         if (prev >= 0) {                                    // the stage before this one has been read
                             wgmma_wait<1>();
-                            if ((threadIdx.x & 127) == 0) mbar_arrive(empty_bar(prev));
+                            mbar_arrive_if(empty_bar(prev), (threadIdx.x & 127) == 0);
                         }
                         prev = s;
                     }
@@ -630,7 +640,7 @@ __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmPa
                     wgmma_fence_regs(acc[hh][0]);
                     wgmma_fence_regs(acc[hh][1]);
                 }
-                if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(empty_bar(prev));
+                if (prev >= 0) mbar_arrive_if(empty_bar(prev), (threadIdx.x & 127) == 0);
             }
             // pass 0 reads the accumulator.  With split-K it only stores this CTA's partial tile into its slice of `ws`;
             // once all `ksplit` CTAs of the output tile have arrived at the tile's counter, pass 1 runs in EVERY one of them on a
@@ -655,10 +665,7 @@ __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmPa
                         if ((spins & 1023u) == 1023u) {
                             const uint64_t now = globaltimer_ns();
                             if (t0 == 0) t0 = now;
-                            if (now - t0 > 4000000000ull) {
-                                printf("sr3: split-K wait timeout cta=%d tile=%d counter=%u target=%u\n", cta, tile, v, target);
-                                __trap();
-                            }
+                            if (now - t0 > 4000000000ull) __trap();   // no printf: a call in the kernel serialises its wgmma (see mbar_wait)
                         }
                     }
                     __threadfence();
@@ -712,7 +719,7 @@ __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmPa
                     }
                     if (use_res_tma) {
                         const uint32_t b = (res_count - 1) & 1;
-                        mbar_wait(res_bar(ew, b), (res_phase >> b) & 1u, 5);
+                        mbar_wait(res_bar(ew, b), (res_phase >> b) & 1u);
                         res_phase ^= (1u << b);
                         const uint8_t* rp = res_ptr + b * 4096 + lane * 128;
 #pragma unroll

@@ -57,6 +57,16 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t byt
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
+// Arrive only where `pred` holds, as one predicated instruction: no branch, so it may sit between wgmma issue and wgmma wait
+// without ptxas serialising the MMAs.
+__device__ __forceinline__ void mbar_arrive_if(uint32_t bar, bool pred) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %1, 0;\n\t"
+        "@p mbarrier.arrive.shared::cta.b64 _, [%0];\n\t}" ::"r"(bar),
+        "r"(static_cast<uint32_t>(pred))
+        : "memory");
+}
 __device__ __forceinline__ void mbar_inval(uint32_t bar) {
     asm volatile("mbarrier.inval.shared::cta.b64 [%0];" ::"r"(bar) : "memory");
 }
@@ -79,31 +89,25 @@ __device__ __forceinline__ void red_release_gpu_add_u64(unsigned long long* p, u
     asm volatile("red.release.gpu.global.add.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
 }
 
-__device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
-    uint32_t ok;
+// Bounded wait: a pipeline bug must trap (-> a CUDA error the host reports) instead of hanging the GPU.  The MMA warpgroups wait here
+// while earlier wgmma groups are in flight, so the loop, the 4 s timeout and the trap are one asm block: a call (printf) anywhere in a
+// kernel, or a divergent branch the compiler can see between two wgmma, makes ptxas serialise every wgmma of the kernel.  The trap
+// carries no message; with -lineinfo a GPU core dump (CUDA_ENABLE_COREDUMP_ON_EXCEPTION=1) points at the wait that expired.
+__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(bar), "r"(parity)
+        "{\n\t.reg .pred p;\n\t.reg .u64 t0, t1;\n\t"
+        "mov.u64 t0, %%globaltimer;\n\t"
+        "WAIT:\n\t"
+        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
+        "@p bra DONE;\n\t"
+        "mov.u64 t1, %%globaltimer;\n\t"
+        "sub.u64 t1, t1, t0;\n\t"
+        "setp.lt.u64 p, t1, 4000000000;\n\t"
+        "@p bra WAIT;\n\t"
+        "trap;\n\t"
+        "DONE:\n\t}" ::"r"(bar),
+        "r"(parity)
         : "memory");
-    return ok != 0;
-}
-// Bounded wait: a pipeline bug must trap (-> a CUDA error the host reports) instead of hanging the GPU.
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity, int tag) {
-    uint64_t t0 = 0;
-    uint32_t spins = 0;
-    while (!mbar_try_wait(bar, parity)) {
-        if ((++spins & 0xfff) == 0) {
-            const uint64_t now = globaltimer_ns();
-            if (t0 == 0) t0 = now;
-            if (now - t0 <= 4000000000ull) continue;
-            printf("sr3: mbarrier wait timeout tag=%d block=(%d,%d,%d) thread=%d parity=%u\n", tag, blockIdx.x, blockIdx.y,
-                   blockIdx.z, threadIdx.x, parity);
-            __trap();
-        }
-    }
 }
 
 // ------------------------------------------------------------------ TMA

@@ -76,7 +76,7 @@ __global__ void __launch_bounds__(WGRAD_THREADS, 1) wgrad_kernel(const __grid_co
             const int b = it / (tiles_w * tiles_h);
             const int r = it % (tiles_w * tiles_h);
             const int w0 = (r % tiles_w) * 8, h0 = (r / tiles_w) * 8;
-            mbar_wait(empty_bar(s), ph ^ 1u, 21);
+            mbar_wait(empty_bar(s), ph ^ 1u);
             if (elect_one_sync()) {
                 const uint32_t dst = base + s * WGRAD_STAGE_BYTES;
                 mbar_arrive_expect_tx(full_bar(s), 16384 + nt * 8192);
@@ -102,20 +102,26 @@ __global__ void __launch_bounds__(WGRAD_THREADS, 1) wgrad_kernel(const __grid_co
         int s = 0, prev = -1;
         uint32_t ph = 0;
         for (int it = 0; it < iters; ++it) {
-            mbar_wait(full_bar(s), ph, 22);
-            wgmma_fence();
+            mbar_wait(full_bar(s), ph);
             const uint32_t st = base + s * WGRAD_STAGE_BYTES;
+            // one branch-free wgmma chain per tap count (a branch between two wgmma makes ptxas re-fence or serialise them)
+            auto issue = [&](auto nt_c) {
+                wgmma_fence();
 #pragma unroll
-            for (int kk = 0; kk < 4; ++kk) {                       // 16 pixels = two 8-pixel atoms per wgmma
-                const uint64_t adesc = wgmma_desc_sw128(st + g * 8192 + kk * 2048, 1024, 1024);
+                for (int kk = 0; kk < 4; ++kk) {                   // 16 pixels = two 8-pixel atoms per wgmma
+                    const uint64_t adesc = wgmma_desc_sw128(st + g * 8192 + kk * 2048, 1024, 1024);
 #pragma unroll
-                for (int t = 0; t < 3; ++t)
-                    if (t < nt) Wgmma<64>::template mma<1, 1>(acc[t], adesc, wgmma_desc_sw128(st + 16384 + t * 8192 + kk * 2048, 1024, 1024), (it | kk) != 0);
-            }
-            wgmma_commit();
+                    for (int t = 0; t < decltype(nt_c)::value; ++t)
+                        Wgmma<64>::template mma<1, 1>(acc[t], adesc, wgmma_desc_sw128(st + 16384 + t * 8192 + kk * 2048, 1024, 1024), (it | kk) != 0);
+                }
+                wgmma_commit();
+            };
+            if (nt == 3) issue(std::integral_constant<int, 3>{});
+            else if (nt == 2) issue(std::integral_constant<int, 2>{});
+            else issue(std::integral_constant<int, 1>{});
             if (prev >= 0) {
                 wgmma_wait<1>();
-                if (leader) mbar_arrive(empty_bar(prev));
+                mbar_arrive_if(empty_bar(prev), leader);
             }
             prev = s;
             if (++s == WGRAD_STAGES) { s = 0; ph ^= 1u; }
