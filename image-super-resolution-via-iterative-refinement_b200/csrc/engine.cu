@@ -527,7 +527,7 @@ int pingpong_knob() {
 // Geometry of an image conv: the "tall halo" form for 3x3 stride-1 convs at >= 16x16, else a plain 128-pixel patch per tap.
 // The tile shape (rows x BLOCK_N) and the split-K factor are chosen by a byte model of the per-CTA critical path: a CTA ingests
 // stages x (A box + B boxes) through TMA at a fixed rate, runs ceil(tiles * split / SMs) waves, and a split tile costs an extra
-// partial-tile store + reload + a grid-level handshake (tools/gpu_splitk_sweep.py sweeps the choices on a device).
+// partial-tile store + reload + a grid-level handshake (`tools/gpu_layer_profile.py --sweep` times every candidate per layer).
 // Bt: images the tiles must cover (tiles_b = ceil(Bt / b_box); images past the A tensor's batch load as zeros).
 void conv_geometry(GemmDesc& d, int OW, int OH, int Bt, int cout, bool has_resid = false, int nz = 1) {
     const int npass = d.passes > 1 ? d.passes : 1;
@@ -537,36 +537,29 @@ void conv_geometry(GemmDesc& d, int OW, int OH, int Bt, int cout, bool has_resid
     const int sms = num_sms();
     // Schedule.  SR3_PINGPONG (tests / A-B timing): 1 = ping-pong wherever the tile shape has that form (the model ranks the ping-pong
     // shapes), 0 = cooperative everywhere; a tile forced by SR3_TALL_BN / SR3_TALL_MH / SR3_BLOCK_N keeps the forced shape and, unless
-    // SR3_PINGPONG=1, the cooperative form.  Unset: the best cooperative tile, charged its exposed epilogue (coop_epi), against the 128x64
-    // ping-pong tile.  That is the only ping-pong shape the model offers: its whole-tile accumulator is 64 registers, while the 256x64 and
-    // 128x128 forms hold 128 registers through the epilogue under the 168-register cap of 288 threads, spill ~15x more and measured slower
-    // than cooperative at every shape of the 16->128 step (DESIGN.md section 8).
+    // SR3_PINGPONG=1, the cooperative form.  Unset: every cooperative tile and every ping-pong tile compete, each charged its epilogue.
     const int pp_knob = pingpong_knob();
     const bool pp_force = pp_knob == 1, pp_auto = pp_knob < 0;
     const bool shape_forced = getenv("SR3_TALL_BN") || getenv("SR3_TALL_MH") || getenv("SR3_BLOCK_N");
-    // Epilogue of one 32x32 output item of a warp (transposition, bias / FiLM, residual, TMA store, bf16 copy, GroupNorm sums) in bytes of
-    // TMA ingest at the ~47 B/clk/SM of the model (~3200 clocks) with two epilogue warps per SM sub-partition (cooperative); a ping-pong
-    // warpgroup's four warps have a sub-partition each and take half that per item.  Calibrated with tools/gpu_layer_profile.py on the
-    // 16->128 step at B = 16 (H100, DESIGN.md section 8): the 128x64 ping-pong tile, with twice the weight ingest per row of a 256-row tile,
-    // was faster on the 3x3 convs at 128x128 (15.5 tiles per CTA against cooperative 256x64 at 7.8) and 64x64 (7.8 tiles against 256x128
-    // at 1.9 and 256x64 at 3.9) and slower on the 32x32 convs with a residual (3.9 tiles against 256x64 at 1.9): the model orders those
-    // cases the same way for 137 K < EPI_ITEM_BYTES < 168 K.  So the epilogue, not TMA ingest, bounds these tiles.
-    constexpr double EPI_ITEM_BYTES = 150000.0;
+    // Epilogue of one 32x32 output item (transposition, bias / FiLM, residual, TMA store, bf16 copy, GroupNorm sums) in bytes of TMA
+    // ingest, one constant per variant family.  Fitted with `tools/gpu_layer_profile.py --sweep` (every tile op of the 16->128 B=16,
+    // 64->512 B=4 and unconditional 128 B=32 steps under every candidate, H100, DESIGN.md section 8) by minimising the summed time of the
+    // tiles the model picks, with the plain 3x3 convs of the 16->128 step at B = 16 held to their measured-and-tested schedules (128x64
+    // ping-pong at 128x128 and 64x64, cooperative at 32x32).  The 256x128 cooperative tile and the 128-register ping-pong forms (256x64,
+    // 128x128) spill through their epilogue (section 8, ptxas table), the 128x64 ping-pong form barely does, so they cannot share one
+    // constant; the tall and generic 128x64 ping-pong tiles fitted apart.
+    constexpr double EPI_COOP = 200000.0, EPI_COOP_256x128 = 2000000.0, EPI_PP_128REG = 600000.0;
+    const double EPI_PP_64REG = tall_ok ? 200000.0 : 10000.0;
     // cost in bytes of the slowest CTA; `split` returns the factor the cost was computed for.  pp: the ping-pong schedule (never split):
     // a warpgroup's epilogue (all MH x NCH items of the tile on its 4 warps) runs under the other warpgroup's MMAs, so only the last one is
-    // exposed, unless the epilogue is longer than the MMA phase it hides behind.  The cooperative cost leaves its epilogue out (so the shape
-    // choice among cooperative tiles is what it was before the ping-pong form existed); coop_epi adds it where the two schedules compete.
+    // exposed, unless the epilogue is longer than the MMA phase it hides behind.  The cooperative cost includes its epilogue, shared by the
+    // consumer warps and never overlapped with MMAs.
     auto items_of = [](int rows, int bn) { return (double)(rows / 128) * (bn >= 32 ? bn / 32 : 1); };   // 32x32 items per warp quadrant
-    auto coop_epi = [&](long long tiles, int rows, int bn, int split) {   // the 8 consumer warps (4: single-warpgroup tile) share the items
-        const double warps = gemm_single_wg(bn, rows / 128) ? 4.0 : 8.0;
-        const long long waves = (tiles * split + sms - 1) / sms;
-        return (double)waves * items_of(rows, bn) * 4.0 / (warps * split) * EPI_ITEM_BYTES;
-    };
     auto model = [&](long long tiles, int nstage, long long stage_bytes, int rows, int bn, int& split, bool pp = false) -> double {
         if (pp) {
             split = 1;
             const long long t = (tiles + sms - 1) / sms;               // tiles of the busiest CTA
-            const double mma = (double)nstage * stage_bytes, epi = items_of(rows, bn) * EPI_ITEM_BYTES * 0.5;
+            const double mma = (double)nstage * stage_bytes, epi = items_of(rows, bn) * (rows == 128 && bn == 64 ? EPI_PP_64REG : EPI_PP_128REG);
             const double serial = (double)t * mma + epi, paired = (double)((t + 1) / 2) * (mma + epi);
             return serial > paired ? serial : paired;
         }
@@ -583,9 +576,12 @@ void conv_geometry(GemmDesc& d, int OW, int OH, int Bt, int cout, bool has_resid
         split = smax;
         const long long waves = (tiles * smax + sms - 1) / sms;
         double c = (double)waves * ((nstage + smax - 1) / smax) * (double)stage_bytes;
-        // a split tile: partial tile out (registers -> L2) and back, weighted 2x against streamed TMA bytes, plus ~1.4 us of
-        // grid-level handshake; a residual is then read with plain loads instead of TMA
-        if (smax > 1) c += 4.0 * rows * bn * 4 + 131072.0 + (has_resid ? 2.0 * rows * bn * 4 : 0.0);
+        // the 8 consumer warps (4: single-warpgroup tile) share the items of the tile's 1/split share
+        const double warps = gemm_single_wg(bn, rows / 128) ? 4.0 : 8.0;
+        c += (double)waves * items_of(rows, bn) * 4.0 / (warps * smax) * (rows == 256 && bn == 128 ? EPI_COOP_256x128 : EPI_COOP);
+        // a split tile: partial tile out (registers -> L2) and back, weighted 2x against streamed TMA bytes, plus the grid-level
+        // handshake (fitted with the epilogue constants); a residual is then read with plain loads instead of TMA
+        if (smax > 1) c += 4.0 * rows * bn * 4 + 2000000.0 + (has_resid ? 2.0 * rows * bn * 4 : 0.0);
         return c;
     };
     d.ksplit_max = 1;
@@ -608,7 +604,7 @@ void conv_geometry(GemmDesc& d, int OW, int OH, int Bt, int cout, bool has_resid
         }
         int mh = 2, bn = 16, split = 1, pp = 0;       // Cout = 3 (final conv) keeps the 16-wide tile
         if (cout % 32 == 0) {
-            double best = 1e300, best_epi = 0.0, best_pp = 1e300, pp128x64 = 1e300;
+            double best = 1e300, best_pp = 1e300;
             int pp_mh = 0, pp_bn = 0;
             for (int i = 0; i < 4; ++i) {
                 const Cand& c = cands[i];
@@ -622,16 +618,12 @@ void conv_geometry(GemmDesc& d, int OW, int OH, int Bt, int cout, bool has_resid
                     int sp1 = 1;
                     const double cpp = model(tiles, nstage * npass, stage_bytes, c.mh * 128, c.bn, sp1, true);
                     if (cpp < best_pp) { best_pp = cpp; pp_mh = c.mh; pp_bn = c.bn; }
-                    if (c.mh == 1 && c.bn == 64) pp128x64 = cpp;
                 }
                 // the residual is staged through smem (8 warps x 8 KB) unless the tile is split: a 256x128 tile would be left with one stage
                 if (c.bn == 128 && has_resid && sp <= 1) continue;
-                if (cost < best) { best = cost; best_epi = coop_epi(tiles, c.mh * 128, c.bn, sp); mh = c.mh; bn = c.bn; split = sp; }
+                if (cost < best) { best = cost; mh = c.mh; bn = c.bn; split = sp; }
             }
-            if (!shape_forced) {
-                if (pp_force && pp_bn) { mh = pp_mh; bn = pp_bn; split = 1; pp = 1; }
-                else if (pp_auto && pp128x64 < best + best_epi) { mh = 1; bn = 64; split = 1; pp = 1; }
-            }
+            if (!shape_forced && pp_bn && (pp_force || (pp_auto && best_pp < best))) { mh = pp_mh; bn = pp_bn; split = 1; pp = 1; }
         }
         if (const char* e = getenv("SR3_TALL_BN")) { int v = atoi(e); if ((v == 32 || v == 64 || v == 128) && cout % v == 0) { bn = v; split = 16; } }
         if (const char* e = getenv("SR3_TALL_MH")) { int v = atoi(e); if (v == 1 || v == 2) { mh = v; split = 16; } }
@@ -668,7 +660,7 @@ void conv_geometry(GemmDesc& d, int OW, int OH, int Bt, int cout, bool has_resid
                 if (bn == 128 && sp > 1) continue;      // 96 KB stages leave a 2-deep pipeline: measured slower than 64-wide split tiles
                 if (cost < best) { best = cost; d.block_n = bn; d.ksplit_max = sp; }
             }
-            if (pp_force && pp_bn) { d.block_n = pp_bn; d.ksplit_max = 1; d.pingpong = 1; }
+            if (pp_bn && (pp_force || (pp_auto && best_pp < best))) { d.block_n = pp_bn; d.ksplit_max = 1; d.pingpong = 1; }
         } else if (pp_force && gemm_pingpong_ok(d.block_n, 1)) {
             d.pingpong = 1;
         }
