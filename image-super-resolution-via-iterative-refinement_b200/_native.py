@@ -52,6 +52,7 @@ _SIGS = {
     "sr3_last_error": (c_char_p, []),
     "sr3_abi_version": (c_int, []),
     "sr3_engine_create": (c_int, [POINTER(UNetConfigC), c_int, c_int, POINTER(c_void_p)]),
+    "sr3_engine_create_sized": (c_int, [POINTER(UNetConfigC), c_int, c_int, c_int, c_int, POINTER(c_void_p)]),
     "sr3_engine_create_train": (c_int, [POINTER(UNetConfigC), c_int, c_int, c_float, POINTER(c_void_p)]),
     "sr3_train_forward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_uint64, POINTER(c_double), c_void_p]),
     "sr3_train_backward": (c_int, [c_void_p, c_float, POINTER(c_void_p), c_int, c_void_p]),
@@ -162,12 +163,35 @@ def _f32c(t, device):
     return t.detach().to(device=device, dtype=torch.float32).contiguous()
 
 
-class Engine:
-    """One (config, batch, device) instance of the native plan: packed weights + activations + captured step graph."""
+class UnsupportedSizeError(ValueError, RuntimeError):
+    """An image size the native plan cannot run (check_image_size)."""
 
-    def __init__(self, cfg: dict, batch: int, device: torch.device, train_dropout=None):
+
+def check_image_size(n_levels, height, width):
+    """The image sizes an inference plan runs on (sr3_engine_create_sized): at every UNet level -- the image halved n_levels - 1 times --
+    both sides are powers of two and at least 8, except that the lowest level may be exactly 4x4.  Returns the lowest level (h, w);
+    raises UnsupportedSizeError naming the size and the rule otherwise."""
+    height, width = int(height), int(width)
+    lh, lw = height >> (n_levels - 1), width >> (n_levels - 1)
+    if height <= 0 or width <= 0:
+        raise UnsupportedSizeError("image size %dx%d: sides must be positive" % (height, width))
+    if lh < 4 or lw < 4:
+        raise UnsupportedSizeError("image size %dx%d: lowest UNet resolution %dx%d < 4 is not supported (%d levels)" % (height, width, lh, lw, n_levels))
+    if height & (height - 1) or width & (width - 1):
+        raise UnsupportedSizeError("image size %dx%d: both sides must be powers of two" % (height, width))
+    if not ((lh >= 8 and lw >= 8) or (lh == 4 and lw == 4)):
+        raise UnsupportedSizeError("image size %dx%d: lowest UNet level %dx%d is not supported (every level must be at least 8x8, or the lowest "
+                                   "exactly 4x4)" % (height, width, lh, lw))
+    return lh, lw
+
+
+class Engine:
+    """One (config, batch, height, width, device) instance of the native plan: packed weights + activations + captured step graph."""
+
+    def __init__(self, cfg: dict, batch: int, device: torch.device, train_dropout=None, height=None, width=None):
         """train_dropout: None = inference plan; a float = TRAINING plan (forward keeps every intermediate, backward recorded) with that
-        Dropout probability (sr3_engine_create_train)."""
+        Dropout probability (sr3_engine_create_train).  height / width: the image size the plan runs on (default image_size; training
+        plans run at image_size only)."""
         if device.type != "cuda":
             raise NativeLibraryError("sr3_b200 runs on a CUDA (sm_90a) device only; got device=%s" % device)
         self.device = device
@@ -176,6 +200,12 @@ class Engine:
         self.in_channel = cfg["in_channel"]
         self.out_channel = cfg["out_channel"]
         self.image_size = cfg["image_size"]
+        self.height = int(cfg["image_size"] if height is None else height)
+        self.width = int(cfg["image_size"] if width is None else width)
+        if train_dropout is not None and (self.height, self.width) != (self.image_size, self.image_size):
+            raise NotImplementedError("sr3_b200: training plans run at image_size x image_size (%d) only, not %dx%d"
+                                      % (self.image_size, self.height, self.width))
+        check_image_size(len(cfg["channel_mults"]), self.height, self.width)
         self.conditional = bool(cfg["conditional"])
         c = UNetConfigC()
         c.in_channel, c.out_channel, c.inner_channel = cfg["in_channel"], cfg["out_channel"], cfg["inner_channel"]
@@ -195,7 +225,7 @@ class Engine:
         idx = device.index if device.index is not None else torch.cuda.current_device()
         self.train_dropout = train_dropout
         if train_dropout is None:
-            _check(lib().sr3_engine_create(ctypes.byref(c), batch, idx, ctypes.byref(self._h)))
+            _check(lib().sr3_engine_create_sized(ctypes.byref(c), batch, self.height, self.width, idx, ctypes.byref(self._h)))
         else:
             _check(lib().sr3_engine_create_train(ctypes.byref(c), batch, idx, float(train_dropout), ctypes.byref(self._h)))
         self.T = 0
@@ -258,14 +288,23 @@ class Engine:
 
     # ---- compute
     def _img(self):
-        return torch.empty(self.batch, self.channels, self.image_size, self.image_size, device=self.device, dtype=torch.float32)
+        return torch.empty(self.batch, self.channels, self.height, self.width, device=self.device, dtype=torch.float32)
+
+    def _check_img(self, t, channels, what):
+        if t is not None and tuple(t.shape) != (self.batch, channels, self.height, self.width):
+            raise ValueError("%s has shape %s; this engine runs [%d, %d, %d, %d]" % (what, tuple(t.shape), self.batch, channels, self.height,
+                                                                                     self.width))
+
+    def _check_inputs(self, x, cond):
+        self._check_img(x, self.channels, "x")
+        self._check_img(cond, self.in_channel - self.channels, "condition_x")
 
     def unet_forward(self, x, noise_level):
         x = _f32c(x, self.device)
         nl = _f32c(noise_level, self.device).reshape(-1)
-        assert x.shape == (self.batch, self.in_channel, self.image_size, self.image_size), x.shape
+        assert x.shape == (self.batch, self.in_channel, self.height, self.width), x.shape
         assert nl.numel() == self.batch
-        eps = torch.empty(self.batch, self.out_channel, self.image_size, self.image_size, device=self.device, dtype=torch.float32)
+        eps = torch.empty(self.batch, self.out_channel, self.height, self.width, device=self.device, dtype=torch.float32)
         with torch.cuda.device(self.device):
             _check(lib().sr3_unet_forward(self._h, _ptr(x), _ptr(nl), _ptr(eps), _stream()))
         return eps
@@ -273,6 +312,7 @@ class Engine:
     def p_mean_variance(self, x, t, clip_denoised=True, condition_x=None):
         x = _f32c(x, self.device)
         c = None if condition_x is None else _f32c(condition_x, self.device)
+        self._check_inputs(x, c)
         mean = self._img()
         lv = c_float()
         with torch.cuda.device(self.device):
@@ -283,6 +323,8 @@ class Engine:
         x = _f32c(x, self.device)
         c = None if condition_x is None else _f32c(condition_x, self.device)
         n = None if noise is None else _f32c(noise, self.device)
+        self._check_inputs(x, c)
+        self._check_img(n, self.channels, "noise")
         out = self._img()
         with torch.cuda.device(self.device):
             _check(lib().sr3_p_sample(self._h, _ptr(x), _ptr(c), int(t), _ptr(n), int(seed), int(first_index), _ptr(out), _stream()))
@@ -292,6 +334,8 @@ class Engine:
         hr, noise = _f32c(hr, self.device), _f32c(noise, self.device)
         s = None if sr is None else _f32c(sr, self.device)
         g = _f32c(gamma, self.device).reshape(-1)
+        self._check_inputs(hr, s)
+        self._check_img(noise, self.channels, "noise")
         out = c_double()
         with torch.cuda.device(self.device):
             _check(lib().sr3_p_losses(self._h, _ptr(hr), _ptr(s), _ptr(g), _ptr(noise), 1 if loss_type == "l1" else 2, ctypes.byref(out), _stream()))
@@ -378,6 +422,10 @@ class Engine:
         c = None if condition_x is None else _f32c(condition_x, self.device)
         x_T = _f32c(x_T, self.device)
         n = None if noises is None else _f32c(noises, self.device)
+        self._check_inputs(x_T, c)
+        if n is not None and tuple(n.shape[1:]) != (self.batch, self.channels, self.height, self.width):
+            raise ValueError("noises has shape %s; this engine needs [T, %d, %d, %d, %d]" % (tuple(n.shape), self.batch, self.channels,
+                                                                                           self.height, self.width))
         T = self.T
         inter = 1 | (T // 10)
         cap = len([i for i in range(T) if i % inter == 0])
@@ -391,7 +439,8 @@ class Engine:
 
     def super_resolution_host(self, cond_host, x_T_host, seed=0, first_index=0):
         """Host (pinned) buffers in, host buffer out; H2D + T steps + D2H inside one native call."""
-        out = torch.empty(self.batch, self.channels, self.image_size, self.image_size, dtype=torch.float32).pin_memory()
+        self._check_inputs(x_T_host, cond_host)
+        out = torch.empty(self.batch, self.channels, self.height, self.width, dtype=torch.float32).pin_memory()
         with torch.cuda.device(self.device):
             _check(lib().sr3_super_resolution_host(self._h, _ptr(cond_host), _ptr(x_T_host), int(seed), int(first_index), _ptr(out), _stream()))
         return out
@@ -399,6 +448,7 @@ class Engine:
     def loop_begin(self, condition_x, x_T, seed=0, first_index=0):
         c = None if condition_x is None else _f32c(condition_x, self.device)
         x_T = _f32c(x_T, self.device)
+        self._check_inputs(x_T, c)
         with torch.cuda.device(self.device):
             _check(lib().sr3_p_sample_loop_begin(self._h, _ptr(c), _ptr(x_T), int(seed), int(first_index), _stream()))
 

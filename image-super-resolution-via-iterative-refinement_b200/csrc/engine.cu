@@ -1098,6 +1098,20 @@ WgradOut attn_bwd_qkv_out(float* dqkv, int col, int nz, int Lt, int C) {
     return o;
 }
 
+// Image sizes an inference plan runs on: at every UNet level (the image halved n_mults - 1 times) both sides are powers of two and at
+// least 8, except that the lowest level may be exactly 4x4.  Returns the lowest level's side, or throws naming the size and the rule.
+int check_image_size(int n_mults, int height, int width) {
+    auto pow2 = [](int v) { return v > 0 && (v & (v - 1)) == 0; };
+    const int lh = height >> (n_mults - 1), lw = width >> (n_mults - 1);
+    REQUIRE(height > 0 && width > 0, "image size %dx%d: sides must be positive", height, width);
+    REQUIRE(lh >= 4 && lw >= 4, "image size %dx%d: lowest UNet resolution %dx%d < 4 is not supported (%d levels)", height, width, lh, lw, n_mults);
+    REQUIRE(pow2(height) && pow2(width), "image size %dx%d: both sides must be powers of two", height, width);
+    REQUIRE((lh >= 8 && lw >= 8) || (lh == 4 && lw == 4),
+            "image size %dx%d: lowest UNet level %dx%d is not supported (every level must be at least 8x8, or the lowest exactly 4x4)", height, width,
+            lh, lw);
+    return lh < lw ? lh : lw;
+}
+
 }  // namespace
 
 struct sr3_engine {
@@ -1676,27 +1690,30 @@ struct sr3_engine {
         }
     }
 
-    void init(const sr3_unet_config& c, int batch, int device) {
+    // height x width: the size of the images the plan runs on (image_size x image_size unless sr3_engine_create_sized says otherwise).
+    // cfg.image_size only places the attention layers (build_plan); every activation takes its size from height and width.
+    void init(const sr3_unet_config& c, int batch, int height, int width, int device) {
         cfg = c; B = batch; dev = device;
+        REQUIRE(B >= 1, "batch must be >= 1");
+        REQUIRE(cfg.n_mults >= 1 && cfg.n_mults <= SR3_MAX_LEVELS, "bad n_mults");
+        // checked before anything touches the device
+        const int min_h = check_image_size(cfg.n_mults, height, width);
         CK(cudaSetDevice(dev));
         cudaDeviceProp prop;
         CK(cudaGetDeviceProperties(&prop, dev));
         REQUIRE(prop.major == 9 && prop.minor == 0, "sr3_b200 needs an sm_90 GPU (found sm_%d%d); there is no fallback path", prop.major, prop.minor);
-        REQUIRE(B >= 1, "batch must be >= 1");
         REQUIRE(cfg.inner_channel % 64 == 0, "inner_channel must be a multiple of 64 (got %d)", cfg.inner_channel);
         REQUIRE(cfg.in_channel <= 64, "in_channel must be <= 64");
-        REQUIRE(cfg.n_mults >= 1 && cfg.n_mults <= SR3_MAX_LEVELS, "bad n_mults");
         for (int i = 0; i < cfg.n_mults; ++i) REQUIRE((cfg.inner_channel * cfg.channel_mults[i]) % (2 * cfg.norm_groups) == 0 || (cfg.inner_channel * cfg.channel_mults[i]) % cfg.norm_groups == 0, "norm_groups must divide the channel counts");
-        inner = cfg.inner_channel; H = W = cfg.image_size;
+        inner = cfg.inner_channel; H = height; W = width;
         REQUIRE(cfg.precision == 0 || cfg.precision == 1, "precision must be 0 (bf16) or 1 (precise)");
         precise = cfg.precision == 1; PW = precise ? 2 : 1;
         cond_c = cfg.conditional ? cfg.in_channel - cfg.channels : 0;
-        int min_res = cfg.image_size;
-        for (int i = 1; i < cfg.n_mults; ++i) min_res /= 2;
-        REQUIRE(min_res >= 4, "lowest UNet resolution %d < 4 is not supported", min_res);
         // 8x8 levels tile two images per CTA.  A 4x4 level tiles four, and its attention batches hold eight 16-token images, which
         // read (P = 0 makes them inert, but they must be finite) every image slot of their batch: Bp is a multiple of 8, and the
-        // slots no layer writes hold the zeros of the allocation (or, in shared scratch, another layer's finite values).
+        // slots no layer writes hold the zeros of the allocation (or, in shared scratch, another layer's finite values).  What counts
+        // is the lowest level of the images actually run, not the one image_size would give.
+        const int min_res = min_h;
         Bp = min_res == 4 ? (B + 7) & ~7 : (B + 1) & ~1;
         Bt = min_res == 4 ? B : Bp;
         T_cap = 4096;
@@ -1861,13 +1878,17 @@ extern "C" {
 const char* sr3_last_error(void) { return g_err.c_str(); }
 int sr3_abi_version(void) { return 3; }
 
-int sr3_engine_create(const sr3_unet_config* cfg, int batch, int device, sr3_engine** out) {
+int sr3_engine_create_sized(const sr3_unet_config* cfg, int batch, int height, int width, int device, sr3_engine** out) {
     API_BEGIN
     REQUIRE(cfg && out, "null argument");
     std::unique_ptr<sr3_engine> e(new sr3_engine());
-    e->init(*cfg, batch, device);
+    e->init(*cfg, batch, height, width, device);
     *out = e.release();
     API_END
+}
+int sr3_engine_create(const sr3_unet_config* cfg, int batch, int device, sr3_engine** out) {
+    if (!cfg) { g_err = "null argument"; return 1; }
+    return sr3_engine_create_sized(cfg, batch, cfg->image_size, cfg->image_size, device, out);
 }
 int sr3_engine_create_train(const sr3_unet_config* cfg, int batch, int device, float dropout, sr3_engine** out) {
     API_BEGIN
@@ -1875,7 +1896,7 @@ int sr3_engine_create_train(const sr3_unet_config* cfg, int batch, int device, f
     REQUIRE(dropout >= 0.f && dropout < 1.f, "dropout %f out of range", dropout);
     std::unique_ptr<sr3_engine> e(new sr3_engine());
     e->train = true; e->drop_p = dropout;
-    e->init(*cfg, batch, device);
+    e->init(*cfg, batch, cfg->image_size, cfg->image_size, device);
     *out = e.release();
     API_END
 }

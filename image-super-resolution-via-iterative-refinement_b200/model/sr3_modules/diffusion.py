@@ -110,11 +110,16 @@ class GaussianDiffusion(nn.Module):
         mean = self.posterior_mean_coef1[t] * x_start + self.posterior_mean_coef2[t] * x_t
         return mean, self.posterior_log_variance_clipped[t]
 
-    def _engine(self, batch):
-        return self.denoise_fn.engine(batch, conditional=self.conditional, channels=self.channels)
+    def _engine(self, batch, height=None, width=None):
+        """The inference engine for `batch` images of height x width (default image_size x image_size)."""
+        return self.denoise_fn.engine(batch, conditional=self.conditional, channels=self.channels, height=height, width=width)
 
+    def _engine_for(self, x):
+        return self._engine(x.shape[0], x.shape[2], x.shape[3])
+
+    # Like the reference, these take the image size from x / x_in (the UNet is fully convolutional); only sample() uses image_size.
     def p_mean_variance(self, x, t, clip_denoised: bool, condition_x=None):
-        mean, _ = self._engine(x.shape[0]).p_mean_variance(x, t, clip_denoised, condition_x)
+        mean, _ = self._engine_for(x).p_mean_variance(x, t, clip_denoised, condition_x)
         return mean, self.posterior_log_variance_clipped[t]
 
     @torch.no_grad()
@@ -122,7 +127,7 @@ class GaussianDiffusion(nn.Module):
         if not clip_denoised:
             raise NotImplementedError("p_sample always clips, as every caller in the reference does")
         seed = int(torch.randint(0, 2 ** 62, (1,)).item()) if noise is None else 0
-        return self._engine(x.shape[0]).p_sample(x, t, condition_x, noise, seed)
+        return self._engine_for(x).p_sample(x, t, condition_x, noise, seed)
 
     @torch.no_grad()
     def p_sample_loop(self, x_in, continous=False, x_T=None, noises=None, seed=None, first_index=0):
@@ -137,7 +142,7 @@ class GaussianDiffusion(nn.Module):
         img = torch.randn(shape, device=device) if x_T is None else x_T.to(device)
         if seed is None:
             seed = int(torch.randint(0, 2 ** 62, (1,)).item())
-        final, snaps = self._engine(shape[0]).p_sample_loop(cond, img, noises, seed, first_index, want_snapshots=continous)
+        final, snaps = self._engine(shape[0], shape[2], shape[3]).p_sample_loop(cond, img, noises, seed, first_index, want_snapshots=continous)
         if continous:
             first = cond if self.conditional else img
             return torch.cat([first, snaps.reshape(-1, *shape[1:])], dim=0)

@@ -159,7 +159,7 @@ class UNet(nn.Module):
         return self
 
     # ---- native engine management
-    MAX_ENGINES = 4          # distinct (batch, device, ...) engines kept alive; least recently used ones are released
+    MAX_ENGINES = 4          # distinct (batch, image size, device, ...) engines kept alive; least recently used ones are released
 
     def _weights_version(self):
         return sum(p._version for p in self.parameters()) + self._manual_version
@@ -179,20 +179,25 @@ class UNet(nn.Module):
         for eng in self._engines.values():
             eng.set_schedule(*self._schedule)
 
-    def engine(self, batch, conditional=True, channels=3, train_dropout=None):
+    def engine(self, batch, conditional=True, channels=3, train_dropout=None, height=None, width=None):
         """train_dropout=None: the inference plan; a float: the TRAINING plan (intermediates kept, backward recorded) with that Dropout
-        probability -- see GaussianDiffusion.p_losses."""
+        probability -- see GaussianDiffusion.p_losses.  height / width: the image size the plan runs on (default image_size; any size
+        _native.check_image_size accepts, inference plans only).  Engines are kept per (batch, size, ...), and every one of them re-packs
+        the weights before its next use once they changed."""
         dev = next(self.parameters()).device
-        key = (batch, str(dev), bool(conditional), channels, self.precision, train_dropout)
+        size = self.arch["image_size"]
+        h, w = int(size if height is None else height), int(size if width is None else width)
+        key = (batch, h, w, str(dev), bool(conditional), channels, self.precision, train_dropout)
         eng = self._engines.pop(key, None)
         if eng is None:
+            _native.check_image_size(len(self.arch["channel_mults"]), h, w)      # before an older engine is released
             while len(self._engines) >= self.MAX_ENGINES:            # dicts keep insertion order: the first key is the least recently used
                 old = next(iter(self._engines))
                 del self._engines[old], self._engine_versions[old]
             if train_dropout is not None and self.precision != "bf16":
                 raise NotImplementedError("sr3_b200: the training plan supports precision='bf16' only")
             cfg = dict(self.arch, channels=channels, conditional=conditional, precision=self.precision)
-            eng = _native.Engine(cfg, batch, dev, train_dropout=train_dropout)
+            eng = _native.Engine(cfg, batch, dev, train_dropout=train_dropout, height=h, width=w)
             self._engine_versions[key] = -1
             if self._schedule is not None:
                 eng.set_schedule(*self._schedule)
@@ -211,9 +216,11 @@ class UNet(nn.Module):
         return eng
 
     def forward(self, x, time):
-        """x [B,in_channel,H,W] fp32, time = noise level [B,1] -> eps [B,out_channel,H,W] (unet.py:235-259)."""
+        """x [B,in_channel,H,W] fp32, time = noise level [B,1] -> eps [B,out_channel,H,W] (unet.py:235-259).  H x W is any size
+        _native.check_image_size accepts; attention stays on the levels image_size placed it on."""
         if torch.is_grad_enabled() and x.requires_grad:
             raise NotImplementedError("sr3_b200: backward through the native UNet is not implemented yet (inference / loss value only)")
         a = self.arch
-        eng = self.engine(x.shape[0], conditional=a["in_channel"] != a["out_channel"], channels=a["out_channel"])
+        eng = self.engine(x.shape[0], conditional=a["in_channel"] != a["out_channel"], channels=a["out_channel"], height=x.shape[2],
+                          width=x.shape[3])
         return eng.unet_forward(x, time)

@@ -49,12 +49,21 @@ int sr3_abi_version(void);
 
 /* UNet.__init__ (model/sr3_modules/unet.py:161-233) + GaussianDiffusion.__init__ (diffusion.py:64-82):
  * builds the layer plan, allocates activations / packed weights on `device` for a fixed batch size.
+ * Runs image_size x image_size images (sr3_engine_create_sized: other sizes).
  * The lowest UNet level (image_size / 2^(n_mults - 1)) must be at least 4x4; a net with a 4x4 level allocates its activations for the batch
  * rounded up to 8 images, but launches the work of the real images only.
  * Threading: calls on one engine must be serialised by the caller.  Kernels whose CTAs wait for partners are safe next to other work on the
  * device: the split-K partners of a tile are one thread-block cluster (gang-scheduled by the hardware), the persistent step kernel (SR3_MEGA=1)
  * is a cooperative launch -- engines driven concurrently from different streams of one device cannot deadlock each other. */
 int sr3_engine_create(const sr3_unet_config* cfg, int batch, int device, sr3_engine** out);
+/* The same inference plan for images of height x width instead of image_size x image_size: the reference UNet is fully convolutional and
+ * runs whatever size it is given (unet.py:235-259; p_sample_loop takes its shape from x_in, diffusion.py:188-200).  cfg->image_size still
+ * decides which levels get self-attention (unet.py:186-231: `now_res in attn_res` at construction); the attention itself runs over the
+ * h * w tokens of the level it sits on.  Supported sizes: at every level (height and width halved n_mults - 1 times) both sides are powers
+ * of two and at least 8, or the lowest level is exactly 4x4; anything else fails before any allocation.  The batch of a plan whose lowest
+ * level is 4x4 is padded to 8 as above.  sr3_engine_create(cfg, ...) is sr3_engine_create_sized(cfg, ..., image_size, image_size, ...).
+ * Every entry point below then reads and writes [B,C,height,width] images.  Training plans (sr3_engine_create_train) run at image_size. */
+int sr3_engine_create_sized(const sr3_unet_config* cfg, int batch, int height, int width, int device, sr3_engine** out);
 void sr3_engine_destroy(sr3_engine* e);
 
 /* Parameter table in the reference's state_dict order and naming ("downs.1.res_block.block1.block.3.weight", ...;
