@@ -117,6 +117,8 @@ _SIGS = {
     "sr3_test_attention_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
                                        c_void_p]),
     "sr3_test_film_embed_bwd": (c_int, [POINTER(TestFilmArgsC), c_void_p]),
+    "sr3_test_film_embed_fwd": (c_int, [c_void_p] * 10 + [c_int, c_int, c_int, c_void_p]),
+    "sr3_test_attention_unfused": (c_int, [c_void_p] * 5 + [c_int] * 5 + [c_void_p]),
     "sr3_test_loss_grad": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, POINTER(c_double), c_void_p, c_int, c_void_p, c_void_p]),
 }
 EXPORTED_SYMBOLS = tuple(_SIGS.keys())
@@ -704,6 +706,28 @@ def test_film_embed_bwd(wf, tau, dfilm, nl, w1, b1, w2, gscale=1.0):
     a.F, a.inner, a.B, a.gscale = F, inner, B, float(gscale)
     _check(lib().sr3_test_film_embed_bwd(ctypes.byref(a), _stream()))
     return out
+
+
+def test_film_embed_fwd(nl, w1, b1, w2, b2, wf, bf, cb):
+    """embed_kernel + film_kernel as the plan launches them; CUDA fp32 operands, nl [B].  Returns (tau [B, inner], film [B, F])."""
+    F, inner = wf.shape
+    B = nl.numel()
+    tau = torch.empty(B, inner, device=wf.device)
+    film = torch.empty(B, F, device=wf.device)
+    _check(lib().sr3_test_film_embed_fwd(*[_ptr(t) for t in (nl, w1, b1, w2, b2, wf, bf, cb, tau, film)], F, inner, B, _stream()))
+    return tau, film
+
+
+def test_attention_unfused(qk, vT, nz, Lt, HW, C, precise=False):
+    """The unfused attention launches: qk bf16 [nz*Lt, 2C PW], vT bf16 [nz*C, Lt PW] (PW = 2 in precise mode) -> (S fp32 [nz*Lt, Lt],
+    P bf16 [nz*Lt, Lt PW], O bf16 [nz*Lt, C PW])."""
+    pw = 2 if precise else 1
+    dev = qk.device
+    S = torch.empty(nz * Lt, Lt, device=dev)
+    P = torch.empty(nz * Lt, Lt * pw, device=dev, dtype=torch.bfloat16)
+    O = torch.empty(nz * Lt, C * pw, device=dev, dtype=torch.bfloat16)
+    _check(lib().sr3_test_attention_unfused(_ptr(qk), _ptr(vT), _ptr(S), _ptr(P), _ptr(O), nz, Lt, HW, C, int(bool(precise)), _stream()))
+    return S, P, O
 
 
 def test_loss_grad(noise, eps, l2, deps=None, ld=64):

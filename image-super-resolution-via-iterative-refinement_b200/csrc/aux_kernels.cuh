@@ -302,31 +302,35 @@ __global__ void __launch_bounds__(256) embed_kernel(const EmbedParams p) {
 
 // All FeatureWiseAffine projections at once (unet.py:34-50, bias-only form) + the block1 conv bias folded in:
 // film[b][j] = Wf[j] . tau[b] + bf[j] + cbias[j],  j over the concatenated Cout of every ResnetBlock.
-// A block owns 64 outputs: their weight rows are staged (coalesced) in padded smem together with tau of every image.
+// A block owns 64 outputs: their weight rows are staged (coalesced) in padded smem, tau in chunks of `chunk` images (any batch fits).
 __global__ void __launch_bounds__(256) film_kernel(const float* __restrict__ wf, const float* __restrict__ bf, const float* __restrict__ cbias,
-                                                   const float* __restrict__ tau, float* __restrict__ film, int F, int inner, int B) {
+                                                   const float* __restrict__ tau, float* __restrict__ film, int F, int inner, int B, int chunk) {
     pdl_launch_dependents();
     pdl_wait();
     extern __shared__ float sm[];
     float* ws = sm;                          // [64][inner + 1]
-    float* ts = sm + 64 * (inner + 1);       // [B][inner]
+    float* ts = sm + 64 * (inner + 1);       // [chunk][inner]
     const int j0 = blockIdx.x * 64;
     for (int i = threadIdx.x; i < 64 * inner; i += blockDim.x) {
         const int r = i / inner, c = i % inner;
         ws[r * (inner + 1) + c] = (j0 + r < F) ? __ldg(&wf[static_cast<long long>(j0 + r) * inner + c]) : 0.f;
     }
-    for (int i = threadIdx.x; i < B * inner; i += blockDim.x) ts[i] = __ldg(&tau[i]);
-    __syncthreads();
     const int jl = threadIdx.x & 63, bq = threadIdx.x >> 6;
     const int j = j0 + jl;
-    if (j >= F) return;
-    const float base = bf[j] + cbias[j];
+    const float base = j < F ? bf[j] + cbias[j] : 0.f;
     const float* w = ws + jl * (inner + 1);
-    for (int b = bq; b < B; b += 4) {
-        float a = base;
-        const float* t = ts + b * inner;
-        for (int i = 0; i < inner; ++i) a += w[i] * t[i];
-        film[static_cast<long long>(b) * F + j] = a;
+    for (int b0 = 0; b0 < B; b0 += chunk) {
+        const int nb = min(chunk, B - b0);
+        __syncthreads();                     // (the previous chunk's tau is no longer read)
+        for (int i = threadIdx.x; i < nb * inner; i += blockDim.x) ts[i] = __ldg(&tau[static_cast<long long>(b0) * inner + i]);
+        __syncthreads();
+        if (j >= F) continue;
+        for (int b = bq; b < nb; b += 4) {
+            float a = base;
+            const float* t = ts + b * inner;
+            for (int i = 0; i < inner; ++i) a += w[i] * t[i];
+            film[static_cast<long long>(b0 + b) * F + j] = a;
+        }
     }
 }
 

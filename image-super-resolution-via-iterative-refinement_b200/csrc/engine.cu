@@ -958,6 +958,23 @@ void launch_loss_grad(const float* noise, const float* eps, int B, int C, int H,
     CK(cudaGetLastError());
 }
 
+// ---- noise-level embedding + FiLM projections forward (the plan's first two launches; sr3_test_film_embed_fwd)
+constexpr int FILM_SMEM_BYTES = 48 * 1024;      // film_kernel stays within the default dynamic shared-memory limit (no opt-in)
+// images of tau film_kernel stages at once next to its 64 weight rows; larger batches are walked in chunks of this many
+int film_tau_chunk(int inner, int B) {
+    const int cap = (FILM_SMEM_BYTES / 4 - 64 * (inner + 1)) / inner;
+    REQUIRE(cap >= 1, "FiLM projections: inner_channel %d does not fit film_kernel's %d KB of shared memory", inner, FILM_SMEM_BYTES / 1024);
+    return std::min(B, cap);
+}
+void launch_embed(const EmbedParams& ep, int B, cudaStream_t st) {
+    launch_k(embed_kernel, dim3(B), dim3(256), (size_t)(5 * ep.inner * 4), st, ep);
+}
+void launch_film(const float* wf, const float* bf, const float* cb, const float* tau, float* film, int F, int inner, int B, cudaStream_t st) {
+    const int chunk = film_tau_chunk(inner, B);
+    launch_k(film_kernel, dim3((F + 63) / 64), dim3(256), (size_t)((64 * (inner + 1) + chunk * inner) * 4), st, wf, bf, cb, tau, film, F, inner, B,
+             chunk);
+}
+
 // ---- FiLM projections + noise-level MLP backward: one block's shared memory holds every image's embedding (and the MLP's hidden layer)
 constexpr int FILM_BWD_SMEM_MAX = 200 * 1024;
 int film_bwd_smem(int B, int inner) { return 2 * B * inner * 4; }
@@ -1041,6 +1058,41 @@ ConvArgs upsample_dgrad_conv(const bf16* dy, int Bp, int yH, int yW, int C, cons
     c.w = w; c.ktot = 16 * C; c.cout = C; c.OH = yH / 2; c.OW = yW / 2;
     Act o; o.p = out; o.C = C; o.H = yH / 2; o.W = yW / 2; c.out = o;
     return c;
+}
+
+// ---- unfused attention forward (attention batches the fused kernel does not take, precise mode, training): nz batches of Lt tokens, HW
+// tokens per image, head dim C; PW = 2 in precise mode (every bf16 row is [hi | lo])
+// S[z] = q k^T / sqrt(C): qk bf16 [nz][Lt][2C PW] (rows [q_hi | k_hi | q_lo | k_lo]) -> S fp32 [nz][Lt][Lt]
+GemmDesc attn_s_desc(const bf16* qk, float* S, int nz, int Lt, int C, int PW) {
+    GemmDesc d; d.n_a = 1; d.a[0] = matrix_src(qk, nz, Lt, 2 * C * PW, 2 * C * PW, (long long)Lt * 2 * C * PW);
+    for (int c = 0; c < C; c += 64) d.slabs.push_back({0, c, 0, 0, 0, C + c});
+    if (PW == 2) set_precise_fields(d, 2 * C, 0, 2 * C);
+    d.block_n = 128; d.b_ptr = qk; d.b_K = 2 * C * PW; d.b_rows = (long long)nz * Lt;
+    d.w_box = 128; d.h_box = 1; d.b_box = 1; d.tiles_w = Lt / 128; d.tiles_h = 1; d.tiles_b = 1;
+    d.n_tiles = Lt / 128; d.nz = nz; d.a_zstep = 1; d.b_zrows = Lt;
+    d.OW = Lt; d.OH = 1; d.OB = nz; d.n_valid = Lt; d.scale = 1.0f / sqrtf((float)C);
+    d.out_f32 = S; d.os = OutSpec{0, (long long)Lt * Lt, 0, Lt, 0};
+    return d;
+}
+// P = softmax of each S row over the keys of its own image (segments of HW keys), bf16 [nz][Lt][Lt PW]
+SoftmaxParams attn_softmax_params(const float* S, bf16* P, int nz, int Lt, int HW, int PW) {
+    SoftmaxParams sp{}; sp.S = S; sp.P = P; sp.rows = (long long)nz * Lt; sp.L = Lt; sp.seg = HW; sp.precise = PW == 2 ? 1 : 0;
+    return sp;
+}
+void launch_softmax(const SoftmaxParams& sp, cudaStream_t st) {
+    launch_k(softmax_kernel, dim3((int)((sp.rows + 7) / 8)), dim3(256), 0, st, sp.S, sp.P, sp.rows, sp.L, sp.seg, sp.precise);
+}
+// O[z] = P v: rows = queries, N = head dim, K = keys.  vT bf16 [nz][C][Lt PW] -> O bf16 [nz][Lt][C PW]
+GemmDesc attn_pv_desc(const bf16* P, const bf16* vT, bf16* O, int nz, int Lt, int C, int PW) {
+    GemmDesc d; d.n_a = 1; d.a[0] = matrix_src(P, nz, Lt, Lt * PW, Lt * PW, (long long)Lt * Lt * PW);
+    for (int c = 0; c < Lt; c += 64) d.slabs.push_back({0, c, 0, 0, 0, c});
+    if (PW == 2) set_precise_fields(d, Lt, 0, Lt);
+    d.block_n = 128; d.b_ptr = vT; d.b_K = Lt * PW; d.b_rows = (long long)nz * C;
+    d.w_box = 128; d.h_box = 1; d.b_box = 1; d.tiles_w = Lt / 128; d.tiles_h = 1; d.tiles_b = 1;
+    d.n_tiles = C / 128; d.nz = nz; d.a_zstep = 1; d.b_zrows = C;
+    d.OW = Lt; d.OH = 1; d.OB = nz; d.n_valid = C;
+    d.out_bf16 = O; d.hs = OutSpec{0, (long long)Lt * C * PW, 0, (long long)C * PW, 0}; d.lo_out_off = PW == 2 ? C : 0;
+    return d;
 }
 
 // ---- attention backward: the four matrix products of nz attention batches of Lt tokens, head dim C
@@ -1466,36 +1518,11 @@ struct sr3_engine {
             const double fl = 4.0 * nz * (double)Lt * Lt * C;
             push(make_attn_op(qk, vT, O, nz, Lt, HW, C), 5, fl, (double)nz * Lt * C * 2 * 4);
         } else {
-            {   // S[z] = q k^T / sqrt(C)
-                GemmDesc d; d.n_a = 1; d.a[0] = matrix_src(qk, nz, Lt, 2 * C * PW, 2 * C * PW, (long long)Lt * 2 * C * PW);
-                for (int c = 0; c < C; c += 64) d.slabs.push_back({0, c, 0, 0, 0, C + c});
-                set_precise(d, 2 * C, 0, 2 * C);
-                d.block_n = 128; d.b_ptr = qk; d.b_K = 2 * C * PW; d.b_rows = (long long)Bp * HW;
-                d.w_box = 128; d.h_box = 1; d.b_box = 1; d.tiles_w = Lt / 128; d.tiles_h = 1; d.tiles_b = 1;
-                d.n_tiles = Lt / 128; d.nz = nz; d.a_zstep = 1; d.b_zrows = Lt;
-                d.OW = Lt; d.OH = 1; d.OB = nz; d.n_valid = Lt; d.scale = 1.0f / sqrtf((float)C);
-                d.out_f32 = S; d.os = OutSpec{0, (long long)Lt * Lt, 0, Lt, 0};
-                push_gemm(d);
-            }
-            {
-                const long long rows = (long long)nz * Lt;
-                const int blocks = (int)((rows + 7) / 8);
-                const int prec = precise ? 1 : 0;
-                push([=](cudaStream_t st) { launch_k(softmax_kernel, dim3(blocks), dim3(256), 0, st, (const float*)S, P, rows, Lt, HW, prec); }, 3, 0, (double)rows * Lt * 6.0);
-                SoftmaxParams sp{}; sp.S = S; sp.P = P; sp.rows = rows; sp.L = Lt; sp.seg = HW; sp.precise = prec;
-                mega_record(MOP_SOFTMAX, sp);
-            }
-            {   // O[z] = P v : rows = queries, N = head dim, K = keys
-                GemmDesc d; d.n_a = 1; d.a[0] = matrix_src(P, nz, Lt, Lt * PW, Lt * PW, (long long)Lt * Lt * PW);
-                for (int c = 0; c < Lt; c += 64) d.slabs.push_back({0, c, 0, 0, 0, c});
-                set_precise(d, Lt, 0, Lt);
-                d.block_n = 128; d.b_ptr = vT; d.b_K = Lt * PW; d.b_rows = (long long)nz * C;
-                d.w_box = 128; d.h_box = 1; d.b_box = 1; d.tiles_w = Lt / 128; d.tiles_h = 1; d.tiles_b = 1;
-                d.n_tiles = C / 128; d.nz = nz; d.a_zstep = 1; d.b_zrows = C;
-                d.OW = Lt; d.OH = 1; d.OB = nz; d.n_valid = C;
-                d.out_bf16 = O; d.hs = OutSpec{0, (long long)Lt * C * PW, 0, (long long)C * PW, 0}; d.lo_out_off = precise ? C : 0;
-                push_gemm(d);
-            }
+            push_gemm(attn_s_desc(qk, S, nz, Lt, C, PW));
+            const SoftmaxParams sp = attn_softmax_params(S, P, nz, Lt, HW, PW);
+            push([=](cudaStream_t st) { launch_softmax(sp, st); }, 3, 0, (double)sp.rows * Lt * 6.0);
+            mega_record(MOP_SOFTMAX, sp);
+            push_gemm(attn_pv_desc(P, vT, O, nz, Lt, C, PW));
         }
         {   // out projection + bias + residual (un-normalised input)
             ConvArgs c; c.n_a = 1; c.a[0] = nhwc_src(O, Bp, Hh, Ww, C * PW); c.c0 = C;
@@ -1574,11 +1601,12 @@ struct sr3_engine {
             push([=](cudaStream_t st) { launch_k(step_begin_kernel, dim3((int)std::min<long long>((n4 + 255) / 256, 592)), dim3(256), 0, st, sa, n4, c); });
             EmbedParams ep{}; ep.ctl = ctl_dev; ep.nl_table = nl_table; ep.nl_buf = nl_buf; ep.w1 = mlp_w1; ep.b1 = mlp_b1; ep.w2 = mlp_w2; ep.b2 = mlp_b2;
             ep.tau = tau; ep.inner = inner;
-            const int Bn = B; const int esm = 5 * inner * 4;
+            const int Bn = B;
+            film_tau_chunk(inner, B);                   // (refuses an inner_channel film_kernel cannot stage before anything is launched)
             side_begin = (int)ops.size();
-            push([=](cudaStream_t st) { launch_k(embed_kernel, dim3(Bn), dim3(256), (size_t)esm, st, ep); });
+            push([=](cudaStream_t st) { launch_embed(ep, Bn, st); });
             float *fw = film_w, *fb = film_b, *fc = film_cb, *ta = tau, *fi = film; const int Fn = F, inn = inner;
-            push([=](cudaStream_t st) { launch_k(film_kernel, dim3((Fn + 63) / 64), dim3(256), (size_t)((64 * (inn + 1) + Bn * inn) * 4), st, (const float*)fw, (const float*)fb, (const float*)fc, (const float*)ta, fi, Fn, inn, Bn); });
+            push([=](cudaStream_t st) { launch_film(fw, fb, fc, ta, fi, Fn, inn, Bn, st); });
             side_end = (int)ops.size();
             EmbedFilmParams fp{}; fp.e = ep; fp.wf = film_w; fp.bf = film_b; fp.cbias = film_cb; fp.film = film; fp.F = F; fp.B = B;
             mega_record(MOP_EMBED_FILM, fp);
@@ -1769,6 +1797,11 @@ struct sr3_engine {
         // SR3_MEGA=1 selects it (bit-identical results).
         use_mega = !train && getenv("SR3_MEGA") != nullptr && atoi(getenv("SR3_MEGA")) != 0;
         if (!use_mega) return;
+        {   // embed_film_body keeps tau of every image in the op region of shared memory (after the 1024-byte alignment and the header)
+            const long long need = embed_film_smem_bytes(B, inner, F, num_sms()), room = SMEM_LIMIT - 1024 - GEMM_HDR_BYTES;
+            REQUIRE(need <= room, "step kernel (SR3_MEGA=1): the noise embedding + FiLM op needs %lld bytes of shared memory at batch %d "
+                    "(inner_channel %d), its op region holds %lld; use a smaller batch or the per-layer path", need, B, inner, room);
+        }
         std::vector<MegaOp> host_ops;
         std::vector<uint8_t> blob;
         for (size_t i = 0; i < mega.size(); ++i) {
@@ -2363,6 +2396,21 @@ int sr3_test_attention(const void* qk, const void* vT, void* out, int nz, int Lt
     API_END
 }
 
+int sr3_test_attention_unfused(const void* qk, const void* vT, float* S, void* P, void* O, int nz, int Lt, int HW, int C, int precise,
+                               void* stream) {
+    API_BEGIN
+    REQUIRE(qk && vT && S && P && O, "null argument");
+    REQUIRE(nz >= 1 && Lt % 128 == 0 && C % 128 == 0 && HW >= 1 && Lt % HW == 0, "unfused attention geometry Lt=%d HW=%d C=%d", Lt, HW, C);
+    const int PW = precise ? 2 : 1;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    DevAllocs mem;
+    make_gemm_op(attn_s_desc(static_cast<const bf16*>(qk), S, nz, Lt, C, PW), mem)(st);
+    launch_softmax(attn_softmax_params(S, static_cast<bf16*>(P), nz, Lt, HW, PW), st);
+    make_gemm_op(attn_pv_desc(static_cast<const bf16*>(P), static_cast<const bf16*>(vT), static_cast<bf16*>(O), nz, Lt, C, PW), mem)(st);
+    CK(cudaStreamSynchronize(st));
+    API_END
+}
+
 int sr3_bench_conv(int B, int H, int W, int Cin, int Cout, int ksize, int stride, int with_resid, int with_stats, int reps, float* ms_out) {
     API_BEGIN
     REQUIRE(ms_out && reps > 0, "bad arguments");
@@ -2878,6 +2926,23 @@ int sr3_test_film_embed_bwd(const sr3_test_film_args* a, void* stream) {
     CK(cudaMemsetAsync(a->dtau, 0, (size_t)a->B * a->inner * sizeof(float), st));
     launch_film_bwd(a->wf, a->tau, a->dfilm, a->dwf, a->dbf, a->dcb, a->dtau, a->F, a->inner, a->B, a->gscale, st);
     launch_embed_bwd(a->nl, a->w1, a->b1, a->w2, a->dtau, a->dw1, a->db1, a->dw2, a->db2, a->inner, a->B, a->gscale, st);
+    CK(cudaStreamSynchronize(st));
+    API_END
+}
+
+int sr3_test_film_embed_fwd(const float* nl, const float* w1, const float* b1, const float* w2, const float* b2, const float* wf, const float* bf,
+                            const float* cb, float* tau, float* film, int F, int inner, int B, void* stream) {
+    API_BEGIN
+    REQUIRE(nl && w1 && b1 && w2 && b2 && wf && bf && cb && tau && film, "null argument");
+    REQUIRE(F >= 1 && inner >= 2 && inner % 2 == 0 && B >= 1, "bad shape");
+    film_tau_chunk(inner, B);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    DevAllocs mem;
+    StepCtl* ctl = static_cast<StepCtl*>(mem.alloc(sizeof(StepCtl), false));
+    CK(cudaMemsetAsync(ctl, 0, sizeof(StepCtl), st));           // nl_from_table = 0: image b's noise level is nl[b]
+    EmbedParams ep{}; ep.ctl = ctl; ep.nl_buf = nl; ep.w1 = w1; ep.b1 = b1; ep.w2 = w2; ep.b2 = b2; ep.tau = tau; ep.inner = inner;
+    launch_embed(ep, B, st);
+    launch_film(wf, bf, cb, tau, film, F, inner, B, st);
     CK(cudaStreamSynchronize(st));
     API_END
 }

@@ -209,6 +209,10 @@ __device__ __noinline__ void softmax_body(const SoftmaxParams& p, const int cta,
 // PositionalEncoding + noise_level_mlp (unet.py:18-31,177-184) and this CTA's share of the FeatureWiseAffine projections
 // (unet.py:34-50, bias-only form, block1's conv bias folded in).  Every CTA recomputes tau (32 K MACs per distinct noise level: cheaper
 // than a grid barrier); during sampling all images share the step's noise level, so tau is computed once.
+// Shared memory it uses on ncta CTAs: pe, h, tau of every image and the CTA's share of the FiLM weight rows (padded rows).
+__host__ __device__ constexpr long long embed_film_smem_bytes(int B, int inner, int F, int ncta) {
+    return 4ll * (5ll * inner + static_cast<long long>(B) * inner + static_cast<long long>((F + ncta - 1) / ncta) * (inner + 1));
+}
 __device__ __noinline__ void embed_film_body(const EmbedFilmParams& p, float* sm, const int t_step, const int cta, const int ncta) {
     const int inner = p.e.inner, hid = 4 * inner, B = p.B;
     const int from_table = p.e.ctl->nl_from_table;

@@ -219,6 +219,12 @@ int sr3_test_gemm(const void* a_bf16, const void* b_bf16, float* d, int M, int N
 /* Test hook for the fused attention core (S = q k^T / sqrt(C), softmax per image, O = P v; unet.py:129-139): qk bf16 [nz*Lt][2C]
  * (q | k), vT bf16 [nz*C][Lt], out bf16 [nz*Lt][C]; Lt in {128, 256} keys per attention batch, HW tokens per image (Lt % HW == 0). */
 int sr3_test_attention(const void* qk_bf16, const void* vT_bf16, void* out_bf16, int nz, int Lt, int HW, int C, void* stream);
+/* Test hook for the unfused attention path (attention batches of other sizes, precise mode, training), the plan's three launches:
+ * S = q k^T / sqrt(C) on the tile kernel, softmax_kernel over the keys of each image, O = P v on the tile kernel.  qk bf16 [nz*Lt][2C PW]
+ * (rows [q | k], precise = 1: [q_hi | k_hi | q_lo | k_lo]), vT bf16 [nz*C][Lt PW] -> S fp32 [nz*Lt][Lt], P bf16 [nz*Lt][Lt PW],
+ * O bf16 [nz*Lt][C PW]; PW = 2 in precise mode (rows [hi | lo]), else 1.  Lt % 128 == 0, C % 128 == 0, HW tokens per image (Lt % HW == 0). */
+int sr3_test_attention_unfused(const void* qk_bf16, const void* vT_bf16, float* S, void* P_bf16, void* O_bf16, int nz, int Lt, int HW, int C,
+                               int precise, void* stream);
 /* Stand-alone NHWC conv for unit tests: x bf16 [B,H,W,Cin], w fp32 OIHW [Cout,Cin,k,k] (k in {1,3}), stride in {1,2},
  * y fp32 [B,OH,OW,Cout]; stats (optional) fp64 [B,Cout,2] (sum, sum of squares per image and channel: the GroupNorm statistics of
  * unet.py:84, accumulated with order-independent fp64 atomics) must be zeroed by the caller. */
@@ -312,6 +318,11 @@ typedef struct sr3_test_film_args {
     float gscale;
 } sr3_test_film_args;
 int sr3_test_film_embed_bwd(const sr3_test_film_args* args, void* stream);
+/* The forward of the same two layers as the plan launches them (embed_kernel, then film_kernel): nl [B] (one noise level per image),
+ * w1 [4 inner][inner], b1 [4 inner], w2 [inner][4 inner], b2 [inner], wf [F][inner], bf [F], cb [F] (block1 conv biases) ->
+ * tau [B][inner], film [B][F] = wf tau + bf + cb.  Any batch that fits in device memory. */
+int sr3_test_film_embed_fwd(const float* nl, const float* w1, const float* b1, const float* w2, const float* b2, const float* wf, const float* bf,
+                            const float* cb, float* tau, float* film, int F, int inner, int B, void* stream);
 /* loss_grad_kernel: noise, eps fp32 NCHW [B][C][H][W] (H * W a multiple of 32) -> *loss_host = sum |eps - noise| (l2 = 0) or
  * sum (eps - noise)^2 (l2 = 1); deps bf16 [B][H][W][ld] channels 0..C-1 = sign(d) or 2 d (the rest untouched); bias_sum [C] += its sums. */
 int sr3_test_loss_grad(const float* noise, const float* eps, int B, int C, int H, int W, int l2, double* loss_host, void* deps_bf16, int ld,

@@ -181,7 +181,9 @@ def test_precise_mode_at_4x4(monkeypatch, B):
 
 @pytest.mark.parametrize("nz,C", [(1, 128), (2, 512)])
 def test_attention_16_tokens_per_image(nz, C):
-    """Eight 4x4 images (16 tokens each) share a 128-token attention batch under the block-diagonal mask."""
+    """Eight 4x4 images (16 tokens each) share a 128-token attention batch under the block-diagonal mask (reference and bound:
+    tests/_attention_ref.py)."""
+    from _attention_ref import check_fused
     from sr3_b200 import _native
     Lt, HW = 128, 16
     g = torch.Generator().manual_seed(nz + C)
@@ -190,11 +192,7 @@ def test_attention_16_tokens_per_image(nz, C):
     vb = v.bfloat16()
     out = _native.test_attention(qk.reshape(nz * Lt, 2 * C).cuda(), vb.transpose(1, 2).contiguous().reshape(nz * C, Lt).cuda(),
                                  nz, Lt, HW, C).float().cpu().reshape(nz, Lt, C)
-    S = qk[..., :C].float() @ qk[..., C:].float().transpose(1, 2) / C ** 0.5
-    seg = torch.arange(Lt) // HW
-    ref = torch.softmax(S.masked_fill(seg[:, None] != seg[None, :], float("-inf")), dim=-1) @ vb.float()
-    assert torch.isfinite(out).all()
-    assert rel(out, ref) < 6e-3, rel(out, ref)
+    check_fused(out, qk, vb, Lt, HW, C)
 
 
 @pytest.mark.parametrize("B,k,stride", [(1, 3, 1), (3, 3, 1), (5, 1, 1), (3, 3, 2), (5, 3, 2)])
