@@ -95,8 +95,6 @@ _SIGS = {
                                   POINTER(c_double), c_void_p]),
     "sr3_engine_num_launches_per_step": (c_int, [c_void_p]),
     "sr3_engine_num_ops_per_step": (c_int, [c_void_p]),
-    "sr3_engine_uses_step_kernel": (c_int, [c_void_p]),
-    "sr3_engine_step_kernel_profile": (c_int, [c_void_p, c_int, POINTER(c_int), POINTER(c_double), POINTER(c_double), POINTER(c_int), c_void_p]),
     "sr3_engine_workspace_bytes": (c_int64, [c_void_p]),
     "sr3_engine_read_activation": (c_int, [c_void_p, c_char_p, c_void_p, c_int64, POINTER(c_int64), POINTER(c_int), c_void_p]),
     "sr3_bench_conv": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, POINTER(c_float)]),
@@ -486,21 +484,9 @@ class Engine:
         return lib().sr3_engine_num_ops_per_step(self._h)
 
     def uses_step_kernel(self):
-        return bool(lib().sr3_engine_uses_step_kernel(self._h))
-
-    STEP_OP_NAMES = {0: "gemm_tile", 1: "groupnorm_apply", 2: "attention", 3: "softmax", 4: "embed_film", 5: "stats_clear"}
-
-    def step_kernel_profile(self, phases=False):
-        """[(op type, microseconds)] of the most recent persistent-step-kernel launch (device globaltimer stamps of CTA 0);
-        phases=True: [(op type, us, (set-up, barrier wait, body, end fence))]."""
-        cap = 4096
-        types, us, ph = (c_int * cap)(), (c_double * cap)(), (c_double * (4 * cap))()
-        n = c_int()
-        with torch.cuda.device(self.device):
-            _check(lib().sr3_engine_step_kernel_profile(self._h, cap, types, us, ph, ctypes.byref(n), _stream()))
-        if phases:
-            return [(types[i], us[i], tuple(ph[4 * i + k] for k in range(4))) for i in range(n.value)]
-        return [(types[i], us[i]) for i in range(n.value)]
+        # Every reverse step runs as the graph of per-layer launches.  Kept for bench.py, which asks before it reads a per-op
+        # step-kernel profile.
+        return False
 
     def workspace_bytes(self):
         return lib().sr3_engine_workspace_bytes(self._h)

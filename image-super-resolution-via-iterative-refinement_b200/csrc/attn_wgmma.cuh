@@ -33,10 +33,9 @@ struct AttnParams {
     float scale_log2e;       // log2(e) / sqrt(C)
 };
 
-// One (attention batch z, query tile qt, channel slice dc) unit for Lt = LT keys and DN output channels.  MEGA = false: the body of
-// attn_kernel (one unit per CTA).  MEGA = true: called by step_kernel for every unit of this CTA; `pm` is the global-memory copy of
-// the parameters (TMA descriptors).
-template <int LT, int DN, bool MEGA>
+// One (attention batch z, query tile qt, channel slice dc) unit for Lt = LT keys and DN output channels: the body of attn_kernel (one
+// unit per CTA).  `pm` points at the parameters in the kernel parameter space (TMA descriptors are addressed through it).
+template <int LT, int DN>
 __device__ __forceinline__ void attn_unit_t(const AttnParams& p, const AttnParams* pm, const uint32_t base_in, uint8_t* base_ptr_in,
                                             const int qt, const int dc, const int z) {
     const uint32_t bar_base = base_in;                                 // header (gemm_wgmma.cuh)
@@ -55,17 +54,12 @@ __device__ __forceinline__ void attn_unit_t(const AttnParams& p, const AttnParam
     if (threadIdx.x == 0) {
         tma_prefetch_desc(&pm->qk_map);
         tma_prefetch_desc(&pm->vt_map);
-        if constexpr (MEGA) {
-            for (int i = 0; i < HDR_NUM_BARS; ++i) mbar_inval(bar_base + 8u * i);
-        }
         for (int s = 0; s < ATTN_STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 2); }   // empty: one arrive per warpgroup
         fence_mbar_init();
     }
     __syncthreads();
-    if constexpr (!MEGA) {
-        pdl_launch_dependents();
-        pdl_wait();                  // q, k, vT come from the two preceding launches
-    }
+    pdl_launch_dependents();
+    pdl_wait();                  // q, k, vT come from the two preceding launches
 
     if (warp == ATTN_PRODUCER_WARP) {
         // ------------------------------------------------------------ TMA producer
@@ -88,13 +82,6 @@ __device__ __forceinline__ void attn_unit_t(const AttnParams& p, const AttnParam
             }
             __syncwarp();
             if (++s == ATTN_STAGES) { s = 0; ph ^= 1u; }
-        }
-        if constexpr (MEGA) {        // tail: no arrival may be in flight when the barriers are recycled
-            const int total = kc1 + kc3, n_wait = total < ATTN_STAGES ? total : ATTN_STAGES;
-            for (int i = 0; i < n_wait; ++i) {
-                mbar_wait(empty_bar(s), ph ^ 1u);
-                if (++s == ATTN_STAGES) { s = 0; ph ^= 1u; }
-            }
         }
     } else if (warp < ATTN_PRODUCER_WARP) {
         // ------------------------------------------------------------ warpgroup g: query rows [64 g, 64 g + 64) of the tile
@@ -187,19 +174,17 @@ __device__ __forceinline__ void attn_unit_t(const AttnParams& p, const AttnParam
             *reinterpret_cast<__nv_bfloat162*>(o) = __floats2bfloat162_rn(oacc[j] * inv[h], oacc[j + 1] * inv[h]);
         }
     }
-    if constexpr (MEGA) fence_proxy_async_all();      // the next unit's TMA loads overwrite shared memory this unit wrote generically
     __syncthreads();
 }
 
-template <bool MEGA>
 __device__ __forceinline__ void attn_unit(const AttnParams& p, const AttnParams* pm, const uint32_t base, uint8_t* base_ptr, const int qt,
                                           const int dc, const int z) {
     if (p.Lt == 256) {
-        if (p.dn == 256) attn_unit_t<256, 256, MEGA>(p, pm, base, base_ptr, qt, dc, z);
-        else attn_unit_t<256, 128, MEGA>(p, pm, base, base_ptr, qt, dc, z);
+        if (p.dn == 256) attn_unit_t<256, 256>(p, pm, base, base_ptr, qt, dc, z);
+        else attn_unit_t<256, 128>(p, pm, base, base_ptr, qt, dc, z);
     } else {
-        if (p.dn == 256) attn_unit_t<128, 256, MEGA>(p, pm, base, base_ptr, qt, dc, z);
-        else attn_unit_t<128, 128, MEGA>(p, pm, base, base_ptr, qt, dc, z);
+        if (p.dn == 256) attn_unit_t<128, 256>(p, pm, base, base_ptr, qt, dc, z);
+        else attn_unit_t<128, 128>(p, pm, base, base_ptr, qt, dc, z);
     }
 }
 
@@ -208,7 +193,7 @@ __global__ void __launch_bounds__(ATTN_THREADS, 1) attn_kernel(const __grid_cons
     const uint32_t raw = smem_u32(smem_raw);
     const uint32_t base = (raw + 1023u) & ~1023u;
     const int n_dc = p.C / p.dn;
-    attn_unit<false>(p, &p, base, smem_raw + (base - raw), blockIdx.x / n_dc, blockIdx.x % n_dc, blockIdx.y);
+    attn_unit(p, &p, base, smem_raw + (base - raw), blockIdx.x / n_dc, blockIdx.x % n_dc, blockIdx.y);
 }
 
 }  // namespace sr3

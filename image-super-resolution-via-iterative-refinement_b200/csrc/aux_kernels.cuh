@@ -62,7 +62,7 @@ struct PrepParams {
     float eps;
     __nv_bfloat16* out_a;                   // [B][HW][C0+C1]
     __nv_bfloat16* out_raw;                 // optional bf16(x), same shape
-    int B, items_per_image;                 // persistent step kernel: work items = B x items_per_image blocks of pix_per_block pixels
+    int B;                                  // images (the GroupNorm backward reads it)
     int precise;                            // 1: operands are (hi | lo) pairs -- out rows are 2 (C0+C1) wide, low halves C0+C1 elements behind
     const DropSpec* drop;                   // training-mode forward only: Dropout after the SiLU (unet.py:86); nullptr otherwise
     float* save_mr;                         // training-mode forward only: [B][groups][2] (mean, rstd) kept for the backward; nullptr otherwise
@@ -196,6 +196,7 @@ __global__ void __launch_bounds__(256) cast_kernel(const float* __restrict__ src
 // Row softmax over keys (torch.softmax(attn, -1), unet.py:136): S fp32 [rows][L] -> P bf16 [rows][L].
 // Rows are grouped in segments of `seg` tokens; a row only attends to the keys of its own segment (two 64-token images share
 // one 128-row attention batch); keys outside get probability 0.
+struct SoftmaxParams { const float* S; __nv_bfloat16* P; long long rows; int L, seg, precise; };
 __global__ void __launch_bounds__(256) softmax_kernel(const float* __restrict__ S, __nv_bfloat16* __restrict__ P, long long rows, int L,
                                                       int seg, int precise) {
     pdl_launch_dependents();

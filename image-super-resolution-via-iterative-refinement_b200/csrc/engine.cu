@@ -20,7 +20,6 @@
 #include "../../include/sr3_b200.h"
 #include "aux_kernels.cuh"
 #include "attn_wgmma.cuh"
-#include "step_megakernel.cuh"
 #include "train_kernels.cuh"
 
 using namespace sr3;
@@ -273,17 +272,6 @@ struct DevAllocs {
 
 typedef std::function<void(cudaStream_t)> Op;
 struct GemmHandle { std::shared_ptr<GemmParams> p; const void* w_ptr = nullptr; long long w_bytes = 0; bool w_is_param = false; int bn = 0, mh = 0; };
-// One op of the persistent step kernel (step_megakernel.cuh), recorded next to the per-layer launch it replaces.
-struct MegaRec { int type = 0, variant = 0; std::shared_ptr<GemmParams> gp; std::vector<uint8_t> raw; };
-static thread_local std::vector<MegaRec>* g_mega_registry = nullptr;
-template <typename T>
-void mega_record(int type, const T& params) {
-    if (!g_mega_registry) return;
-    MegaRec r; r.type = type;
-    r.raw.resize((sizeof(T) + 3) & ~size_t(3));
-    memcpy(r.raw.data(), &params, sizeof(T));
-    g_mega_registry->push_back(std::move(r));
-}
 static thread_local std::vector<GemmHandle>* g_gemm_registry = nullptr;   // set by the engine while it builds its plan
 // what the most recent sr3_test_conv_ex of this thread launched (sr3_tile_schedule with no engine)
 struct LastTestConv { sr3_gemm_geometry geo{}; int schedule = -1; int out_hwc[3] = {0, 0, 0}; };
@@ -380,7 +368,6 @@ Op make_gemm_op(const GemmDesc& d, DevAllocs& mem, sr3_gemm_geometry* geo = null
     p.resid = d.resid; p.rs = d.rs; p.out_f32 = d.out_f32; p.os = d.os; p.out_bf16 = d.out_bf16; p.hs = d.hs;
     p.out_t = d.out_t; p.t_col0 = d.t_col0; p.t_rows = d.t_rows; p.t_ld = d.t_ld; p.t_per = d.t_per > 0 ? d.t_per : 1;
     p.stats = d.stats; p.stats_C = d.stats_C; p.stats_coff = d.stats_coff; p.ctl = d.ctl; p.post = d.post;
-    p.t_fixed = -1;
     p.z_phase = d.z_phase; p.z_off_hi = d.z_off_hi; p.z_off_lo = d.z_off_lo;
     p.passes = d.passes; p.lo_b_col = d.lo_b_col; p.lo_a_chan[0] = d.lo_a_chan[0]; p.lo_a_chan[1] = d.lo_a_chan[1];
     p.lo_out_off = d.lo_out_off; p.lo_t_off = d.lo_t_off;
@@ -465,10 +452,6 @@ Op make_gemm_op(const GemmDesc& d, DevAllocs& mem, sr3_gemm_geometry* geo = null
         GemmHandle h; h.p = sp; h.w_ptr = d.b_ptr; h.w_bytes = 2LL * d.b_rows * d.b_K; h.w_is_param = d.b_is_param; h.bn = bn; h.mh = mh;
         g_gemm_registry->push_back(h);
     }
-    if (g_mega_registry) {
-        MegaRec r; r.type = MOP_GEMM; r.variant = bn | (mh << 16) | (pp ? MEGA_VARIANT_PP : 0); r.gp = sp;
-        g_mega_registry->push_back(std::move(r));
-    }
     return [sp, grid, bn, mh, pp, smem](cudaStream_t st) {
         const GemmParams& p = *sp;
         if (pp) {
@@ -512,7 +495,6 @@ Op make_attn_op(const bf16* qk, const bf16* vT, bf16* out, int nz, int Lt, int H
     static std::vector<int> seen;
     if (first_use_on_device(seen)) CK(cudaFuncSetAttribute(attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ATTN_SMEM_BYTES));
     const dim3 grid((Lt / 128) * (C / p.dn), nz, 1);
-    mega_record(MOP_ATTN, p);
     return [p, grid](cudaStream_t st) { launch_k(attn_kernel, grid, dim3(ATTN_THREADS), ATTN_SMEM_BYTES, st, p); };
 }
 
@@ -1215,11 +1197,6 @@ struct sr3_engine {
     StepCtl* ctl_dev = nullptr;
     StepCtl ctl{};
     double* stats_arena = nullptr; size_t stats_cap = 0, stats_used = 0;
-    // persistent step kernel (one cooperative launch per reverse step)
-    std::vector<MegaRec> mega;
-    bool use_mega = false;
-    MegaOp* mega_ops_dev = nullptr; uint8_t* mega_blob = nullptr; unsigned long long* mega_bar = nullptr; unsigned long long* mega_prof = nullptr;
-    std::vector<int> mega_types;
     bf16* in_buf = nullptr;
     float *x_state = nullptr, *eps_buf = nullptr, *mean_buf = nullptr, *noise_buf = nullptr, *nl_buf = nullptr, *io_a = nullptr, *io_b = nullptr;
     float *nl_table = nullptr, *post_tab = nullptr;
@@ -1362,20 +1339,8 @@ struct sr3_engine {
         if (train) { last_mr = static_cast<float*>(mem.alloc((size_t)Bp * groups * 2 * sizeof(float))); p.save_mr = last_mr; }
         p.out_a = out_a; p.out_raw = out_raw; p.precise = precise ? 1 : 0;
         const int C = p.C0 + p.C1;
-        const int vpp = C / 4;
         const RowLaunch L = prep_launch(C, groups, p.HW, B);
         p.pix_per_block = L.ppb;
-        {   // the same op inside the persistent step kernel: B x items_per_image work items dealt contiguously to the CTAs
-            PrepParams m = p;
-            const int nth = GEMM_THREADS;
-            const int kp = vpp > nth ? 1 : nth / vpp;
-            int ipi = (4 * num_sms() + B / 2) / B; if (ipi < 1) ipi = 1;
-            int mp = (p.HW + ipi - 1) / ipi;
-            mp = ((mp + kp - 1) / kp) * kp;
-            if (mp > p.HW) mp = p.HW;
-            m.pix_per_block = mp; m.items_per_image = (p.HW + mp - 1) / mp; m.B = B;
-            mega_record(MOP_PREP, m);
-        }
         push([p, L](cudaStream_t st) { launch_prep(p, L, st); }, 1, 0, (double)B * p.HW * C * (4.0 + 2.0 + (out_raw ? 2.0 : 0.0)));
     }
     void add_cast(const Act& s, bf16* dst, int up) {
@@ -1521,7 +1486,6 @@ struct sr3_engine {
             push_gemm(attn_s_desc(qk, S, nz, Lt, C, PW));
             const SoftmaxParams sp = attn_softmax_params(S, P, nz, Lt, HW, PW);
             push([=](cudaStream_t st) { launch_softmax(sp, st); }, 3, 0, (double)sp.rows * Lt * 6.0);
-            mega_record(MOP_SOFTMAX, sp);
             push_gemm(attn_pv_desc(P, vT, O, nz, Lt, C, PW));
         }
         {   // out projection + bias + residual (un-normalised input)
@@ -1608,8 +1572,6 @@ struct sr3_engine {
             float *fw = film_w, *fb = film_b, *fc = film_cb, *ta = tau, *fi = film; const int Fn = F, inn = inner;
             push([=](cudaStream_t st) { launch_film(fw, fb, fc, ta, fi, Fn, inn, Bn, st); });
             side_end = (int)ops.size();
-            EmbedFilmParams fp{}; fp.e = ep; fp.wf = film_w; fp.bf = film_b; fp.cbias = film_cb; fp.film = film; fp.F = F; fp.B = B;
-            mega_record(MOP_EMBED_FILM, fp);
         }
 
         int film_off = 0;
@@ -1710,10 +1672,6 @@ struct sr3_engine {
                 d.post.x_state = x_state; d.post.eps_out = eps_buf; d.post.mean_out = mean_buf; d.post.noise_buf = noise_buf;
                 d.post.in_buf = in_buf; d.post.in_C = in_C * PW; d.post.in_coff = cond_c; d.post.in_lo_off = precise ? in_C : 0;
                 push_gemm(d);
-                // the statistics arena is cleared for the NEXT step once nobody reads it any more (every GroupNorm apply has passed
-                // the grid barrier in front of the final conv)
-                ZeroParams zp{}; zp.ptr = reinterpret_cast<float4*>(stats_arena); zp.n4 = (long long)(stats_cap * sizeof(double) / 16);
-                mega_record(MOP_ZERO, zp);
             }
         }
     }
@@ -1771,10 +1729,8 @@ struct sr3_engine {
         // pass 2: real plan
         dry = false; stats_used = 0; zero_used = 0;
         g_gemm_registry = &gemms;
-        g_mega_registry = &mega;
-        try { build_plan(); } catch (...) { g_gemm_registry = nullptr; g_mega_registry = nullptr; throw; }
+        try { build_plan(); } catch (...) { g_gemm_registry = nullptr; throw; }
         g_gemm_registry = nullptr;
-        g_mega_registry = nullptr;
         if (!train) {
             // every tile kernel pulls the weights of the next one into L2 (the last one those of the next step's first)
             for (size_t i = 0; i < gemms.size(); ++i) {
@@ -1786,72 +1742,10 @@ struct sr3_engine {
             }
         }
         CK(cudaStreamCreateWithFlags(&cap_stream, cudaStreamNonBlocking));
-        build_mega();
         CK(cudaDeviceSynchronize());
     }
 
-    // ---- persistent step kernel: serialise the recorded ops (parameter blocks 128-byte aligned) and upload them
-    void build_mega() {
-        // Off by default: the grid barrier + per-op fill / drain cost about as much as a launch inside a CUDA graph, and the 288-thread
-        // GroupNorm apply has less bandwidth than the stand-alone kernel.
-        // SR3_MEGA=1 selects it (bit-identical results).
-        use_mega = !train && getenv("SR3_MEGA") != nullptr && atoi(getenv("SR3_MEGA")) != 0;
-        if (!use_mega) return;
-        {   // embed_film_body keeps tau of every image in the op region of shared memory (after the 1024-byte alignment and the header)
-            const long long need = embed_film_smem_bytes(B, inner, F, num_sms()), room = SMEM_LIMIT - 1024 - GEMM_HDR_BYTES;
-            REQUIRE(need <= room, "step kernel (SR3_MEGA=1): the noise embedding + FiLM op needs %lld bytes of shared memory at batch %d "
-                    "(inner_channel %d), its op region holds %lld; use a smaller batch or the per-layer path", need, B, inner, room);
-        }
-        std::vector<MegaOp> host_ops;
-        std::vector<uint8_t> blob;
-        for (size_t i = 0; i < mega.size(); ++i) {
-            MegaRec& r = mega[i];
-            MegaOp o{}; o.type = r.type; o.variant = r.variant;
-            const uint8_t* src = r.raw.data(); size_t n = r.raw.size();
-            if (r.type == MOP_GEMM) {
-                const int bn = r.variant & 0xffff, mh = (r.variant >> 16) & 0xff;
-                if (!((bn == 16 || bn == 32 || bn == 64 || bn == 128) && (mh == 1 || mh == 2) && !(bn == 32 && mh == 2))) { use_mega = false; return; }
-                src = reinterpret_cast<const uint8_t*>(r.gp.get()); n = sizeof(GemmParams);
-            }
-            REQUIRE(n % 4 == 0 && n <= (size_t)(GEMM_HDR_BYTES - HDR_PARAMS), "step kernel: parameter block of %zu bytes does not fit the header", n);
-            // ops 0 (embedding + FiLM + nothing upstream) and 1 (first conv: reads the input buffer of the previous launch) and the final
-            // clear need no barrier; every other op consumes what all CTAs of its predecessor produced
-            o.sync_before = (i >= 2 && r.type != MOP_ZERO) ? 1 : 0;
-            o.param_bytes = (int)n;
-            blob.resize((blob.size() + 127) & ~size_t(127));
-            o.param_off = (long long)blob.size();
-            blob.insert(blob.end(), src, src + n);
-            host_ops.push_back(o);
-            mega_types.push_back(r.type);
-        }
-        REQUIRE(host_ops.size() >= 3 && mega[0].type == MOP_EMBED_FILM && mega[1].type == MOP_GEMM, "step kernel: unexpected plan head");
-        mega_ops_dev = static_cast<MegaOp*>(mem.alloc(host_ops.size() * sizeof(MegaOp), false));
-        mega_blob = static_cast<uint8_t*>(mem.alloc(blob.size(), false));
-        mega_bar = static_cast<unsigned long long*>(mem.alloc(128));
-        mega_prof = static_cast<unsigned long long*>(mem.alloc((host_ops.size() + 1) * 4 * sizeof(unsigned long long)));
-        REQUIRE((reinterpret_cast<uintptr_t>(mega_blob) & 127) == 0, "blob not 128B aligned");
-        CK(cudaMemcpy(mega_ops_dev, host_ops.data(), host_ops.size() * sizeof(MegaOp), cudaMemcpyHostToDevice));
-        CK(cudaMemcpy(mega_blob, blob.data(), blob.size(), cudaMemcpyHostToDevice));
-        static std::vector<int> seen;
-        if (first_use_on_device(seen)) CK(cudaFuncSetAttribute(step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT));
-        int per_sm = 0;
-        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, step_kernel, GEMM_THREADS, SMEM_LIMIT));
-        REQUIRE(per_sm >= 1, "step kernel does not fit an SM");
-    }
-    void launch_mega(cudaStream_t st) {
-        MegaParams mp{};
-        mp.ops = mega_ops_dev; mp.n_ops = (int)mega_types.size(); mp.blob = mega_blob; mp.bar = mega_bar; mp.prof = mega_prof; mp.ctl = ctl_dev;
-        cudaLaunchConfig_t cfg{};
-        cfg.gridDim = dim3(num_sms()); cfg.blockDim = dim3(GEMM_THREADS); cfg.dynamicSmemBytes = SMEM_LIMIT; cfg.stream = st;
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeCooperative;            // all CTAs co-resident: the grid barriers (and split-K meets) cannot deadlock
-        attr[0].val.cooperative = 1;
-        cfg.attrs = attr; cfg.numAttrs = 1;
-        CK(cudaLaunchKernelEx(&cfg, step_kernel, mp));
-    }
-
     void run_step(cudaStream_t st) {
-        if (use_mega) { launch_mega(st); return; }
         if (!graph) {
             cudaGraph_t g;
             const bool fork = side_begin > 0 && side_end > side_begin && side_join >= side_end;
@@ -1909,7 +1803,7 @@ struct sr3_engine {
 extern "C" {
 
 const char* sr3_last_error(void) { return g_err.c_str(); }
-int sr3_abi_version(void) { return 3; }
+int sr3_abi_version(void) { return 4; }
 
 int sr3_engine_create_sized(const sr3_unet_config* cfg, int batch, int height, int width, int device, sr3_engine** out) {
     API_BEGIN
@@ -2317,40 +2211,10 @@ int sr3_engine_profile_step(sr3_engine* e, int t, int reps, int cap, int* kinds,
     }
     *n_ops = n;
     for (auto& x : ev) cudaEventDestroy(x);
-    // the per-layer path clears the statistics arena at the START of a step, the step kernel at the END of one: leave it clean
-    CK(cudaMemsetAsync(e->stats_arena, 0, e->stats_cap * sizeof(double), st));
-    CK(cudaStreamSynchronize(st));
     API_END
 }
 
-int sr3_engine_uses_step_kernel(const sr3_engine* e) { return (e && e->use_mega) ? 1 : 0; }
-
-// Per-op device time of the most recent step-kernel launch (globaltimer stamps taken by CTA 0 after each grid barrier).
-int sr3_engine_step_kernel_profile(sr3_engine* e, int cap, int* types, double* us, double* phases, int* n_ops, void* stream) {
-    API_BEGIN
-    REQUIRE(e && types && us && n_ops, "null argument");
-    REQUIRE(e->use_mega, "this engine runs the per-layer path (set SR3_MEGA=1 for the step kernel), there is nothing to profile here");
-    const int n = (int)e->mega_types.size();
-    REQUIRE(cap >= n, "profile buffers too small (%d ops)", n);
-    CK(cudaSetDevice(e->dev));
-    CK(cudaStreamSynchronize(static_cast<cudaStream_t>(stream)));
-    std::vector<unsigned long long> ts((size_t)(n + 1) * 4);
-    CK(cudaMemcpy(ts.data(), e->mega_prof, ts.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-    for (int i = 0; i < n; ++i) {
-        types[i] = e->mega_types[i];
-        us[i] = (double)(ts[4 * (i + 1)] - ts[4 * i]) * 1e-3;
-        if (phases) {      // [set-up (arrive + parameter / stage-table copy), barrier wait, body, end-of-op fence]
-            phases[4 * i + 0] = (double)(ts[4 * i + 1] - ts[4 * i]) * 1e-3;
-            phases[4 * i + 1] = (double)(ts[4 * i + 2] - ts[4 * i + 1]) * 1e-3;
-            phases[4 * i + 2] = (double)(ts[4 * i + 3] - ts[4 * i + 2]) * 1e-3;
-            phases[4 * i + 3] = (double)(ts[4 * (i + 1)] - ts[4 * i + 3]) * 1e-3;
-        }
-    }
-    *n_ops = n;
-    API_END
-}
-
-int sr3_engine_num_launches_per_step(const sr3_engine* e) { return e ? (e->use_mega ? 1 : (int)e->ops.size()) : 0; }
+int sr3_engine_num_launches_per_step(const sr3_engine* e) { return e ? (int)e->ops.size() : 0; }
 int sr3_engine_num_ops_per_step(const sr3_engine* e) { return e ? (int)e->ops.size() : 0; }
 int64_t sr3_engine_workspace_bytes(const sr3_engine* e) { return e ? e->mem.bytes : 0; }
 

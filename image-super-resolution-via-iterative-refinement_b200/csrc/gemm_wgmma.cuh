@@ -137,7 +137,6 @@ struct GemmParams {
     // bf16 outputs go lo_out_off elements (lo_t_off for the transposed store) behind the high halves.  passes = 1: plain bf16.
     int passes, lo_b_col, lo_a_chan[2];
     long long lo_out_off, lo_t_off;
-    int t_fixed;             // >= 0: timestep of the running step (persistent step kernel: ctl->t_cur is not used there); -1: read ctl->t_cur
 };
 
 constexpr int GEMM_THREADS = 288;           // warps 0..7: two consumer warpgroups (MMA + epilogue), warp 8: TMA producer
@@ -148,12 +147,9 @@ constexpr int GEMM_MAX_STAGES = 8;
 __host__ __device__ constexpr int gemm_epi_warp_bytes(bool resid) { return resid ? 12288 : 4096; }
 __host__ __device__ constexpr int gemm_epi_bytes(bool resid) { return GEMM_EPI_WARPS * gemm_epi_warp_bytes(resid); }
 constexpr int GEMM_MAX_K = 160;              // stages per tile (<= 3 K slabs each); the table is sized per launch
-// Shared-memory header (first 2 KB of the 1024-aligned region, same place for every op of the persistent step kernel):
-//   [0, 512) mbarriers | [520, 528) step scalars | [768, 2048) parameter block of the running op
+// Shared-memory header (first 2 KB of the 1024-aligned region): the mbarriers, in [0, 512).  They need less than 2 KB, but the size
+// enters gemm_aux_bytes and so the stage counts the planner picks: shrinking it changes plans, and with them results and speed.
 constexpr int GEMM_HDR_BYTES = 2048;
-constexpr int HDR_SCALARS = 512;
-constexpr int HDR_PARAMS = 768;
-constexpr int HDR_NUM_BARS = 64;
 // Tiles of at most 32 columns (MH = 1) are computed by warpgroup 0 alone; every other tile is shared by both consumer warpgroups.
 __host__ __device__ constexpr bool gemm_single_wg(int block_n, int mh) { return mh == 1 && block_n <= 32; }
 // Ping-pong schedule: each consumer warpgroup owns whole tiles (local tiles g, g + 2, ... of the CTA's range), their MMA phases take
@@ -229,7 +225,7 @@ __device__ __forceinline__ void final_epilogue(const GemmParams& p, const float 
         for (int c = 0; c < q.C; ++c) q.eps_out[(static_cast<long long>(img) * q.C + c) * plane + pix] = eps[c];
         return;
     }
-    const int t = p.t_fixed >= 0 ? p.t_fixed : ctl.t_cur;
+    const int t = ctl.t_cur;
     const float c1 = q.tab[t], c2 = q.tab[q.T + t], pc1 = q.tab[2 * q.T + t], pc2 = q.tab[3 * q.T + t];
     const float sigma = (t > 0) ? expf(0.5f * q.tab[4 * q.T + t]) : 0.0f;
     float z[4] = {0.f, 0.f, 0.f, 0.f};
@@ -262,13 +258,10 @@ __device__ __forceinline__ void final_epilogue(const GemmParams& p, const float 
     }
 }
 
-static_assert(sizeof(GemmParams) <= GEMM_HDR_BYTES - HDR_PARAMS, "GemmParams must fit the shared-memory header");
-
-// CTA-local set-up of one tile-kernel op: stage table -> shared memory, TMA descriptor prefetch, mbarrier (re-)initialisation.  Nothing here
-// depends on data produced by other CTAs, so the persistent step kernel runs it BEFORE waiting at the grid barrier in front of the op.
+// CTA-local set-up of one tile-kernel launch: stage table -> shared memory, TMA descriptor prefetch, mbarrier initialisation.
 // Must be followed by a block-wide barrier.
 __device__ __forceinline__ void gemm_stage_setup(const GemmParams& p, const GemmParams* pm, const uint32_t base, uint8_t* base_ptr, const int block_n,
-                                                 const int mh, const bool pp, const bool recycle) {
+                                                 const int mh, const bool pp) {
     const int stages = p.stages;
     const int stage_bytes = p.a_stage_bytes + p.b_taps * block_n * 128;
     const bool use_res_tma = p.tma_epi && p.resid != nullptr && p.ksplit <= 1;
@@ -285,9 +278,6 @@ __device__ __forceinline__ void gemm_stage_setup(const GemmParams& p, const Gemm
         tma_prefetch_desc(&pm->b_map);
         if (p.tma_epi) { tma_prefetch_desc(&pm->out_map); tma_prefetch_desc(&pm->res_map); }
         const uint32_t bar_base = base;
-        if (recycle) {                           // the previous op's barriers (all quiescent: see the end of gemm_tile_body) are recycled
-            for (int i = 0; i < HDR_NUM_BARS; ++i) mbar_inval(bar_base + 8u * i);
-        }
         const uint32_t consumers = gemm_stage_readers(block_n, mh, pp);
         for (int s = 0; s < stages; ++s) {
             mbar_init(bar_base + 8u * s, 1);                                     // full
@@ -369,16 +359,13 @@ struct StatRun {
     }
 };
 
-// Persistent, warp-specialised tile loop (see the file header).  Two callers:
-//   MEGA = false: gemm_tile_kernel, one launch per layer; `p` lives in the kernel parameter space, barriers are set up here.
-//   MEGA = true : step_kernel (step_megakernel.cuh), the whole reverse step in ONE cooperative launch; `p` is the shared-memory copy
-//                 of the op's parameter block, `pm` its global-memory original (TMA descriptors must not live in shared memory),
-//                 `cta / ncta` replace blockIdx / gridDim.
-// `base` / `base_ptr`: 1024-aligned start of the CTA's dynamic shared memory (header first).
+// Persistent, warp-specialised tile loop of gemm_tile_kernel (see the file header).  `p` lives in the kernel parameter space and `pm`
+// points at it (TMA descriptors are addressed through it).  `base` / `base_ptr`: 1024-aligned start of the CTA's dynamic shared memory
+// (header first).
 // PP = false: cooperative schedule, both warpgroups share every tile.  PP = true: ping-pong schedule (gemm_pingpong_ok shapes, no split-K):
 // warpgroup g owns the CTA's local tiles g, g + 2, ... with an accumulator of the whole tile, and the warpgroups issue their MMAs in
 // turn (order barrier GEMM_ORDER_BAR + g), so the stage ring is consumed strictly in order, one warpgroup per stage.
-template <int BLOCK_N, int MH, bool MEGA, bool PP = false>
+template <int BLOCK_N, int MH, bool PP = false>
 __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmParams* pm, const uint32_t base, uint8_t* base_ptr,
                                                const int cta, const int ncta) {
     static_assert(!PP || gemm_pingpong_ok(BLOCK_N, MH), "ping-pong tile shape");
@@ -417,10 +404,8 @@ __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmPa
     const int ksplit = p.ksplit > 1 ? p.ksplit : 1;
     const int total_tiles = tiles_m * p.n_tiles * p.nz * ksplit;      // split index fastest: the CTAs of one output tile run together
     const int num_kt = p.num_k * (p.passes > 1 ? p.passes : 1);       // stages per tile (precise mode: three passes over the table)
-    if constexpr (!MEGA) {
-        gemm_stage_setup(p, pm, base, base_ptr, BLOCK_N, MH, PP, false);  // (the step kernel did this before its grid barrier)
-        __syncthreads();
-    }
+    gemm_stage_setup(p, pm, base, base_ptr, BLOCK_N, MH, PP);
+    __syncthreads();
     if (warp == 2 && lane == 0 && p.pf_bytes > 0) {                   // L2 prefetch of this CTA's slice of the next layer's weights
         long long chunk = ((p.pf_bytes + ncta - 1) / ncta + 15) & ~15ll;
         const long long off = chunk * cta;
@@ -433,10 +418,8 @@ __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmPa
             }
         }
     }
-    if constexpr (!MEGA) {
-        pdl_launch_dependents();  // the next kernel may be scheduled onto SMs as our CTAs retire ...
-        pdl_wait();               // ... and we touch upstream activations / statistics only after the previous kernel completed
-    }
+    pdl_launch_dependents();  // the next kernel may be scheduled onto SMs as our CTAs retire ...
+    pdl_wait();               // ... and we touch upstream activations / statistics only after the previous kernel completed
 
     auto decode = [&](int tile_s, int& w0, int& h0, int& b0, int& n0, int& z) {
         const int tile = tile_s / ksplit;
@@ -480,20 +463,6 @@ __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmPa
                         tma_load_2d(a_dst + p.a_stage_bytes + t * B_BYTES, &pm->b_map, full_bar(s), e.tap[t].b_col + b_lo, brow);
                 }
                 __syncwarp();
-                if (++s == stages) { s = 0; ph ^= 1u; }
-            }
-        }
-        if constexpr (MEGA) {
-            // tail: every stage this CTA filled has been released by the consumers -> no arrival is in flight when the barriers are
-            // recycled by the next op
-            int filled = 0;
-            for (int tile = tile_begin; tile < tile_end; ++tile) {
-                const int sp = tile % ksplit;
-                filled += (num_kt * (sp + 1)) / ksplit - (num_kt * sp) / ksplit;
-            }
-            const int n_wait = filled < stages ? filled : stages;
-            for (int i = 0; i < n_wait; ++i) {
-                mbar_wait(empty_bar(s), ph ^ 1u);
                 if (++s == stages) { s = 0; ph ^= 1u; }
             }
         }
@@ -556,7 +525,7 @@ __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmPa
                 const int n = n0 + ch * 32 + lane;
                 if (n < p.n_valid) {
                     if (p.bias) bv += __ldg(&p.bias[n]);
-                    if (p.bias2) bv += __ldcg(&p.bias2[static_cast<long long>(img < p.OB ? img : 0) * p.bias2_stride + n]);   // written earlier in the same launch (step kernel): L2 only
+                    if (p.bias2) bv += __ldcg(&p.bias2[static_cast<long long>(img < p.OB ? img : 0) * p.bias2_stride + n]);   // written by this step's FiLM kernel: L2 only
                 }
                 return bv;
             };
@@ -918,13 +887,7 @@ __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmPa
             }       // pass
         }           // tiles
         if (p.stats) st_own.flush(p, ch0, lane);
-        if constexpr (MEGA) {
-            // the consumer is a later op of the SAME launch (other CTAs, after a grid barrier): the bulk stores must be complete in
-            // global memory, not merely done reading shared memory
-            if (use_out_tma && out_pending && lane == 0) tma_store_wait_all<0>();
-        } else {
-            if (use_out_tma && out_pending && lane == 0) tma_store_wait_read<0>();     // smem must outlive the reads of the last bulk stores
-        }
+        if (use_out_tma && out_pending && lane == 0) tma_store_wait_read<0>();     // smem must outlive the reads of the last bulk stores
     }
 }
 
@@ -933,7 +896,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tile_kernel(const __grid
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw = smem_u32(smem_raw);
     const uint32_t base = (raw + 1023u) & ~1023u;
-    gemm_tile_body<BLOCK_N, MH, false, PP>(p, &p, base, smem_raw + (base - raw), blockIdx.x, gridDim.x);
+    gemm_tile_body<BLOCK_N, MH, PP>(p, &p, base, smem_raw + (base - raw), blockIdx.x, gridDim.x);
 }
 
 }  // namespace sr3

@@ -35,8 +35,8 @@ __device__ __forceinline__ uint64_t globaltimer_ns() {
     return t;
 }
 
-// fp64 reduction on a GLOBAL address (no return value).  Spelled in PTX because the pointer may come out of a parameter block that
-// lives in shared memory (persistent step kernel): the compiler would otherwise emit a generic-address atomic with a CAS fallback.
+// fp64 reduction on a GLOBAL address (no return value), spelled in PTX so that it is one red.global.add.f64 whatever the compiler
+// can prove about the pointer.
 __device__ __forceinline__ void red_add_f64_global(double* p, double v) {
     asm volatile("red.global.add.f64 [%0], %1;" ::"l"(__cvta_generic_to_global(p)), "d"(v) : "memory");
 }
@@ -67,26 +67,9 @@ __device__ __forceinline__ void mbar_arrive_if(uint32_t bar, bool pred) {
         "r"(static_cast<uint32_t>(pred))
         : "memory");
 }
-__device__ __forceinline__ void mbar_inval(uint32_t bar) {
-    asm volatile("mbarrier.inval.shared::cta.b64 [%0];" ::"r"(bar) : "memory");
-}
 // add to the pending transaction count WITHOUT arriving (the arrival comes later with its own byte count)
 __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
     asm volatile("mbarrier.expect_tx.relaxed.cta.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-// generic <-> async proxy ordering for ALL state spaces (global data written with st.global and then read by TMA, and back)
-__device__ __forceinline__ void fence_proxy_async_all() { asm volatile("fence.proxy.async;" ::: "memory"); }
-
-// ------------------------------------------------------------------ grid-wide barrier (persistent step kernel)
-// All CTAs of a cooperative launch are co-resident.  The counter only ever grows: a launch starts with it at a multiple of the
-// grid size, barrier k of the launch completes when it reaches base + k * grid.
-__device__ __forceinline__ unsigned long long ld_acquire_gpu_u64(const unsigned long long* p) {
-    unsigned long long v;
-    asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
-    return v;
-}
-__device__ __forceinline__ void red_release_gpu_add_u64(unsigned long long* p, unsigned long long v) {
-    asm volatile("red.release.gpu.global.add.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
 }
 
 // Bounded wait: a pipeline bug must trap (-> a CUDA error the host reports) instead of hanging the GPU.  The MMA warpgroups wait here
@@ -139,10 +122,6 @@ __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk
 template <int N>
 __device__ __forceinline__ void tma_store_wait_read() {
     asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
-}
-template <int N>
-__device__ __forceinline__ void tma_store_wait_all() {
-    asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
 }
 
 // ------------------------------------------------------------------ wgmma (Hopper warpgroup MMA)

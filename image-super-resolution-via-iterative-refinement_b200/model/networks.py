@@ -39,7 +39,7 @@ def define_G(opt):
         init_weights(netG, init_type="orthogonal")
     if opt["gpu_ids"] and opt["distributed"]:
         # The reference wraps the net in nn.DataParallel here (networks.py:113-115).  DataParallel replicates nn.Modules per forward
-        # call; a module that owns native engines (packed weights, TMA descriptors, a persistent step kernel) cannot be replicated that
+        # call; a module that owns native engines (packed weights, TMA descriptors, a captured step graph) cannot be replicated that
         # way.  The multi-GPU path of this implementation is one process per GPU: sr3_b200.parallel (batch-sharded sampling over NCCL).
         raise NotImplementedError(
             "sr3_b200.define_G: opt['distributed']=True (nn.DataParallel) is not supported; run one process per GPU "

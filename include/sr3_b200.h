@@ -53,8 +53,8 @@ int sr3_abi_version(void);
  * The lowest UNet level (image_size / 2^(n_mults - 1)) must be at least 4x4; a net with a 4x4 level allocates its activations for the batch
  * rounded up to 8 images, but launches the work of the real images only.
  * Threading: calls on one engine must be serialised by the caller.  Kernels whose CTAs wait for partners are safe next to other work on the
- * device: the split-K partners of a tile are one thread-block cluster (gang-scheduled by the hardware), the persistent step kernel (SR3_MEGA=1)
- * is a cooperative launch -- engines driven concurrently from different streams of one device cannot deadlock each other. */
+ * device: the split-K partners of a tile are one thread-block cluster (gang-scheduled by the hardware) -- engines driven concurrently from
+ * different streams of one device cannot deadlock each other. */
 int sr3_engine_create(const sr3_unet_config* cfg, int batch, int device, sr3_engine** out);
 /* The same inference plan for images of height x width instead of image_size x image_size: the reference UNet is fully convolutional and
  * runs whatever size it is given (unet.py:235-259; p_sample_loop takes its shape from x_in, diffusion.py:188-200).  cfg->image_size still
@@ -193,16 +193,8 @@ int sr3_resize_bicubic_u8(const unsigned char* src_u8, unsigned char* dst_u8, fl
                           float min_v, float max_v, void* stream);
 
 /* Introspection for tests / bench. */
-int sr3_engine_num_launches_per_step(const sr3_engine* e);   /* kernel launches per reverse step: 1 with the persistent step kernel */
-int sr3_engine_num_ops_per_step(const sr3_engine* e);        /* launches of the per-layer path (the default; also what sr3_engine_profile_step times) */
-/* 1 when one reverse step (reference p_sample: diffusion.py:151-174, UNet.forward unet.py:235-259) runs as ONE persistent
- * cooperative launch (csrc/step_megakernel.cuh), 0 when it runs as a CUDA graph of per-layer launches (the default; SR3_MEGA=1 selects the step kernel). */
-int sr3_engine_uses_step_kernel(const sr3_engine* e);
-/* Per-op device time (us) of the most recent step-kernel launch: globaltimer stamps taken by CTA 0 after each grid barrier.
- * types: 0 tensor-core tile loop, 1 GroupNorm apply, 2 fused attention, 3 row softmax, 4 embedding + FiLM, 5 statistics clear. */
-int sr3_engine_step_kernel_profile(sr3_engine* e, int cap, int* types, double* us, double* phases_or_null, int* n_ops, void* stream);
-/* phases (optional, [cap][4] us): per op, time CTA 0 spent in set-up (barrier arrive + parameter / stage-table copy), waiting at the grid
- * barrier, in the op body, and in the end-of-op fence. */
+int sr3_engine_num_launches_per_step(const sr3_engine* e);   /* kernel launches per reverse step (the nodes of the captured step graph) */
+int sr3_engine_num_ops_per_step(const sr3_engine* e);        /* ops of the step plan, one launch each (what sr3_engine_profile_step times) */
 int64_t sr3_engine_workspace_bytes(const sr3_engine* e);
 /* Per-kernel timing of one eager (non-graph) reverse step at timestep t, averaged over `reps` repetitions after one warm-up,
  * CUDA events on `stream` around every launch.  kinds: 0 tensor-core tile kernel, 1 GroupNorm apply, 2 cast/upsample,

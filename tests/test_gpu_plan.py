@@ -12,7 +12,7 @@ import test_gpu_unet as tu
 
 pytestmark = pytest.mark.gpu
 
-KNOBS = ("SR3_TALL_BN", "SR3_TALL_MH", "SR3_BLOCK_N", "SR3_KSPLIT", "SR3_STAGES", "SR3_PINGPONG", "SR3_MEGA", "SR3_MAX_CTAS")
+KNOBS = ("SR3_TALL_BN", "SR3_TALL_MH", "SR3_BLOCK_N", "SR3_KSPLIT", "SR3_STAGES", "SR3_PINGPONG", "SR3_MAX_CTAS")
 
 # (op index of the eager step, output (H, W, C), tall halo, tile rows, BLOCK_N, schedule, split-K factor)
 PLAN_16_128_B16 = [

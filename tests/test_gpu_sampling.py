@@ -13,12 +13,12 @@ from oracle import sr3_oracle as orc
 
 pytestmark = pytest.mark.gpu
 
-KNOBS = ("SR3_TALL_BN", "SR3_TALL_MH", "SR3_BLOCK_N", "SR3_KSPLIT", "SR3_STAGES", "SR3_PINGPONG", "SR3_MEGA", "SR3_MAX_CTAS")
+KNOBS = ("SR3_TALL_BN", "SR3_TALL_MH", "SR3_BLOCK_N", "SR3_KSPLIT", "SR3_STAGES", "SR3_PINGPONG", "SR3_MAX_CTAS")
 SEED = 2 ** 62 + 0x1234_5678_9ABC          # both key words set
 FIRST = 2 ** 32 - 2                        # batch 3: sample indices 2^32 - 2, 2^32 - 1, 2^32 (the high word of the index changes)
 B = 3
-SIZES = [(32, 32), (32, 64)]
-MODES = ["graph", "mega"]
+SIZES = [(32, 32), (32, 64), (64, 32), (64, 64)]
+MODES = ["graph"]
 PRECISIONS = ["bf16", "fp32"]
 
 
@@ -29,12 +29,10 @@ def make_opt(unet, image_size, sched):
                       "diffusion": {"image_size": image_size, "channels": 3, "conditional": True}}}
 
 
-def build(monkeypatch, mode, precision, sched, unet=si.TINY, image_size=32, seed=0):
+def build(monkeypatch, precision, sched, unet=si.TINY, image_size=32, seed=0):
     import sr3_b200
     for k in KNOBS:
         monkeypatch.delenv(k, raising=False)
-    if mode == "mega":
-        monkeypatch.setenv("SR3_MEGA", "1")
     torch.manual_seed(seed)
     net = sr3_b200.define_G(make_opt(dict(unet, precision=precision), image_size, sched)).cuda()
     net.set_new_noise_schedule(sched, "cuda")
@@ -47,23 +45,17 @@ def data(h, w, seed):
     return torch.rand(B, 3, h, w, generator=g) * 2 - 1, torch.randn(B, 3, h, w, generator=g)
 
 
-def engine(net, h, w, mode):
-    eng = net._engine(B, h, w)
-    assert eng.uses_step_kernel() == (mode == "mega")
-    return eng
-
-
 @pytest.mark.parametrize("mode", MODES)
 @pytest.mark.parametrize("precision", PRECISIONS)
 @pytest.mark.parametrize("h,w", SIZES)
 def test_posterior_mean_bit_for_bit(monkeypatch, h, w, precision, mode):
     """predict_start_from_noise, clamp and q_posterior in torch-CPU fp32 on the eps unet_forward returns at the step's noise level equal the
     device's p_mean_variance mean bit for bit: the epilogue rounds every product and sum separately, as torch does."""
-    net = build(monkeypatch, mode, precision, si.SCHED)
+    net = build(monkeypatch, precision, si.SCHED)
     sch = orc.make_schedule(si.SCHED)
     T = sch.num_timesteps
     cond, x_t = data(h, w, h + w)
-    eng = engine(net, h, w, mode)
+    eng = net._engine(B, h, w)
     for t in (T - 1, T // 2, 1, 0):
         eps = eng.unet_forward(torch.cat([cond, x_t], 1), orc.noise_level_for_t(sch, t, B)).cpu()
         for clip in (True, False):
@@ -91,11 +83,11 @@ def test_seeded_noise_is_the_documented_stream(monkeypatch, h, w, precision, mod
     """p_sample(seed, first_index) = mean + sampling_noise(...) exp(0.5 logvar) within the ulp bound of the device's logf / sincospif / expf,
     with a seed >= 2^62 and a batch that crosses the sample index's high-word boundary.  The bound is tight: the restatement with any
     counter word off by one, or with the seed's words swapped, misses it by orders of magnitude.  At t = 0 x is the mean, bit for bit."""
-    net = build(monkeypatch, mode, precision, si.SCHED)
+    net = build(monkeypatch, precision, si.SCHED)
     sch = orc.make_schedule(si.SCHED)
     T = sch.num_timesteps
     cond, x_t = data(h, w, 7 * h + w)
-    eng = engine(net, h, w, mode)
+    eng = net._engine(B, h, w)
     idx = FIRST + np.arange(B, dtype=np.uint64)
     wrong = {f"counter word {i} + 1": (lambda i: lambda *w: tuple(x + np.uint64(1) if j == i else x for j, x in enumerate(w)))(i)
              for i in range(4)}
@@ -123,9 +115,9 @@ def test_loop_is_its_steps(monkeypatch, h, w, precision, mode):
     """p_sample_loop(seed, first_index) over a 10-step schedule equals p_sample(seed, first_index) chained from x_T, bit for bit at every
     snapshot: the loop hands x_{t-1} (and in precise mode its low half) to the next step's input exactly as a fresh load does, and keys
     the noise with the step's own t."""
-    net = build(monkeypatch, mode, precision, si.SCHED10)
+    net = build(monkeypatch, precision, si.SCHED10)
     cond, x_T = data(h, w, 11 * h + w)
-    eng = engine(net, h, w, mode)
+    eng = net._engine(B, h, w)
     final, snaps = eng.p_sample_loop(cond, x_T, None, SEED, FIRST, want_snapshots=True)
     assert snaps.shape[0] == 10
     x = x_T.cuda()
@@ -184,35 +176,23 @@ def test_embedding_and_film_forward_match_fp64(batch, inner):
 @pytest.mark.parametrize("inner,batch", [(128, 32), (64, 128)])
 def test_film_at_large_batch(monkeypatch, inner, batch):
     """A batch whose embeddings do not fit film_kernel's shared memory at once (inner_channel 128 at 32 images, 64 at 128) runs: eps
-    matches the same images through a batch-2 engine within the bf16 tolerance, and the step kernel gives the per-layer path's bits."""
+    matches the same images through a batch-2 engine within the bf16 tolerance."""
     unet = dict(in_channel=6, out_channel=3, inner_channel=inner, channel_multiplier=[1, 2], attn_res=[8], res_blocks=1, dropout=0.0)
     g = torch.Generator().manual_seed(inner + batch)
     x = torch.randn(batch, 6, 16, 16, generator=g)
     nl = torch.rand(batch, 1, generator=g)
-    eps = {}
-    for mode in MODES:
-        net = build(monkeypatch, mode, "bf16", si.SCHED10, unet=unet, image_size=16)
-        eps[mode] = net.denoise_fn(x.cuda(), nl.cuda()).cpu()
-        if mode == "graph":
-            pairs = torch.cat([net.denoise_fn(x[i:i + 2].cuda(), nl[i:i + 2].cuda()).cpu() for i in range(0, batch, 2)])
-        del net
-    for k in KNOBS:
-        monkeypatch.delenv(k, raising=False)
-    e = ((eps["graph"] - pairs).norm() / pairs.norm()).item()
+    net = build(monkeypatch, "bf16", si.SCHED10, unet=unet, image_size=16)
+    eps = net.denoise_fn(x.cuda(), nl.cuda()).cpu()
+    pairs = torch.cat([net.denoise_fn(x[i:i + 2].cuda(), nl[i:i + 2].cuda()).cpu() for i in range(0, batch, 2)])
+    e = ((eps - pairs).norm() / pairs.norm()).item()
     print(f"inner {inner} batch {batch}: eps vs batch-2 engines rel L2 {e:.2e} (bound 1e-2)")
-    assert torch.isfinite(eps["graph"]).all()
+    assert torch.isfinite(eps).all()
     assert e < 1e-2, e
-    assert torch.equal(eps["mega"], eps["graph"])
 
 
-def test_step_kernel_refuses_a_batch_beyond_its_shared_memory(monkeypatch):
-    """The step kernel's embedding + FiLM op keeps every image's embedding in shared memory: at inner_channel 128 a batch of 448 needs more
-    than its op region holds, and building that plan fails with a message before anything is launched; the per-layer path runs it."""
+def test_per_layer_path_runs_a_batch_of_448(monkeypatch):
+    """At inner_channel 128 a batch of 448, far beyond one chunk of film_kernel's tau staging (31 images), builds and runs: eps is finite."""
     unet = dict(in_channel=6, out_channel=3, inner_channel=128, channel_multiplier=[1, 2], attn_res=[8], res_blocks=1, dropout=0.0)
     x, nl = torch.zeros(448, 6, 16, 16).cuda(), torch.full((448, 1), 0.5).cuda()
-    net = build(monkeypatch, "mega", "bf16", si.SCHED10, unet=unet, image_size=16)
-    with pytest.raises(RuntimeError, match="op region holds"):
-        net.denoise_fn(x, nl)
-    del net
-    net = build(monkeypatch, "graph", "bf16", si.SCHED10, unet=unet, image_size=16)
+    net = build(monkeypatch, "bf16", si.SCHED10, unet=unet, image_size=16)
     assert torch.isfinite(net.denoise_fn(x, nl)).all()

@@ -273,32 +273,32 @@ def test_sharded_super_resolution_single_rank(golden):
     assert a.shape == (2, 3, 32, 32) and rel(a, b) < BF16_TOL
 
 
-@pytest.mark.parametrize("batch", [2, 3])
-def test_step_kernel_matches_per_layer_path_bit_for_bit(golden, batch, monkeypatch):
-    """One reverse step as ONE persistent cooperative launch (csrc/step_megakernel.cuh) against the same plan run as a CUDA graph of
-    per-layer launches (the default; SR3_MEGA=1 selects the step kernel): identical arithmetic, identical bits -- for eps and for a seeded 10-step loop."""
+def check_two_engines_agree(golden, batch):
+    """Two engines built from the same weights give the same bits for eps and for a seeded 10-step loop, and run a step as one launch
+    per op of the plan.  Returns the tile schedules of the plan."""
     g = golden["tiny_diffusion"]
-    c = g["cond"][:batch] if batch <= g["cond"].shape[0] else torch.cat([g["cond"], g["cond"][:1]], 0)
-    xT = g["x_T"][:batch] if batch <= g["x_T"].shape[0] else torch.cat([g["x_T"], g["x_T"][:1]], 0)
-    outs = {}
-    for mode in ("mega", "layers"):
-        if mode == "mega":
-            monkeypatch.setenv("SR3_MEGA", "1")
-        else:
-            monkeypatch.delenv("SR3_MEGA", raising=False)
+    reps = (batch + g["cond"].shape[0] - 1) // g["cond"].shape[0]
+    c, xT = g["cond"].repeat(reps, 1, 1, 1)[:batch], g["x_T"].repeat(reps, 1, 1, 1)[:batch]
+    outs = []
+    for _ in range(2):
         net = build(TINY_UNET, 32, 0, sched=g["sched"])
         eng = net.denoise_fn.engine(batch)
-        assert eng.uses_step_kernel() == (mode == "mega")
-        assert eng.launches_per_step() == (1 if mode == "mega" else eng.ops_per_step())
+        assert eng.launches_per_step() == eng.ops_per_step()
+        schedules = eng.tile_schedules()
         x = torch.cat([c, xT], 1).cuda()
         nl = torch.linspace(0.2, 0.9, batch).view(-1, 1).cuda()
         eps = net.denoise_fn(x, nl)
         loop = net.super_resolution(c.cuda(), continous=True, x_T=xT.cuda(), seed=5)
-        outs[mode] = (eps.cpu(), loop.cpu())
+        outs.append((eps.cpu(), loop.cpu()))
         del eng, net
-    monkeypatch.delenv("SR3_MEGA", raising=False)
-    assert torch.equal(outs["mega"][0], outs["layers"][0])
-    assert torch.equal(outs["mega"][1], outs["layers"][1])
+    assert torch.equal(outs[0][0], outs[1][0])
+    assert torch.equal(outs[0][1], outs[1][1])
+    return schedules
+
+
+@pytest.mark.parametrize("batch", [2, 3])
+def test_per_layer_path_is_bit_reproducible(golden, batch):
+    check_two_engines_agree(golden, batch)
 
 
 @pytest.mark.timeout(900)

@@ -36,7 +36,7 @@ def test_library_exports_every_header_symbol():
     for name in sorted(declared):
         assert hasattr(lib, name), f"{name} declared in sr3_b200.h but not exported by the library"
     assert declared == set(_native.EXPORTED_SYMBOLS), declared ^ set(_native.EXPORTED_SYMBOLS)
-    assert _native.lib().sr3_abi_version() == 3          # v3: training entry points (sr3_engine_create_train, sr3_train_*, sr3_adam_step)
+    assert _native.lib().sr3_abi_version() == 4          # v4: the step-kernel entry points are gone
 
 
 def test_state_dict_layout_matches_reference_names_and_init():
