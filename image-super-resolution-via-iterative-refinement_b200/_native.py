@@ -54,6 +54,7 @@ _SIGS = {
     "sr3_engine_create": (c_int, [POINTER(UNetConfigC), c_int, c_int, POINTER(c_void_p)]),
     "sr3_engine_create_sized": (c_int, [POINTER(UNetConfigC), c_int, c_int, c_int, c_int, POINTER(c_void_p)]),
     "sr3_engine_create_train": (c_int, [POINTER(UNetConfigC), c_int, c_int, c_float, POINTER(c_void_p)]),
+    "sr3_engine_create_train_sized": (c_int, [POINTER(UNetConfigC), c_int, c_int, c_int, c_int, c_float, POINTER(c_void_p)]),
     "sr3_train_forward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_uint64, POINTER(c_double), c_void_p]),
     "sr3_train_backward": (c_int, [c_void_p, c_float, POINTER(c_void_p), c_int, c_void_p]),
     "sr3_train_num_backward_blocks": (c_int, [c_void_p]),
@@ -190,8 +191,8 @@ class Engine:
 
     def __init__(self, cfg: dict, batch: int, device: torch.device, train_dropout=None, height=None, width=None):
         """train_dropout: None = inference plan; a float = TRAINING plan (forward keeps every intermediate, backward recorded) with that
-        Dropout probability (sr3_engine_create_train).  height / width: the image size the plan runs on (default image_size; training
-        plans run at image_size only)."""
+        Dropout probability (sr3_engine_create_train_sized).  height / width: the image size the plan runs on (default image_size; any size
+        check_image_size accepts, for both kinds of plan)."""
         if device.type != "cuda":
             raise NativeLibraryError("sr3_b200 runs on a CUDA (sm_90a) device only; got device=%s" % device)
         self.device = device
@@ -202,9 +203,6 @@ class Engine:
         self.image_size = cfg["image_size"]
         self.height = int(cfg["image_size"] if height is None else height)
         self.width = int(cfg["image_size"] if width is None else width)
-        if train_dropout is not None and (self.height, self.width) != (self.image_size, self.image_size):
-            raise NotImplementedError("sr3_b200: training plans run at image_size x image_size (%d) only, not %dx%d"
-                                      % (self.image_size, self.height, self.width))
         check_image_size(len(cfg["channel_mults"]), self.height, self.width)
         self.conditional = bool(cfg["conditional"])
         c = UNetConfigC()
@@ -227,7 +225,8 @@ class Engine:
         if train_dropout is None:
             _check(lib().sr3_engine_create_sized(ctypes.byref(c), batch, self.height, self.width, idx, ctypes.byref(self._h)))
         else:
-            _check(lib().sr3_engine_create_train(ctypes.byref(c), batch, idx, float(train_dropout), ctypes.byref(self._h)))
+            _check(lib().sr3_engine_create_train_sized(ctypes.byref(c), batch, self.height, self.width, idx, float(train_dropout),
+                                                       ctypes.byref(self._h)))
         self.T = 0
         self._keep = []
 
@@ -346,6 +345,8 @@ class Engine:
         hr, noise = _f32c(hr, self.device), _f32c(noise, self.device)
         s = None if sr is None else _f32c(sr, self.device)
         g = _f32c(gamma, self.device).reshape(-1)
+        self._check_inputs(hr, s)
+        self._check_img(noise, self.channels, "noise")
         self._keep = [hr, noise, s, g]
         out = c_double()
         with torch.cuda.device(self.device):

@@ -1168,6 +1168,7 @@ struct sr3_engine {
     std::map<std::string, size_t> role_max;
     std::map<std::string, void*> role_ptr;
     bool dry = true;
+    size_t plan_bytes = 0;                  // sizing pass: the bytes the real pass allocates outside the shared scratch (role_max) and arenas
     // ---- training plan (sr3_engine_create_train): every scratch tensor of the forward is kept for the backward, which is recorded layer by
     // layer while the forward plan is built and replayed in reverse order
     bool train = false; float drop_p = 0.f;
@@ -1226,7 +1227,7 @@ struct sr3_engine {
     void* role(const std::string& r, size_t bytes) {
         // training plan: forward scratch is read again by the backward -> one allocation per use ("g_*" = backward scratch stays shared)
         if (train && r.compare(0, 2, "g_") != 0) {
-            if (dry) return reinterpret_cast<void*>(0x1000);
+            if (dry) { plan_bytes += bytes; return reinterpret_cast<void*>(0x1000); }
             return mem.alloc(bytes);
         }
         if (dry) { size_t& m = role_max[r]; if (bytes > m) m = bytes; return reinterpret_cast<void*>(0x1000); }
@@ -1245,6 +1246,7 @@ struct sr3_engine {
         Act a; a.C = C; a.H = Hh; a.W = Ww;
         a.stats = new_stats(C);
         if (train) a.gsum = new_zero((size_t)Bp * C);
+        if (dry) plan_bytes += (size_t)Bp * Hh * Ww * C * (train ? 10 : 4);      // fp32 value (+ fp32 and bf16 gradient)
         if (!dry) {
             a.p = static_cast<float*>(mem.alloc((size_t)Bp * Hh * Ww * C * sizeof(float)));
             if (train) {
@@ -1272,8 +1274,8 @@ struct sr3_engine {
         params.push_back(std::move(e));
     }
     float* f32_param(const std::string& name, std::vector<int64_t> shape) {
-        if (dry) return nullptr;
         int64_t n = 1; for (auto s : shape) n *= s;
+        if (dry) { plan_bytes += n * sizeof(float); return nullptr; }
         float* dst = static_cast<float*>(mem.alloc(n * sizeof(float)));
         f32_param_into(name, shape, dst);
         return dst;
@@ -1293,9 +1295,10 @@ struct sr3_engine {
         add_pack(name, d);
     }
     bf16* new_weight(int rows, int ktot) {      // [rows_pad][PW * ktot]: precise mode appends the low halves of every row
-        if (dry) return nullptr;
         const int rows_pad = ((rows + 127) / 128) * 128;
-        return static_cast<bf16*>(mem.alloc((size_t)rows_pad * PW * ktot * sizeof(bf16)));
+        const size_t bytes = (size_t)rows_pad * PW * ktot * sizeof(bf16);
+        if (dry) { plan_bytes += bytes; return nullptr; }
+        return static_cast<bf16*>(mem.alloc(bytes));
     }
     // precise-mode fields of an image conv whose A sources have c0 (c1) channels and whose weight rows hold ktot (high) columns
     void set_precise(GemmDesc& d, int c0, int c1, int ktot) {
@@ -1540,6 +1543,7 @@ struct sr3_engine {
         F = F_total;
         if (train) {
             fin_bias_sum = new_zero(4); dfilm = new_zero((size_t)Bp * F); dtau = new_zero((size_t)Bp * inner);
+            if (dry) plan_bytes += (size_t)Bp * H * W * 64 * sizeof(bf16) + (size_t)F * (inner + 2) * 4;
             if (!dry) {
                 deps_b = static_cast<bf16*>(mem.alloc((size_t)Bp * H * W * 64 * sizeof(bf16)));
                 dwf_all = static_cast<float*>(mem.alloc((size_t)F * inner * 4)); dbf_all = static_cast<float*>(mem.alloc((size_t)F * 4));
@@ -1626,8 +1630,10 @@ struct sr3_engine {
                 const int C = x.C, Hl = x.H, Wl = x.W;
                 const int rows_pad = ((C + 127) / 128) * 128;
                 bf16* wall = nullptr;     // [phase][rows_pad][PW * 4C]
+                const size_t wall_bytes = (size_t)4 * rows_pad * 4 * C * PW * sizeof(bf16);
+                if (dry) plan_bytes += wall_bytes;
                 if (!dry) {
-                    wall = static_cast<bf16*>(mem.alloc((size_t)4 * rows_pad * 4 * C * PW * sizeof(bf16)));
+                    wall = static_cast<bf16*>(mem.alloc(wall_bytes));
                     add_param(L.name + ".conv.weight", {C, C, 3, 3});
                     PackDesc d{}; d.type = 5; d.dst = wall; d.Cout = C; d.Cin = C; d.ld = 4 * C * PW; d.lo_off = precise ? 4 * C : 0;
                     d.n = (long long)rows_pad * 4 * C * PW;
@@ -1705,9 +1711,20 @@ struct sr3_engine {
         T_cap = 4096;
         REQUIRE(!(train && precise), "the training plan supports the bf16 precision only");
         // pass 1: sizes
-        dry = true; stats_used = 0; zero_used = 0;
+        dry = true; stats_used = 0; zero_used = 0; plan_bytes = 0;
         build_plan();
         bwd_blocks.clear(); bwd_kinds.clear(); bwd_block_params.clear(); film_slices.clear(); drop_host.clear(); drop_names.clear();
+        if (train) {
+            // a training plan keeps every intermediate, and its attention scratch grows as (tokens per image)^2: refuse one that cannot fit
+            // now, rather than let an allocation fail halfway through the plan
+            size_t need = plan_bytes + ((stats_used + 3) & ~size_t(3)) * sizeof(double) + (zero_used + 4) * sizeof(float);
+            for (auto& kv : role_max) need += kv.second;
+            need += (size_t)Bp * H * W * in_C * 2 + (size_t)6 * Bp * cfg.channels * H * W * 4;     // in_buf and the six image buffers
+            size_t free_b = 0, total_b = 0;
+            CK(cudaMemGetInfo(&free_b, &total_b));
+            REQUIRE(need <= free_b, "training plan at %dx%d, batch %d: needs %zu bytes (%.2f GiB) of device memory, %zu bytes (%.2f GiB) are free",
+                    H, W, B, need, need / 1073741824.0, free_b, free_b / 1073741824.0);
+        }
         if (train) {
             zero_cap = zero_used + 4;
             zero_arena = static_cast<float*>(mem.alloc(zero_cap * sizeof(float)));
@@ -1817,15 +1834,19 @@ int sr3_engine_create(const sr3_unet_config* cfg, int batch, int device, sr3_eng
     if (!cfg) { g_err = "null argument"; return 1; }
     return sr3_engine_create_sized(cfg, batch, cfg->image_size, cfg->image_size, device, out);
 }
-int sr3_engine_create_train(const sr3_unet_config* cfg, int batch, int device, float dropout, sr3_engine** out) {
+int sr3_engine_create_train_sized(const sr3_unet_config* cfg, int batch, int height, int width, int device, float dropout, sr3_engine** out) {
     API_BEGIN
     REQUIRE(cfg && out, "null argument");
     REQUIRE(dropout >= 0.f && dropout < 1.f, "dropout %f out of range", dropout);
     std::unique_ptr<sr3_engine> e(new sr3_engine());
     e->train = true; e->drop_p = dropout;
-    e->init(*cfg, batch, cfg->image_size, cfg->image_size, device);
+    e->init(*cfg, batch, height, width, device);
     *out = e.release();
     API_END
+}
+int sr3_engine_create_train(const sr3_unet_config* cfg, int batch, int device, float dropout, sr3_engine** out) {
+    if (!cfg) { g_err = "null argument"; return 1; }
+    return sr3_engine_create_train_sized(cfg, batch, cfg->image_size, cfg->image_size, device, dropout, out);
 }
 void sr3_engine_destroy(sr3_engine* e) { delete e; }
 
@@ -2815,7 +2836,7 @@ int sr3_test_loss_grad(const float* noise, const float* eps, int B, int C, int H
                        float* bias_sum, void* stream) {
     API_BEGIN
     REQUIRE(noise && eps && loss_host && deps_bf16 && bias_sum, "null argument");
-    REQUIRE(B >= 1 && C >= 1 && C <= ld && (H * W) % 32 == 0, "bad loss shape");
+    REQUIRE(B >= 1 && C >= 1 && C <= ld && H >= 1 && W >= 1, "bad loss shape");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     DevAllocs mem;
     double* loss = static_cast<double*>(mem.alloc(sizeof(double)));

@@ -575,6 +575,10 @@ __global__ void __launch_bounds__(256) loss_grad_kernel(const float* __restrict_
         const int c = static_cast<int>(r % C);
         const int b = static_cast<int>(r / C);
         deps[((static_cast<long long>(b) * H + h) * W + w) * ld + c] = __float2bfloat16_rn(g);
+        if ((H * W) & 31) {                            // a 4x4 image: (b, c) changes inside a warp
+            atomicAdd(&bias_sum[c], g);
+            continue;
+        }
         float gs = g;                                  // H * W is a multiple of 32: the lanes of a warp share (b, c)
 #pragma unroll
         for (int o = 16; o; o >>= 1) gs += __shfl_xor_sync(0xffffffffu, gs, o);

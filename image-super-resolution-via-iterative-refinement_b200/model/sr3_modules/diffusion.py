@@ -163,9 +163,22 @@ class GaussianDiffusion(nn.Module):
     def p_losses(self, x_in, noise=None, gamma=None, dropout_seed=None):
         """diffusion.py:221-246.  With autograd enabled and trainable parameters the value carries a grad_fn (the native backward,
         csrc/train_plan.inc), so the reference's `l_pix.backward(); optG.step()` (model.py:48-58) works unchanged; in train() mode the
-        Dropout of every ResnetBlock's block2 (unet.py:86,100-101) is applied.  `gamma` / `dropout_seed` inject the random draws (tests)."""
+        Dropout of every ResnetBlock's block2 (unet.py:86,100-101) is applied.  `gamma` / `dropout_seed` inject the random draws (tests).
+        Like the reference, the image size is x_in['HR']'s (any size _native.check_image_size accepts); x_in['SR'] must have the same."""
         x_start = x_in["HR"]
-        b = x_start.shape[0]
+        b, _, h, w = x_start.shape
+        sr = x_in["SR"] if self.conditional else None
+        if sr is not None and tuple(sr.shape[2:]) != (h, w):
+            raise ValueError("x_in['SR'] is %dx%d but x_in['HR'] is %dx%d" % (sr.shape[2], sr.shape[3], h, w))
+        params = [p for p in self.denoise_fn.parameters()]
+        needs_grad = torch.is_grad_enabled() and any(p.requires_grad for p in params)
+        drop = float(getattr(self.denoise_fn, "dropout", 0) or 0) if self.training else 0.0
+        plain = not needs_grad and drop == 0.0
+        # the engine first: an unsupported size is refused before anything is drawn or allocated
+        if plain:      # q_sample + UNet + summed loss on the inference plan (no intermediates kept)
+            eng = self._engine(b, h, w)
+        else:
+            eng = self.denoise_fn.engine(b, conditional=self.conditional, channels=self.channels, train_dropout=drop, height=h, width=w)
         if gamma is None:
             t = np.random.randint(1, self.num_timesteps + 1)
             gamma = torch.FloatTensor(np.random.uniform(self.sqrt_alphas_cumprod_prev[t - 1], self.sqrt_alphas_cumprod_prev[t], size=b))
@@ -173,17 +186,11 @@ class GaussianDiffusion(nn.Module):
         noise = torch.randn_like(x_start) if noise is None else noise
         if self.loss_type not in ("l1", "l2"):
             raise NotImplementedError()
-        sr = x_in["SR"] if self.conditional else None
-        params = [p for p in self.denoise_fn.parameters()]
-        needs_grad = torch.is_grad_enabled() and any(p.requires_grad for p in params)
-        drop = float(getattr(self.denoise_fn, "dropout", 0) or 0) if self.training else 0.0
-        if not needs_grad and drop == 0.0:
-            # q_sample + UNet + summed loss on the inference plan (no intermediates kept)
-            val = self._engine(b).p_losses(x_start, sr, gamma.view(-1), noise, self.loss_type)
+        if plain:
+            val = eng.p_losses(x_start, sr, gamma.view(-1), noise, self.loss_type)
             return torch.tensor(val, dtype=torch.float32, device=x_start.device)
         if dropout_seed is None:
             dropout_seed = int(torch.randint(0, 2 ** 62, (1,)).item())
-        eng = self.denoise_fn.engine(b, conditional=self.conditional, channels=self.channels, train_dropout=drop)
         return _PLossesFn.apply(self, eng, x_start, sr, gamma.view(-1), noise, int(dropout_seed), *params)
 
     def forward(self, x, *args, **kwargs):

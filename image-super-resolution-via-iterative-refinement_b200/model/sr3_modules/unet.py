@@ -182,7 +182,7 @@ class UNet(nn.Module):
     def engine(self, batch, conditional=True, channels=3, train_dropout=None, height=None, width=None):
         """train_dropout=None: the inference plan; a float: the TRAINING plan (intermediates kept, backward recorded) with that Dropout
         probability -- see GaussianDiffusion.p_losses.  height / width: the image size the plan runs on (default image_size; any size
-        _native.check_image_size accepts, inference plans only).  Engines are kept per (batch, size, ...), and every one of them re-packs
+        _native.check_image_size accepts, for both kinds of plan).  Engines are kept per (batch, size, ...), and every one of them re-packs
         the weights before its next use once they changed."""
         dev = next(self.parameters()).device
         size = self.arch["image_size"]

@@ -203,14 +203,15 @@ class DataParallelTrainer:
         self._eng = eng
 
     def step(self, hr, sr, gamma=None, noise=None, dropout_seed=None, global_batch=None):
-        """hr / sr: THIS rank's slice [b,3,H,W] (device or host).  Returns the summed loss of the slice (python float)."""
+        """hr / sr: THIS rank's slice [b,3,H,W] (device or host), H x W any size _native.check_image_size accepts.  Returns the summed loss
+        of the slice (python float)."""
         import numpy as np
         net = self.net
         b, c, h, w = hr.shape
         world = dist.get_world_size(self.group) if dist.is_initialized() else 1
         gb = global_batch if global_batch is not None else b * world
         drop = float(getattr(net.denoise_fn, "dropout", 0) or 0) if net.training else 0.0
-        eng = net.denoise_fn.engine(b, conditional=net.conditional, channels=net.channels, train_dropout=drop)
+        eng = net.denoise_fn.engine(b, conditional=net.conditional, channels=net.channels, train_dropout=drop, height=h, width=w)
         self._prepare(eng)
         if gamma is None:
             t = np.random.randint(1, net.num_timesteps + 1)

@@ -62,7 +62,8 @@ int sr3_engine_create(const sr3_unet_config* cfg, int batch, int device, sr3_eng
  * h * w tokens of the level it sits on.  Supported sizes: at every level (height and width halved n_mults - 1 times) both sides are powers
  * of two and at least 8, or the lowest level is exactly 4x4; anything else fails before any allocation.  The batch of a plan whose lowest
  * level is 4x4 is padded to 8 as above.  sr3_engine_create(cfg, ...) is sr3_engine_create_sized(cfg, ..., image_size, image_size, ...).
- * Every entry point below then reads and writes [B,C,height,width] images.  Training plans (sr3_engine_create_train) run at image_size. */
+ * Every entry point below then reads and writes [B,C,height,width] images.  Training plans take the same sizes through
+ * sr3_engine_create_train_sized. */
 int sr3_engine_create_sized(const sr3_unet_config* cfg, int batch, int height, int width, int device, sr3_engine** out);
 void sr3_engine_destroy(sr3_engine* e);
 
@@ -113,6 +114,12 @@ int sr3_p_losses(sr3_engine* e, const float* hr, const float* sr, const float* g
  * backward recorded next to it.  `dropout` = opt['model']['unet']['dropout'] (nn.Dropout in block2 of every ResnetBlock, unet.py:86,100-101);
  * bf16 precision only.  Inference entry points keep working on such an engine (eval-mode semantics are NOT applied: use a plain engine). */
 int sr3_engine_create_train(const sr3_unet_config* cfg, int batch, int device, float dropout, sr3_engine** out);
+/* The same training plan for images of height x width (p_losses takes its size from x_in['HR'], diffusion.py:221-246): the sizes, the
+ * attention placement and the batch padding of sr3_engine_create_sized; an unsupported size fails before any device work.  The training
+ * plan keeps every intermediate, and its attention scratch grows as (tokens per image)^2, so the plan's device bytes are counted before
+ * anything is allocated: a plan larger than the device's free memory fails here, with a message naming the size, the batch and the bytes,
+ * never in a step.  sr3_engine_create_train(cfg, ...) is sr3_engine_create_train_sized(cfg, ..., image_size, image_size, ...). */
+int sr3_engine_create_train_sized(const sr3_unet_config* cfg, int batch, int height, int width, int device, float dropout, sr3_engine** out);
 /* p_losses forward in training mode with the random draws injected (as sr3_p_losses): q_sample, UNet with Dropout (Philox keyed by
  * dropout_seed, or the masks given to sr3_train_set_dropout_mask), summed L1 / L2 loss -> *loss_host (may be NULL: no synchronisation). */
 int sr3_train_forward(sr3_engine* e, const float* hr, const float* sr, const float* gamma, const float* noise, int loss_type, uint64_t dropout_seed,
