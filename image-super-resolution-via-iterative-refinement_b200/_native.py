@@ -464,7 +464,8 @@ class Engine:
         return out
 
     def profile_step(self, t, reps=3):
-        """[(kind, ms, flops, bytes)] per launch of one eager step (kinds: 0 gemm tile, 1 GN apply, 2 cast, 3 softmax, 4 other)."""
+        """[(kind, ms, flops, bytes)] per launch of one eager step (kinds: 0 gemm tile, 1 GN apply, 2 cast, 3 softmax, 4 other,
+        5 fused attention core: attn_kernel up to 256 tokens per attention batch, attn_long_kernel above)."""
         cap = lib().sr3_engine_num_ops_per_step(self._h)
         kinds, ms = (c_int * cap)(), (c_float * cap)()
         fl, by = (c_double * cap)(), (c_double * cap)()

@@ -7,7 +7,7 @@
 // image at 16x16: cheaper than a second launch) so that 2 * C/DN CTAs per image run instead of 2.  n_head = 1 in every reference
 // config, so the head dimension is C (512): S needs all of it (K loop over C); O's columns are split across CTAs.  Key count
 // Lt <= 256 (16x16 = 256 tokens; two 8x8 images share a 128-token batch with a block-diagonal mask, as in softmax_kernel); longer
-// sequences (32x32 mid block of the 64->512 config) keep the three-launch path.
+// sequences (32x32 mid block of the 64->512 config, larger images) run attn_long_kernel (attn_long_wgmma.cuh).
 //
 // Operands (both produced by tile-kernel launches): qk [nz*Lt][2C] bf16 (q = columns [0,C), k = [C,2C)), vT [nz*C][Lt] bf16.
 // Warp roles: 8 = TMA producer, 0..7 = two warpgroups, each owning 64 query rows: S (64 x Lt) and O (64 x DN) in registers.

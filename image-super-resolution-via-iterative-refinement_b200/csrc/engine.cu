@@ -20,6 +20,7 @@
 #include "../../include/sr3_b200.h"
 #include "aux_kernels.cuh"
 #include "attn_wgmma.cuh"
+#include "attn_long_wgmma.cuh"
 #include "train_kernels.cuh"
 
 using namespace sr3;
@@ -470,11 +471,14 @@ Op make_gemm_op(const GemmDesc& d, DevAllocs& mem, sr3_gemm_geometry* geo = null
     };
 }
 
-// Fused attention core (attn_wgmma.cuh): S = q k^T / sqrt(C), softmax, O = P v in one launch.  qk [nz*Lt][2C], vT [nz*C][Lt], out [nz*Lt][C].
-bool attn_fusable(int Lt, int C) { return (Lt == 128 || Lt == 256) && C % 128 == 0 && C >= 128; }
+// Fused attention core: S = q k^T / sqrt(C), softmax, O = P v in one launch.  qk [nz*Lt][2C], vT [nz*C][Lt], out [nz*Lt][C].
+// Up to 256 tokens a row block of S stays in registers (attn_wgmma.cuh); above, the keys stream through in blocks of 128 with a
+// running maximum (attn_long_wgmma.cuh), and an attention batch is then always one image.
+bool attn_fusable(int Lt, int C) { return Lt >= 128 && Lt % 128 == 0 && C % 128 == 0 && C >= 128; }
 
 Op make_attn_op(const bf16* qk, const bf16* vT, bf16* out, int nz, int Lt, int HW, int C) {
     REQUIRE(attn_fusable(Lt, C) && Lt % HW == 0, "attention shape Lt=%d HW=%d C=%d is not supported by the fused kernel", Lt, HW, C);
+    REQUIRE(Lt <= 256 || HW == Lt, "attention over %d tokens per batch takes one image per batch (HW=%d)", Lt, HW);
     AttnParams p;
     memset(&p, 0, sizeof(p));
     {
@@ -492,6 +496,13 @@ Op make_attn_op(const bf16* qk, const bf16* vT, bf16* out, int nz, int Lt, int H
     p.out = out; p.C = C; p.Lt = Lt; p.HW = HW; p.nz = nz;
     p.dn = (C % 256 == 0) ? 256 : 128;
     p.scale_log2e = 1.4426950408889634f / sqrtf((float)C);
+    if (Lt > 256) {
+        p.dn = ATTNL_DN;
+        static std::vector<int> seen_long;
+        if (first_use_on_device(seen_long)) CK(cudaFuncSetAttribute(attn_long_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ATTNL_SMEM_BYTES));
+        const dim3 grid((Lt / 128) * (C / ATTNL_DN), nz, 1);
+        return [p, grid](cudaStream_t st) { launch_k(attn_long_kernel, grid, dim3(ATTN_THREADS), ATTNL_SMEM_BYTES, st, p); };
+    }
     static std::vector<int> seen;
     if (first_use_on_device(seen)) CK(cudaFuncSetAttribute(attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ATTN_SMEM_BYTES));
     const dim3 grid((Lt / 128) * (C / p.dn), nz, 1);
@@ -1042,7 +1053,7 @@ ConvArgs upsample_dgrad_conv(const bf16* dy, int Bp, int yH, int yW, int C, cons
     return c;
 }
 
-// ---- unfused attention forward (attention batches the fused kernel does not take, precise mode, training): nz batches of Lt tokens, HW
+// ---- unfused attention forward (precise mode, training): nz batches of Lt tokens, HW
 // tokens per image, head dim C; PW = 2 in precise mode (every bf16 row is [hi | lo])
 // S[z] = q k^T / sqrt(C): qk bf16 [nz][Lt][2C PW] (rows [q_hi | k_hi | q_lo | k_lo]) -> S fp32 [nz][Lt][Lt]
 GemmDesc attn_s_desc(const bf16* qk, float* S, int nz, int Lt, int C, int PW) {
@@ -1160,7 +1171,7 @@ struct sr3_engine {
     std::map<std::string, int> pindex;
     std::vector<Op> ops;
     std::vector<GemmHandle> gemms;          // tile-kernel launches of the step, in order (for next-layer weight prefetch)
-    // kind: 0 gemm, 1 groupnorm-apply, 2 cast/upsample, 3 softmax, 4 other.  Tile ops also keep the variant they launch (sr3_tile_schedule):
+    // kind: 0 gemm, 1 groupnorm-apply, 2 cast/upsample, 3 softmax, 4 other, 5 fused attention core.  Tile ops also keep the variant they launch (sr3_tile_schedule):
     // geometry, schedule (0 cooperative, 1 ping-pong; -1 not a tile op) and output rows x columns x channels.
     struct OpInfo { int kind; double flops; double bytes; sr3_gemm_geometry geo; int schedule; int out_hwc[3]; };
     std::vector<OpInfo> op_info;
@@ -1457,8 +1468,9 @@ struct sr3_engine {
         bf16* n = static_cast<bf16*>(role("a1", (size_t)Bp * HW * C * 2 * PW));
         bf16* qk = static_cast<bf16*>(role("qk", (size_t)Bp * HW * 2 * C * 2 * PW));
         bf16* vT = static_cast<bf16*>(role("vT", (size_t)nz * C * Lt * 2 * PW));
-        float* S = static_cast<float*>(role("S", (size_t)nz * Lt * Lt * 4));
-        bf16* P = static_cast<bf16*>(role("P", (size_t)nz * Lt * Lt * 2 * PW));
+        const bool fused = attn_fusable(Lt, C) && !precise && !train;      // one launch; S and P then never exist in device memory
+        float* S = fused ? nullptr : static_cast<float*>(role("S", (size_t)nz * Lt * Lt * 4));
+        bf16* P = fused ? nullptr : static_cast<bf16*>(role("P", (size_t)nz * Lt * Lt * 2 * PW));
         bf16* O = static_cast<bf16*>(role("O", (size_t)Bp * HW * C * 2 * PW));
         Act y = new_act(C, Hh, Ww, L.name);
         add_prep(x, nullptr, gn_w, gn_b, G, false, n, nullptr);
@@ -1481,8 +1493,8 @@ struct sr3_engine {
             d.pingpong = pingpong_knob() == 1 ? 1 : 0;         // (fixed 128x128 shape: the byte model is not consulted)
             push_gemm(d);
         }
-        if (attn_fusable(Lt, C) && !precise && !train) {
-            // S = q k^T / sqrt(C), softmax over the keys of the same image, O = P v: one launch (attn_wgmma.cuh)
+        if (fused) {
+            // S = q k^T / sqrt(C), softmax over the keys of the same image, O = P v: one launch (attn_wgmma.cuh, attn_long_wgmma.cuh)
             const double fl = 4.0 * nz * (double)Lt * Lt * C;
             push(make_attn_op(qk, vT, O, nz, Lt, HW, C), 5, fl, (double)nz * Lt * C * 2 * 4);
         } else {

@@ -205,7 +205,8 @@ int sr3_engine_num_ops_per_step(const sr3_engine* e);        /* ops of the step 
 int64_t sr3_engine_workspace_bytes(const sr3_engine* e);
 /* Per-kernel timing of one eager (non-graph) reverse step at timestep t, averaged over `reps` repetitions after one warm-up,
  * CUDA events on `stream` around every launch.  kinds: 0 tensor-core tile kernel, 1 GroupNorm apply, 2 cast/upsample,
- * 3 softmax, 4 other; flops / bytes are the executed work of each launch.  Does not modify the sampler state. */
+ * 3 softmax, 4 other, 5 fused attention core (flops: the algorithmic 4 nz Lt^2 C, not the recomputed S); flops / bytes are otherwise the
+ * executed work of each launch.  Does not modify the sampler state. */
 int sr3_engine_profile_step(sr3_engine* e, int t, int reps, int cap, int* kinds, float* ms, double* flops, double* bytes, int* n_ops,
                             void* stream);
 /* Debug tap: copy the fp32 NHWC output of top-level layer `name` ("downs.3", "mid.0", ...) of the last forward to dst
@@ -216,9 +217,10 @@ int sr3_engine_read_activation(sr3_engine* e, const char* name, float* dst, int6
  * K%64==0, N%block_n==0. */
 int sr3_test_gemm(const void* a_bf16, const void* b_bf16, float* d, int M, int N, int K, int block_n, void* stream);
 /* Test hook for the fused attention core (S = q k^T / sqrt(C), softmax per image, O = P v; unet.py:129-139): qk bf16 [nz*Lt][2C]
- * (q | k), vT bf16 [nz*C][Lt], out bf16 [nz*Lt][C]; Lt in {128, 256} keys per attention batch, HW tokens per image (Lt % HW == 0). */
+ * (q | k), vT bf16 [nz*C][Lt], out bf16 [nz*Lt][C]; Lt keys per attention batch (a multiple of 128), HW tokens per image (Lt % HW == 0; above 256 keys
+ * HW == Lt and the streaming-softmax kernel runs). */
 int sr3_test_attention(const void* qk_bf16, const void* vT_bf16, void* out_bf16, int nz, int Lt, int HW, int C, void* stream);
-/* Test hook for the unfused attention path (attention batches of other sizes, precise mode, training), the plan's three launches:
+/* Test hook for the unfused attention path (precise mode, training), the plan's three launches:
  * S = q k^T / sqrt(C) on the tile kernel, softmax_kernel over the keys of each image, O = P v on the tile kernel.  qk bf16 [nz*Lt][2C PW]
  * (rows [q | k], precise = 1: [q_hi | k_hi | q_lo | k_lo]), vT bf16 [nz*C][Lt PW] -> S fp32 [nz*Lt][Lt], P bf16 [nz*Lt][Lt PW],
  * O bf16 [nz*Lt][C PW]; PW = 2 in precise mode (rows [hi | lo]), else 1.  Lt % 128 == 0, C % 128 == 0, HW tokens per image (Lt % HW == 0). */

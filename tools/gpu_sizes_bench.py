@@ -1,10 +1,10 @@
 """Speed of the 16->128 config (sr_sr3_16_128: image_size 128, attention on the 16x16 level of a 128x128 image) at other image sizes.
 The attention layers stay on the level image_size placed them on, so their token count grows with the image: 256 tokens at 128x128
-(fused attention kernel), 512 at 128x256, 1024 at 256x256 and 4096 at 512x512 (S = q k^T, row softmax and P v as three launches).
+(attn_kernel), 512 at 128x256, 1024 at 256x256 and 4096 at 512x512 (attn_long_kernel, the streaming-softmax form: one launch as well).
 Prints one JSON line:
   * sampling steps/s per size at a fixed batch (sampler state resident on the device, CUDA events around K steps);
-  * the per-launch time split of one eager step (sr3_engine_profile_step), summed by launch kind, with the attention core (fused kernel,
-    or the S and P v tile launches and the softmax) also summed on its own;
+  * the per-launch time split of one eager step (sr3_engine_profile_step), summed by launch kind, with the attention core (the fused launches;
+    in a plan that does not fuse, the S and P v tile launches and the softmax) also summed on its own, and the plan's device bytes;
   * the GPU's name, power limit and maximum SM clock, read in the same run.
 
     python tools/gpu_sizes_bench.py [--batch 4] [--steps 20] [--warmup 3] [--sizes 128x128,128x256,256x256,512x512]
@@ -63,7 +63,7 @@ def sampling(net, B, H, W, K, warm):
         if k in (3, 5) or (k == 0 and sched[i] is not None and sched[i]["out_hwc"][0] == 1):
             attn += t
     return {"size": f"{H}x{W}", "batch": B, "attention_tokens": (H // 8) * (W // 8), "ms_per_step": ms, "steps_per_s": 1e3 / ms,
-            "images_per_s": B * 1e3 / ms, "launches_per_step": eng.launches_per_step(), "eager_step_ms_by_kind": by_kind,
+            "images_per_s": B * 1e3 / ms, "launches_per_step": eng.launches_per_step(), "workspace_bytes": eng.workspace_bytes(), "eager_step_ms_by_kind": by_kind,
             "eager_step_attention_core_ms": attn, "eager_step_ms_total": sum(t for _, t, _, _ in prof)}
 
 
