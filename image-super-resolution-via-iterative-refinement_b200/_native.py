@@ -57,6 +57,8 @@ _SIGS = {
     "sr3_engine_create_train_sized": (c_int, [POINTER(UNetConfigC), c_int, c_int, c_int, c_int, c_float, POINTER(c_void_p)]),
     "sr3_train_forward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_uint64, POINTER(c_double), c_void_p]),
     "sr3_train_backward": (c_int, [c_void_p, c_float, POINTER(c_void_p), c_int, c_void_p]),
+    "sr3_train_unet_forward": (c_int, [c_void_p, c_void_p, c_void_p, c_uint64, c_void_p, c_void_p]),
+    "sr3_train_unet_backward": (c_int, [c_void_p, c_void_p, POINTER(c_void_p), c_int, c_void_p, c_void_p, c_void_p]),
     "sr3_train_num_backward_blocks": (c_int, [c_void_p]),
     "sr3_train_backward_begin": (c_int, [c_void_p, c_float, POINTER(c_void_p), c_int]),
     "sr3_train_backward_block": (c_int, [c_void_p, c_int, c_void_p]),
@@ -119,6 +121,9 @@ _SIGS = {
     "sr3_test_film_embed_fwd": (c_int, [c_void_p] * 10 + [c_int, c_int, c_int, c_void_p]),
     "sr3_test_attention_unfused": (c_int, [c_void_p] * 5 + [c_int] * 5 + [c_void_p]),
     "sr3_test_loss_grad": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, POINTER(c_double), c_void_p, c_int, c_void_p, c_void_p]),
+    "sr3_test_grad_load": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p]),
+    "sr3_test_noise_level_bwd": (c_int, [c_void_p] * 6 + [c_int, c_int, c_void_p]),
+    "sr3_test_input_grad": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
 }
 EXPORTED_SYMBOLS = tuple(_SIGS.keys())
 
@@ -229,6 +234,11 @@ class Engine:
                                                        ctypes.byref(self._h)))
         self.T = 0
         self._keep = []
+        # training forwards run on this engine (train_forward and train_unet_forward alike): each replaces the intermediates the previous
+        # one kept, so a UNet backward checks that its forward is still the latest one and has not been backpropagated yet
+        self.forward_count = 0
+        self._last_forward = None
+        self._unet_backward_done = 0
 
     def __del__(self):
         try:
@@ -348,6 +358,8 @@ class Engine:
         self._check_inputs(hr, s)
         self._check_img(noise, self.channels, "noise")
         self._keep = [hr, noise, s, g]
+        self.forward_count += 1
+        self._last_forward = "p_losses"
         out = c_double()
         with torch.cuda.device(self.device):
             _check(lib().sr3_train_forward(self._h, _ptr(hr), _ptr(s), _ptr(g), _ptr(noise), 1 if loss_type == "l1" else 2, int(dropout_seed),
@@ -366,6 +378,49 @@ class Engine:
         arr = self._grad_ptrs(grads)
         with torch.cuda.device(self.device):
             _check(lib().sr3_train_backward(self._h, float(grad_scale), arr, len(grads), _stream()))
+
+    # ---- UNet.forward alone in training form, and its backward from any upstream gradient (the differentiable denoise_fn)
+    def train_unet_forward(self, x, noise_level, dropout_seed=0):
+        """x [B,in_channel,H,W] (cat(cond, x_t) for a conditional net), noise_level [B] or [B,1] -> (eps [B,out_channel,H,W], the index of
+        this forward on the engine, which train_unet_backward takes).  sr3_train_unet_forward."""
+        x = _f32c(x, self.device)
+        nl = _f32c(noise_level, self.device).reshape(-1)
+        self._check_img(x, self.in_channel, "x")
+        if nl.numel() != self.batch:
+            raise ValueError("noise_level has %d elements; this engine runs a batch of %d" % (nl.numel(), self.batch))
+        eps = torch.empty(self.batch, self.out_channel, self.height, self.width, device=self.device, dtype=torch.float32)
+        self._keep = [x, nl]
+        self.forward_count += 1
+        self._last_forward = None
+        with torch.cuda.device(self.device):
+            _check(lib().sr3_train_unet_forward(self._h, _ptr(x), _ptr(nl), int(dropout_seed), _ptr(eps), _stream()))
+        self._last_forward = "unet"
+        return eps, self.forward_count
+
+    def train_unet_backward(self, deps, grads, want_dx=False, want_dnl=False, forward=None):
+        """Backward of the UNet forward with index `forward` (default: the latest) for the upstream gradient deps [B,out_channel,H,W].  grads:
+        one contiguous fp32 CUDA tensor per parameter, in param_table() order; overwritten.  Returns (dx [B,in_channel,H,W] or None,
+        d noise_level [B] or None).  Raises RuntimeError when a later forward on this engine has replaced that forward's intermediates, or
+        when it has already been backpropagated: either would give silently wrong gradients."""
+        fwd = self.forward_count if forward is None else int(forward)
+        if fwd != self.forward_count:
+            raise RuntimeError("sr3_b200: cannot backpropagate UNet forward #%d: a later forward (#%d, %s) on the same engine has replaced the "
+                               "intermediates it kept; run the backward before the next forward" %
+                               (fwd, self.forward_count, "p_losses" if self._last_forward == "p_losses" else "UNet"))
+        if self._last_forward != "unet":
+            raise RuntimeError("sr3_b200: the latest forward on this engine is not a UNet forward (train_unet_forward)")
+        if self._unet_backward_done == fwd:
+            raise RuntimeError("sr3_b200: UNet forward #%d has already been backpropagated; the native backward runs once per forward "
+                               "(retain_graph is not supported)" % fwd)
+        deps = _f32c(deps, self.device)
+        self._check_img(deps, self.out_channel, "the gradient of eps")
+        arr = self._grad_ptrs(grads)
+        dx = torch.empty(self.batch, self.in_channel, self.height, self.width, device=self.device, dtype=torch.float32) if want_dx else None
+        dnl = torch.empty(self.batch, device=self.device, dtype=torch.float32) if want_dnl else None
+        self._unet_backward_done = fwd
+        with torch.cuda.device(self.device):
+            _check(lib().sr3_train_unet_backward(self._h, _ptr(deps), arr, len(grads), _ptr(dx), _ptr(dnl), _stream()))
+        return dx, dnl
 
     def train_backward_profile(self, grad_scale, grads):
         """{kind: ms} of one backward, CUDA events around every op."""
@@ -729,3 +784,32 @@ def test_loss_grad(noise, eps, l2, deps=None, ld=64):
     _check(lib().sr3_test_loss_grad(_ptr(noise), _ptr(eps), B, C, H, W, int(bool(l2)), ctypes.byref(loss), _ptr(deps), deps.shape[3], _ptr(bias),
                                     _stream()))
     return loss.value, deps, bias
+
+
+def test_grad_load(g, deps=None, ld=64):
+    """grad_load_kernel.  g fp32 NCHW.  deps: bf16 [B,H,W,ld] updated in place (fresh zeros by default).  Returns (deps, bias_sum [C])."""
+    B, C, H, W = g.shape
+    if deps is None:
+        deps = torch.zeros(B, H, W, ld, device=g.device, dtype=torch.bfloat16)
+    bias = torch.zeros(C, device=g.device)
+    _check(lib().sr3_test_grad_load(_ptr(g), B, C, H, W, _ptr(deps), deps.shape[3], _ptr(bias), _stream()))
+    return deps, bias
+
+
+def test_noise_level_bwd(nl, w1, b1, w2, dtau):
+    """noise_level_bwd_kernel: nl [B], w1 [4 inner, inner], b1, w2 [inner, 4 inner], dtau [B, inner] (CUDA fp32) -> dnl [B]."""
+    B, inner = dtau.shape
+    dnl = torch.empty(B, device=nl.device)
+    _check(lib().sr3_test_noise_level_bwd(*[_ptr(t) for t in (nl, w1, b1, w2, dtau, dnl)], inner, B, _stream()))
+    return dnl
+
+
+def test_input_grad(dy, w_oihw):
+    """The input gradient of the UNet backward: dy bf16 NHWC [B,H,W,inner] (the first conv's output gradient), w fp32 OIHW
+    [inner,in_channel,3,3] -> dx fp32 NCHW [B,in_channel,H,W]."""
+    B, H, W, inner = dy.shape
+    cin = w_oihw.shape[1]
+    dx = torch.empty(B, cin, H, W, device=dy.device)
+    w = _f32c(w_oihw, dy.device)
+    _check(lib().sr3_test_input_grad(_ptr(dy), _ptr(w), _ptr(dx), B, H, W, inner, cin, _stream()))
+    return dx

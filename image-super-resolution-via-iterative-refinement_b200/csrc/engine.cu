@@ -950,6 +950,17 @@ void launch_loss_grad(const float* noise, const float* eps, int B, int C, int H,
     loss_grad_kernel<<<296, 256, 0, st>>>(noise, eps, B, C, H, W, l2, loss, deps, ld, bias_sum);
     CK(cudaGetLastError());
 }
+// the upstream gradient of UNet.forward in place of the loss gradient (same operand, same launch shape); bias_sum must be zero
+void launch_grad_load(const float* g, int B, int C, int H, int W, bf16* deps, int ld, float* bias_sum, cudaStream_t st) {
+    grad_load_kernel<<<296, 256, 0, st>>>(g, B, C, H, W, deps, ld, bias_sum);
+    CK(cudaGetLastError());
+}
+// dx NCHW [B][C][H][W] from the first conv's fp32 NHWC data gradient (ld channels per pixel)
+void launch_input_grad_store(const float* src, int B, int C, int H, int W, int ld, float* dst, cudaStream_t st) {
+    const long long total = 1LL * B * C * H * W;
+    input_grad_store_kernel<<<(int)std::min<long long>((total + 255) / 256, num_sms() * 8LL), 256, 0, st>>>(src, B, C, H, W, ld, dst);
+    CK(cudaGetLastError());
+}
 
 // ---- noise-level embedding + FiLM projections forward (the plan's first two launches; sr3_test_film_embed_fwd)
 constexpr int FILM_SMEM_BYTES = 48 * 1024;      // film_kernel stays within the default dynamic shared-memory limit (no opt-in)
@@ -991,6 +1002,15 @@ void launch_embed_bwd(const float* nl, const float* w1, const float* b1, const f
     embed_bwd_kernel<<<1, 256, esm, st>>>(nl, w1, b1, w2, dtau, dw1, db1, dw2, db2, inner, B, gscale);
     CK(cudaGetLastError());
 }
+void launch_noise_level_bwd(const float* nl, const float* w1, const float* b1, const float* w2, const float* dtau, float* dnl, int inner, int B,
+                            cudaStream_t st) {
+    const int esm = embed_bwd_smem(B, inner);
+    static std::vector<int> seen;
+    if (first_use_on_device(seen)) CK(cudaFuncSetAttribute(noise_level_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FILM_BWD_SMEM_MAX));
+    REQUIRE(esm <= FILM_BWD_SMEM_MAX, "noise-level backward: batch %d too large for one block", B);
+    noise_level_bwd_kernel<<<1, 256, esm, st>>>(nl, w1, b1, w2, dtau, dnl, inner, B);
+    CK(cudaGetLastError());
+}
 
 // ---- data gradients on the forward tile kernel
 // the packed weight of a data gradient (pack_entry types 2, 3, 4; the source parameter is filled in when it is packed):
@@ -1022,6 +1042,13 @@ ConvArgs dgrad_conv(const bf16* A, int Bp, int CA, int Hh, int Ww, int k, const 
     Act o; o.p = out; o.C = N; o.H = Hh; o.W = Ww; c.out = o;
     c.raw_out = out_b;
     return c;
+}
+// the data gradient of the first conv (unet.py:193, in_channel -> inner, 3x3): dy = its output gradient, bf16 [Bp][H][W][inner], w = the
+// type-2 packed weight (rows = in_channel, zero up to 128) -> out fp32 [Bp][H][W][64].  The output channels are padded to the 64 of the
+// input buffer, as the final conv's 3 channels are in its 64-channel gradient operand; channels >= in_channel come out zero.
+constexpr int INPUT_GRAD_LD = 64;
+ConvArgs input_dgrad_conv(const bf16* dy, int Bp, int Hh, int Ww, int inner, const bf16* w, float* out) {
+    return dgrad_conv(dy, Bp, inner, Hh, Ww, 3, w, INPUT_GRAD_LD, out, nullptr);
 }
 // Downsample (conv3x3 stride 2): four input-parity phases on the low-resolution dY grid (bf16 [Bp][yH][yW][C]) -> out fp32 [Bp][2yH][2yW][C]
 ConvArgs downsample_dgrad_conv(const bf16* dy, int Bp, int yH, int yW, int C, const bf16* w, float* out) {
@@ -1184,8 +1211,12 @@ struct sr3_engine {
     // layer while the forward plan is built and replayed in reverse order
     bool train = false; float drop_p = 0.f;
     std::vector<Op>* bwd_sink = nullptr;                   // where push() records while a layer's backward is being described
+    std::vector<int>* kind_sink = nullptr;                 // ... and the kinds of those ops
     std::vector<std::vector<Op>> bwd_blocks;               // one op list per forward layer, executed last to first
     std::vector<std::vector<int>> bwd_kinds;               // op kinds (profiling): 0 data-gradient tile kernel, 1 GroupNorm / elementwise, 4 other, 6 weight gradient, 7 attention GEMMs
+    // the input gradient (data gradient of the first conv, then its NCHW store into dx_out): recorded with the backward, outside the blocks,
+    // and run only when sr3_train_unet_backward is asked for dx
+    std::vector<Op> dx_ops; std::vector<int> dx_kinds; float* dx_out = nullptr;
     // every packed copy of a parameter: one PackDesc, its source = parameter `pack_src[i]` (second source of a fused bias: `pack_src2[i]`).
     // sr3_engine_load_all_params binds the sources to the caller's tensors and packs the whole table in one launch (device table rebuilt
     // only when the parameter pointers change); sr3_engine_load_param packs the entries of one parameter, and sr3_engine_finalize_params
@@ -1317,7 +1348,7 @@ struct sr3_engine {
     }
     void push(Op op, int kind = 4, double flops = 0, double bytes = 0) {
         if (dry) return;
-        if (bwd_sink) { bwd_sink->push_back(std::move(op)); bwd_kinds.back().push_back(kind); return; }
+        if (bwd_sink) { bwd_sink->push_back(std::move(op)); kind_sink->push_back(kind); return; }
         ops.push_back(std::move(op));
         op_info.push_back({kind, flops, bytes, sr3_gemm_geometry{}, -1, {0, 0, 0}});
     }
@@ -1878,6 +1909,22 @@ int sr3_train_backward(sr3_engine* e, float grad_scale, float* const* grads, int
     REQUIRE(n_grads == (int)e->params.size(), "expected %d gradient pointers, got %d", (int)e->params.size(), n_grads);
     CK(cudaSetDevice(e->dev));
     e->train_backward(grad_scale, grads, static_cast<cudaStream_t>(stream));
+    API_END
+}
+int sr3_train_unet_forward(sr3_engine* e, const float* x, const float* noise_level, uint64_t dropout_seed, float* eps, void* stream) {
+    API_BEGIN
+    REQUIRE(e && x && noise_level && eps, "null argument");
+    CK(cudaSetDevice(e->dev));
+    e->check_params();
+    e->train_unet_forward(x, noise_level, dropout_seed, eps, static_cast<cudaStream_t>(stream));
+    API_END
+}
+int sr3_train_unet_backward(sr3_engine* e, const float* deps, float* const* grads, int n_grads, float* dx, float* dnoise_level, void* stream) {
+    API_BEGIN
+    REQUIRE(e && deps && grads, "null argument");
+    REQUIRE(n_grads == (int)e->params.size(), "expected %d gradient pointers, got %d", (int)e->params.size(), n_grads);
+    CK(cudaSetDevice(e->dev));
+    e->train_unet_backward(deps, grads, dx, dnoise_level, static_cast<cudaStream_t>(stream));
     API_END
 }
 /* the same backward, layer by layer (last layer first), so that a caller can overlap the gradient all-reduce of finished layers */
@@ -2854,6 +2901,46 @@ int sr3_test_loss_grad(const float* noise, const float* eps, int B, int C, int H
     double* loss = static_cast<double*>(mem.alloc(sizeof(double)));
     launch_loss_grad(noise, eps, B, C, H, W, l2 ? 1 : 0, loss, static_cast<bf16*>(deps_bf16), ld, bias_sum, st);
     CK(cudaMemcpyAsync(loss_host, loss, sizeof(double), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    API_END
+}
+
+int sr3_test_grad_load(const float* g, int B, int C, int H, int W, void* deps_bf16, int ld, float* bias_sum, void* stream) {
+    API_BEGIN
+    REQUIRE(g && deps_bf16 && bias_sum, "null argument");
+    REQUIRE(B >= 1 && C >= 1 && C <= ld && H >= 1 && W >= 1, "bad gradient shape");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    launch_grad_load(g, B, C, H, W, static_cast<bf16*>(deps_bf16), ld, bias_sum, st);
+    CK(cudaStreamSynchronize(st));
+    API_END
+}
+
+int sr3_test_noise_level_bwd(const float* nl, const float* w1, const float* b1, const float* w2, const float* dtau, float* dnl, int inner, int B,
+                             void* stream) {
+    API_BEGIN
+    REQUIRE(nl && w1 && b1 && w2 && dtau && dnl, "null argument");
+    REQUIRE(inner >= 2 && inner % 2 == 0 && B >= 1, "bad shape");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    launch_noise_level_bwd(nl, w1, b1, w2, dtau, dnl, inner, B, st);
+    CK(cudaStreamSynchronize(st));
+    API_END
+}
+
+int sr3_test_input_grad(const void* dy_bf16, const float* w_oihw, float* dx, int B, int H, int W, int inner, int in_channel, void* stream) {
+    API_BEGIN
+    REQUIRE(dy_bf16 && w_oihw && dx, "null argument");
+    REQUIRE(B >= 1 && H >= 1 && W >= 1 && inner % 64 == 0 && in_channel >= 1 && in_channel <= INPUT_GRAD_LD, "bad input-gradient shape");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    DevAllocs mem;
+    bf16* w = static_cast<bf16*>(mem.alloc(dgrad_weight_elems(2, inner, in_channel, 3) * sizeof(bf16)));     // zero padding, as new_weight
+    PackDesc pd = dgrad_pack_desc(2, w, inner, in_channel, 3);
+    pd.src = w_oihw;
+    pack_one(pd, st);
+    float* gx = static_cast<float*>(mem.alloc((size_t)B * H * W * INPUT_GRAD_LD * sizeof(float), false));
+    GemmDesc d = conv_desc(input_dgrad_conv(static_cast<const bf16*>(dy_bf16), B, H, W, inner, w, gx), B, B, 1);
+    d.out_imgs = B;
+    make_gemm_op(d, mem)(st);
+    launch_input_grad_store(gx, B, in_channel, H, W, INPUT_GRAD_LD, dx, st);
     CK(cudaStreamSynchronize(st));
     API_END
 }

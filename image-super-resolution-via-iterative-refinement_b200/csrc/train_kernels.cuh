@@ -458,11 +458,10 @@ __global__ void __launch_bounds__(256) film_bwd_kernel(const float* __restrict__
     __syncthreads();
     for (int i = threadIdx.x; i < B * inner; i += blockDim.x) atomicAdd(&dtau[i], dts[i]);
 }
-// tau = W2 swish(W1 pe + b1) + b2 (unet.py:177-184): one block, everything in shared memory.  pe / pre are recomputed from the noise level.
-__global__ void __launch_bounds__(256) embed_bwd_kernel(const float* __restrict__ nl, const float* __restrict__ w1, const float* __restrict__ b1,
-                                                        const float* __restrict__ w2, const float* __restrict__ dtau, float* __restrict__ dw1, float* __restrict__ db1,
-                                                        float* __restrict__ dw2, float* __restrict__ db2, int inner, int B, float gscale) {
-    extern __shared__ float sm[];
+// The shared part of the noise-level MLP's backward: pe and pre recomputed from the noise level, dpre = d pre from dtau.  Shared memory
+// (embed_bwd_smem) holds pe [B][inner], pre [B][hid], dpre [B][hid], dt [B][inner] in that order; returns with all of it written.
+__device__ __forceinline__ void embed_bwd_dpre(const float* __restrict__ nl, const float* __restrict__ w1, const float* __restrict__ b1,
+                                               const float* __restrict__ w2, const float* __restrict__ dtau, float* sm, int inner, int B) {
     const int hid = 4 * inner;
     float* pe = sm;                       // [B][inner]
     float* pre = pe + B * inner;          // [B][hid]
@@ -493,6 +492,18 @@ __global__ void __launch_bounds__(256) embed_bwd_kernel(const float* __restrict_
         dpre[idx] = a * sg * (1.0f + x * (1.0f - sg));
     }
     __syncthreads();
+}
+// tau = W2 swish(W1 pe + b1) + b2 (unet.py:177-184): one block, everything in shared memory.  pe / pre are recomputed from the noise level.
+__global__ void __launch_bounds__(256) embed_bwd_kernel(const float* __restrict__ nl, const float* __restrict__ w1, const float* __restrict__ b1,
+                                                        const float* __restrict__ w2, const float* __restrict__ dtau, float* __restrict__ dw1, float* __restrict__ db1,
+                                                        float* __restrict__ dw2, float* __restrict__ db2, int inner, int B, float gscale) {
+    extern __shared__ float sm[];
+    const int hid = 4 * inner;
+    float* pe = sm;                       // [B][inner]
+    float* pre = pe + B * inner;          // [B][hid]
+    float* dpre = pre + B * hid;          // [B][hid]
+    float* dt = dpre + B * hid;           // [B][inner]
+    embed_bwd_dpre(nl, w1, b1, w2, dtau, sm, inner, B);
     for (int idx = threadIdx.x; idx < inner * hid; idx += blockDim.x) {     // dW2[o][j] = sum_b dtau[b][o] swish(pre[b][j])
         const int o = idx / hid, j = idx % hid;
         float a = 0.f;
@@ -507,6 +518,33 @@ __global__ void __launch_bounds__(256) embed_bwd_kernel(const float* __restrict_
         dw1[idx] = a * gscale;
     }
     for (int j = threadIdx.x; j < hid; j += blockDim.x) { float a = 0.f; for (int b = 0; b < B; ++b) a += dpre[b * hid + j]; db1[j] = a * gscale; }
+}
+// Gradient of the noise level itself (unet.py:18-31 PositionalEncoding, the MLP's input): dPE[b] = W1^T dpre[b] (dpre as embed_bwd_kernel
+// forms it), then dnl[b] = sum_i dPE[b][i] dPE_i/dnl with PE_i = sin(nl f_i) for i < inner/2 (derivative cos(nl f_i) f_i), cos(nl f_i) for
+// the other half (-sin(nl f_i) f_i), f_i = exp(-ln(1e4) (i mod inner/2) / (inner/2)).  One block (shared memory as embed_bwd_kernel), one
+// warp per image.  Unscaled: the caller's upstream gradient carries any scale.
+__global__ void __launch_bounds__(256) noise_level_bwd_kernel(const float* __restrict__ nl, const float* __restrict__ w1, const float* __restrict__ b1,
+                                                              const float* __restrict__ w2, const float* __restrict__ dtau, float* __restrict__ dnl, int inner,
+                                                              int B) {
+    extern __shared__ float sm[];
+    const int hid = 4 * inner, count = inner / 2;
+    const float* dpre = sm + B * inner + B * hid;
+    embed_bwd_dpre(nl, w1, b1, w2, dtau, sm, inner, B);
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarp = blockDim.x >> 5;
+    for (int b = warp; b < B; b += nwarp) {
+        float acc = 0.f;
+        for (int i = lane; i < inner; i += 32) {
+            float d = 0.f;
+            for (int j = 0; j < hid; ++j) d += w1[j * inner + i] * dpre[b * hid + j];
+            const int ii = i < count ? i : i - count;
+            const float f = expf(-9.210340371976184f * (static_cast<float>(ii) / static_cast<float>(count)));
+            const float e = nl[b] * f;
+            acc += d * (i < count ? cosf(e) : -sinf(e)) * f;
+        }
+#pragma unroll
+        for (int o = 16; o; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+        if (lane == 0) dnl[b] = acc;
+    }
 }
 
 // ------------------------------------------------------------------------------------------------ attention backward (unet.py:129-139)
@@ -593,6 +631,43 @@ __global__ void __launch_bounds__(256) loss_grad_kernel(const float* __restrict_
         double t = 0.0;
         for (int i = 0; i < 8; ++i) t += ws[i];
         atomicAdd(loss, t);
+    }
+}
+// The backward of UNet.forward alone, from an upstream gradient g = d(anything) / d eps (fp32 NCHW [B][C][H][W]), loaded in place of
+// loss_grad_kernel's loss gradient: bf16 NHWC with `ld` channels per pixel (the padded A operand of the final conv's data / weight
+// gradient; the padding channels and padded images are not touched and stay zero) and bias_sum [C] += its sums, taken from the unrounded
+// fp32 values.
+__global__ void __launch_bounds__(256) grad_load_kernel(const float* __restrict__ g_in, int B, int C, int H, int W, __nv_bfloat16* __restrict__ deps,
+                                                        int ld, float* __restrict__ bias_sum) {
+    const long long n = static_cast<long long>(B) * C * H * W;
+    for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n; i += static_cast<long long>(gridDim.x) * blockDim.x) {
+        const float g = g_in[i];
+        long long r = i;
+        const int w = static_cast<int>(r % W); r /= W;
+        const int h = static_cast<int>(r % H); r /= H;
+        const int c = static_cast<int>(r % C);
+        const int b = static_cast<int>(r / C);
+        deps[((static_cast<long long>(b) * H + h) * W + w) * ld + c] = __float2bfloat16_rn(g);
+        if ((H * W) & 31) {                            // a 4x4 image: (b, c) changes inside a warp
+            atomicAdd(&bias_sum[c], g);
+            continue;
+        }
+        float gs = g;                                  // H * W is a multiple of 32: the lanes of a warp share (b, c)
+#pragma unroll
+        for (int o = 16; o; o >>= 1) gs += __shfl_xor_sync(0xffffffffu, gs, o);
+        if ((threadIdx.x & 31) == 0) atomicAdd(&bias_sum[c], gs);
+    }
+}
+// The input gradient: channels [0, C) of the fp32 NHWC data gradient of the first conv (ld channels per pixel) -> fp32 NCHW [B][C][H][W]
+__global__ void __launch_bounds__(256) input_grad_store_kernel(const float* __restrict__ src, int B, int C, int H, int W, int ld, float* __restrict__ dst) {
+    const long long n = static_cast<long long>(B) * C * H * W;
+    for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n; i += static_cast<long long>(gridDim.x) * blockDim.x) {
+        long long r = i;
+        const int w = static_cast<int>(r % W); r /= W;
+        const int h = static_cast<int>(r % H); r /= H;
+        const int c = static_cast<int>(r % C);
+        const int b = static_cast<int>(r / C);
+        dst[i] = src[((static_cast<long long>(b) * H + h) * W + w) * ld + c];
     }
 }
 __global__ void scale_vec_kernel(const float* __restrict__ src, float* __restrict__ dst, int n, float s) {

@@ -91,6 +91,34 @@ class _Node(nn.Module):
     """Anonymous container used to reproduce the reference's dotted state_dict names."""
 
 
+class _UNetFn(torch.autograd.Function):
+    """UNet.forward as one autograd node on a training engine: forward = sr3_train_unet_forward (every intermediate kept), backward =
+    sr3_train_unet_backward from the upstream gradient of eps -> gradients of x, of the noise level and of every parameter."""
+
+    @staticmethod
+    def forward(ctx, unet, eng, x, time, seed, *params):
+        eps, ctx.fwd = eng.train_unet_forward(x, time, seed)
+        ctx.eng = eng
+        order = getattr(eng, "_param_order", None)          # parameters in the engine's (= the reference's state_dict) order, cached per engine
+        if order is None:
+            by_name = dict(unet.named_parameters())
+            order = eng._param_order = [by_name[n] for n, _ in eng.param_table()]
+        ctx.order = order
+        ctx.params = params
+        ctx.time_shape = time.shape
+        return eps
+
+    @staticmethod
+    def backward(ctx, deps):
+        if torch.is_grad_enabled():
+            raise RuntimeError("sr3_b200: double backward (create_graph=True) through the native UNet is not supported")
+        grads = {id(p): torch.empty_like(p, memory_format=torch.contiguous_format) for p in ctx.order}
+        dx, dnl = ctx.eng.train_unet_backward(deps, [grads[id(p)] for p in ctx.order], want_dx=ctx.needs_input_grad[2],
+                                              want_dnl=ctx.needs_input_grad[3], forward=ctx.fwd)
+        return (None, None, dx, None if dnl is None else dnl.view(ctx.time_shape), None) + \
+            tuple(grads[id(p)] if p.requires_grad else None for p in ctx.params)
+
+
 class UNet(nn.Module):
     def __init__(self, in_channel=6, out_channel=3, inner_channel=32, norm_groups=32, channel_mults=(1, 2, 4, 8, 8), attn_res=(8),
                  res_blocks=3, dropout=0, with_noise_level_emb=True, image_size=128, precision="bf16"):
@@ -119,6 +147,7 @@ class UNet(nn.Module):
         self._engine_versions: Dict[tuple, int] = {}
         self._schedule = None
         self._manual_version = 0
+        self._differentiable = False
 
     # torch's default Conv2d / Linear initialisation, drawn in the reference's construction order so that
     # torch.manual_seed(s) yields bit-identical weights in both implementations.
@@ -215,12 +244,26 @@ class UNet(nn.Module):
             self._engine_versions[key] = ver
         return eng
 
+    def set_differentiable(self, flag=True):
+        """Make forward() differentiable with respect to the parameters even when neither x nor time requires grad (losses on the
+        parameters alone).  Off by default: see forward()."""
+        self._differentiable = bool(flag)
+        return self
+
     def forward(self, x, time):
         """x [B,in_channel,H,W] fp32, time = noise level [B,1] -> eps [B,out_channel,H,W] (unet.py:235-259).  H x W is any size
-        _native.check_image_size accepts; attention stays on the levels image_size placed it on."""
-        if torch.is_grad_enabled() and x.requires_grad:
-            raise NotImplementedError("sr3_b200: backward through the native UNet is not implemented yet (inference / loss value only)")
+        _native.check_image_size accepts; attention stays on the levels image_size placed it on.
+
+        With grad mode on and x or time requiring grad (or after set_differentiable(True)) eps carries a grad_fn: the forward runs on the
+        bf16 training plan (intermediates kept; Dropout(self.dropout) in train() mode, seeded from torch's RNG) and backward() gives the
+        gradients of x, time and every parameter that requires grad.  Otherwise it runs the inference plan and returns a plain tensor."""
         a = self.arch
-        eng = self.engine(x.shape[0], conditional=a["in_channel"] != a["out_channel"], channels=a["out_channel"], height=x.shape[2],
-                          width=x.shape[3])
+        cond = a["in_channel"] != a["out_channel"]
+        wants_grad = self._differentiable or x.requires_grad or (torch.is_tensor(time) and time.requires_grad)
+        if torch.is_grad_enabled() and wants_grad:
+            drop = float(self.dropout or 0) if self.training else 0.0
+            eng = self.engine(x.shape[0], conditional=cond, channels=a["out_channel"], train_dropout=drop, height=x.shape[2], width=x.shape[3])
+            seed = int(torch.randint(0, 2 ** 62, (1,)).item())
+            return _UNetFn.apply(self, eng, x, time, seed, *self.parameters())
+        eng = self.engine(x.shape[0], conditional=cond, channels=a["out_channel"], height=x.shape[2], width=x.shape[3])
         return eng.unet_forward(x, time)

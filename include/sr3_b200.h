@@ -103,7 +103,7 @@ int sr3_p_sample(sr3_engine* e, const float* x, const float* condition_x, int t,
 /* p_losses forward (diffusion.py:221-246) with the random draws injected: hr = x_in['HR'] [B,3,H,W], sr = x_in['SR'] (NULL when
  * unconditional), gamma [B] = continuous_sqrt_alpha_cumprod, noise [B,3,H,W] (all DEVICE fp32).  q_sample (diffusion.py:212-219),
  * the UNet and the summed L1 (loss_type 1) / L2 (2) loss (diffusion.py:84-90) run natively; *loss_host receives the scalar.
- * Forward value only: the backward pass is not implemented. */
+ * Forward value only: gradients come from the training entry points below. */
 int sr3_p_losses(sr3_engine* e, const float* hr, const float* sr, const float* gamma, const float* noise, int loss_type, double* loss_host,
                  void* stream);
 
@@ -128,6 +128,16 @@ int sr3_train_forward(sr3_engine* e, const float* hr, const float* sr, const flo
  * sr3_engine_param_info order, n_grads == sr3_engine_num_params) is OVERWRITTEN with grad_scale * d(summed loss)/d(parameter i)
  * (grad_scale = 1 / (b c h w) reproduces model.py:50-53).  One backward per forward. */
 int sr3_train_backward(sr3_engine* e, float grad_scale, float* const* grads, int n_grads, void* stream);
+/* UNet.forward (model/sr3_modules/unet.py:235-259) in training form, on a training engine: x [B,in_channel,H,W] (for a conditional net the
+ * already concatenated cat(cond, x_t)), noise_level [B] -> eps [B,out_channel,H,W], all DEVICE fp32 NCHW.  Every intermediate is kept for
+ * sr3_train_unet_backward; Dropout as in sr3_train_forward (the plan's p, Philox keyed by dropout_seed, or the masks given to
+ * sr3_train_set_dropout_mask).  Like sr3_train_forward it replaces whatever forward the engine ran before. */
+int sr3_train_unet_forward(sr3_engine* e, const float* x, const float* noise_level, uint64_t dropout_seed, float* eps, void* stream);
+/* The backward of the sr3_train_unet_forward that just ran, for an upstream gradient deps = d(anything)/d eps (DEVICE fp32 NCHW, eps's
+ * shape; any scale is carried in deps).  grads as in sr3_train_backward (OVERWRITTEN, sr3_engine_param_info order).  dx [B,in_channel,H,W]
+ * and dnoise_level [B] (DEVICE fp32) receive the gradients of the input and of the noise level; either may be NULL, and is then not
+ * computed at all.  One backward per forward. */
+int sr3_train_unet_backward(sr3_engine* e, const float* deps, float* const* grads, int n_grads, float* dx, float* dnoise_level, void* stream);
 /* The same backward layer by layer, so that the caller can overlap the gradient all-reduce (SURVEY 8e, training row) with the layers still to
  * come: begin -> block n-1, n-2, ..., 0 -> finish (FiLM projections + noise-level MLP).  sr3_train_block_params lists the parameters whose
  * gradient is final once `block` has run AND sr3_train_backward_flush has been called (conv weight gradients leave the tensor-core kernel as
@@ -328,6 +338,17 @@ int sr3_test_film_embed_fwd(const float* nl, const float* w1, const float* b1, c
  * sum (eps - noise)^2 (l2 = 1); deps bf16 [B][H][W][ld] channels 0..C-1 = sign(d) or 2 d (the rest untouched); bias_sum [C] += its sums. */
 int sr3_test_loss_grad(const float* noise, const float* eps, int B, int C, int H, int W, int l2, double* loss_host, void* deps_bf16, int ld,
                        float* bias_sum, void* stream);
+/* grad_load_kernel, the start of sr3_train_unet_backward: g fp32 NCHW [B][C][H][W] -> deps bf16 [B][H][W][ld] channels 0..C-1 = bf16(g) (the
+ * rest untouched); bias_sum [C] += the fp32 sums of g. */
+int sr3_test_grad_load(const float* g, int B, int C, int H, int W, void* deps_bf16, int ld, float* bias_sum, void* stream);
+/* noise_level_bwd_kernel: the gradient of the noise level through the positional encoding and the noise-level MLP, given dtau [B][inner]
+ * (the gradient of its output): nl [B], w1 [4 inner][inner], b1 [4 inner], w2 [inner][4 inner] -> dnl [B]. */
+int sr3_test_noise_level_bwd(const float* nl, const float* w1, const float* b1, const float* w2, const float* dtau, float* dnl, int inner, int B,
+                             void* stream);
+/* The input gradient of sr3_train_unet_backward: the data gradient of the first conv (in_channel -> inner, 3x3, padding 1; w fp32 OIHW
+ * [inner][in_channel][3][3], packed on the device as the plan packs it) on the tile kernel, then the store of its first in_channel channels:
+ * dy bf16 NHWC [B][H][W][inner] -> dx fp32 NCHW [B][in_channel][H][W]. */
+int sr3_test_input_grad(const void* dy_bf16, const float* w_oihw, float* dx, int B, int H, int W, int inner, int in_channel, void* stream);
 
 /* Timing harness for one conv shape on zero-filled buffers (kernel-tuning experiments): average ms over `reps` launches. */
 int sr3_bench_conv(int B, int H, int W, int Cin, int Cout, int ksize, int stride, int with_resid, int with_stats, int reps, float* ms_out);
