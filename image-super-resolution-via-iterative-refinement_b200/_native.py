@@ -87,6 +87,14 @@ _SIGS = {
     "sr3_p_sample_loop_begin": (c_int, [c_void_p, c_void_p, c_void_p, c_uint64, c_uint64, c_void_p]),
     "sr3_p_sample_steps": (c_int, [c_void_p, c_int, c_int, c_void_p]),
     "sr3_read_state": (c_int, [c_void_p, c_void_p, c_void_p]),
+    "sr3_windowed_create": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, POINTER(c_void_p)]),
+    "sr3_windowed_destroy": (None, [c_void_p]),
+    "sr3_windowed_begin": (c_int, [c_void_p, c_void_p, c_void_p, c_uint64, c_uint64, c_void_p]),
+    "sr3_windowed_set_snapshots": (c_int, [c_void_p, c_void_p, c_int]),
+    "sr3_windowed_steps": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p]),
+    "sr3_windowed_read_state": (c_int, [c_void_p, c_void_p, c_void_p]),
+    "sr3_windowed_grid": (c_int, [c_void_p, POINTER(c_int), POINTER(c_int), POINTER(c_int), POINTER(c_int), POINTER(c_float), POINTER(c_float)]),
+    "sr3_windowed_profile_step": (c_int, [c_void_p, c_int, c_int, POINTER(c_float), c_void_p]),
     "sr3_engine_profile_step": (c_int, [c_void_p, c_int, c_int, c_int, POINTER(c_int), POINTER(c_float), POINTER(c_double), POINTER(c_double),
                                         POINTER(c_int), c_void_p]),
     "sr3_pil_bicubic_tables": (c_int, [c_int, c_int, POINTER(c_int), POINTER(c_int), c_int, POINTER(c_int)]),
@@ -556,6 +564,118 @@ class Engine:
         t = torch.empty(tuple(shape), device=self.device, dtype=torch.float32)
         _check(lib().sr3_engine_read_activation(self._h, name.encode(), _ptr(t), t.numel(), ctypes.byref(numel), shape, _stream()))
         return t.permute(0, 3, 1, 2).contiguous()
+
+
+def window_grid(length, side, overlap):
+    """Window origins along one axis of `length` pixels for windows of `side` pixels that overlap their neighbours by at least `overlap`:
+    one window when length == side, else n = ceil((length - overlap) / (side - overlap)) windows at round-half-up(i (length - side) / (n - 1)),
+    so the first starts at 0, the last ends at `length` and nothing lies outside.  Pure host arithmetic, the same as the native side's."""
+    length, side, overlap = int(length), int(side), int(overlap)
+    if length < side:
+        raise ValueError("canvas side %d is smaller than the window side %d (canvases are not padded)" % (length, side))
+    if not 0 <= overlap < side:
+        raise ValueError("overlap %d must be at least 0 and below the window side %d" % (overlap, side))
+    if length == side:
+        return [0]
+    n = -(-(length - overlap) // (side - overlap))
+    return [(2 * i * (length - side) + (n - 1)) // (2 * (n - 1)) for i in range(n)]
+
+
+def window_weights(n, side, overlap):
+    """Blend weights [n][side] (fp32) of the n windows of one axis: min(i + 1, side - i, ramp) / ramp with ramp = max(overlap, 1); the ramp
+    towards a border of the canvas, where no neighbour exists, is replaced by 1."""
+    ramp = max(int(overlap), 1)
+    i = torch.arange(side)
+    rows = []
+    for k in range(n):
+        m = torch.full((side,), ramp)
+        if k > 0:
+            m = torch.minimum(m, i + 1)
+        if k < n - 1:
+            m = torch.minimum(m, side - i)
+        rows.append(m.to(torch.float32) / float(ramp))
+    return torch.stack(rows)
+
+
+class WindowedSampler:
+    """A canvas [batch, C, height, width] sampled by overlapping windows of `engine`'s image size, merged inside every reverse step
+    (sr3_windowed_*).  Borrows the engine (engine.batch windows run per pass) and keeps it alive."""
+
+    def __init__(self, engine, batch, height, width, overlap_h, overlap_w):
+        self.engine = engine
+        self.device = engine.device
+        self.shape = (int(batch), engine.channels, int(height), int(width))
+        self.overlap = (int(overlap_h), int(overlap_w))
+        self._h = c_void_p()
+        with torch.cuda.device(self.device):
+            _check(lib().sr3_windowed_create(engine._h, *self.shape[:1], *self.shape[2:], *self.overlap, ctypes.byref(self._h)))
+        self._keep = None
+
+    def __del__(self):
+        try:
+            if getattr(self, "_h", None):
+                lib().sr3_windowed_destroy(self._h)
+                self._h = None
+        except Exception:
+            pass
+
+    def grid(self):
+        """(origins_y, origins_x, weights_y [ny, wh], weights_x [nx, ww]) as the native side built them."""
+        ny, nx = c_int(), c_int()
+        _check(lib().sr3_windowed_grid(self._h, ctypes.byref(ny), ctypes.byref(nx), None, None, None, None))
+        wh, ww = self.engine.height, self.engine.width
+        oy, ox = (c_int * ny.value)(), (c_int * nx.value)()
+        wy, wx = (c_float * (ny.value * wh))(), (c_float * (nx.value * ww))()
+        _check(lib().sr3_windowed_grid(self._h, ctypes.byref(ny), ctypes.byref(nx), oy, ox, wy, wx))
+        return list(oy), list(ox), torch.tensor(list(wy)).view(ny.value, wh), torch.tensor(list(wx)).view(nx.value, ww)
+
+    def _canvas(self, t, channels, what):
+        t = _f32c(t, self.device)
+        want = (self.shape[0], channels, self.shape[2], self.shape[3])
+        if tuple(t.shape) != want:
+            raise ValueError("%s has shape %s; this canvas is %s" % (what, tuple(t.shape), want))
+        return t
+
+    def begin(self, condition_x, x_T, seed=0, first_index=0):
+        c = None if condition_x is None else self._canvas(condition_x, self.engine.in_channel - self.engine.channels, "condition_x")
+        x_T = self._canvas(x_T, self.shape[1], "x_T")
+        with torch.cuda.device(self.device):
+            _check(lib().sr3_windowed_begin(self._h, _ptr(c), _ptr(x_T), int(seed), int(first_index), _stream()))
+
+    def steps(self, t_start, n, noises=None, snapshots=None):
+        """n canvas steps from timestep t_start down.  noises: [T, *canvas shape], noises[t] used at step t; snapshots: a CUDA fp32 tensor
+        [cap, *canvas shape] that receives x_{t-1} of every t with t % (1 | T // 10) == 0."""
+        if noises is not None:
+            noises = _f32c(noises, self.device)
+            if tuple(noises.shape) != (self.engine.T,) + self.shape:
+                raise ValueError("noises has shape %s; this canvas needs %s" % (tuple(noises.shape), (self.engine.T,) + self.shape))
+        self._keep = (noises, snapshots)
+        with torch.cuda.device(self.device):
+            _check(lib().sr3_windowed_set_snapshots(self._h, _ptr(snapshots), 0 if snapshots is None else snapshots.shape[0]))
+            _check(lib().sr3_windowed_steps(self._h, int(t_start), int(n), _ptr(noises), _stream()))
+
+    def read_state(self):
+        out = torch.empty(self.shape, device=self.device, dtype=torch.float32)
+        with torch.cuda.device(self.device):
+            _check(lib().sr3_windowed_read_state(self._h, _ptr(out), _stream()))
+        return out
+
+    def sample_loop(self, condition_x, x_T, noises=None, seed=0, first_index=0, want_snapshots=True):
+        """The whole reverse loop; returns (x_0, snapshots or None) like Engine.p_sample_loop."""
+        T = self.engine.T
+        inter = 1 | (T // 10)
+        cap = len([i for i in range(T) if i % inter == 0])
+        snaps = torch.empty((cap,) + self.shape, device=self.device, dtype=torch.float32) if want_snapshots else None
+        self.begin(condition_x, x_T, seed, first_index)
+        self.steps(T - 1, T, noises, snaps)
+        return self.read_state(), snaps
+
+    def profile_step(self, t, reps=3):
+        """{"gather", "engine", "merge"}: device ms per eager canvas step (CUDA events)."""
+        ms = (c_float * 3)()
+        with torch.cuda.device(self.device):
+            _check(lib().sr3_windowed_profile_step(self._h, int(t), int(reps), ms, _stream()))
+        return {"gather": ms[0], "engine": ms[1], "merge": ms[2]}
 
 
 def bench_conv(B, H, W, Cin, Cout, k=3, stride=1, resid=False, stats=True, reps=20):

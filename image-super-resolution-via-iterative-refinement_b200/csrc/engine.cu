@@ -22,6 +22,7 @@
 #include "attn_wgmma.cuh"
 #include "attn_long_wgmma.cuh"
 #include "train_kernels.cuh"
+#include "window_kernels.cuh"
 
 using namespace sr3;
 typedef __nv_bfloat16 bf16;
@@ -1805,27 +1806,31 @@ struct sr3_engine {
         CK(cudaDeviceSynchronize());
     }
 
+    // Records the ops of one step into the capture running on `main` (the noise-level embedding + FiLM projections on a forked branch).
+    void record_step(cudaStream_t main) {
+        const bool fork = side_begin > 0 && side_end > side_begin && side_join >= side_end;
+        if (fork && !side_stream) {
+            CK(cudaStreamCreateWithFlags(&side_stream, cudaStreamNonBlocking));
+            CK(cudaEventCreateWithFlags(&ev_fork, cudaEventDisableTiming));
+            CK(cudaEventCreateWithFlags(&ev_join, cudaEventDisableTiming));
+        }
+        for (int i = 0; i < (int)ops.size(); ++i) {
+            if (fork && i == side_begin) {              // branch: embed + film depend on the step prologue only
+                CK(cudaEventRecord(ev_fork, main));
+                CK(cudaStreamWaitEvent(side_stream, ev_fork, 0));
+            }
+            if (fork && i == side_join) {
+                CK(cudaEventRecord(ev_join, side_stream));
+                CK(cudaStreamWaitEvent(main, ev_join, 0));
+            }
+            ops[i](fork && i >= side_begin && i < side_end ? side_stream : main);
+        }
+    }
     void run_step(cudaStream_t st) {
         if (!graph) {
             cudaGraph_t g;
-            const bool fork = side_begin > 0 && side_end > side_begin && side_join >= side_end;
-            if (fork && !side_stream) {
-                CK(cudaStreamCreateWithFlags(&side_stream, cudaStreamNonBlocking));
-                CK(cudaEventCreateWithFlags(&ev_fork, cudaEventDisableTiming));
-                CK(cudaEventCreateWithFlags(&ev_join, cudaEventDisableTiming));
-            }
             CK(cudaStreamBeginCapture(cap_stream, cudaStreamCaptureModeThreadLocal));
-            for (int i = 0; i < (int)ops.size(); ++i) {
-                if (fork && i == side_begin) {              // branch: embed + film depend on the step prologue only
-                    CK(cudaEventRecord(ev_fork, cap_stream));
-                    CK(cudaStreamWaitEvent(side_stream, ev_fork, 0));
-                }
-                if (fork && i == side_join) {
-                    CK(cudaEventRecord(ev_join, side_stream));
-                    CK(cudaStreamWaitEvent(cap_stream, ev_join, 0));
-                }
-                ops[i](fork && i >= side_begin && i < side_end ? side_stream : cap_stream);
-            }
+            record_step(cap_stream);
             CK(cudaStreamEndCapture(cap_stream, &g));
             CK(cudaGraphInstantiate(&graph, g, 0));
             CK(cudaGraphDestroy(g));
@@ -1847,6 +1852,137 @@ struct sr3_engine {
         if (cfg.conditional) { REQUIRE(cond != nullptr, "condition_x is required by a conditional model"); load_nchw(cond, cond_c, 0, nullptr, st); }
         else REQUIRE(cond == nullptr, "condition_x given to an unconditional model");
         load_nchw(x, cfg.channels, cond_c, x_state, st);
+    }
+};
+
+// ------------------------------------------------------------------------------------------------ windowed sampling
+// Window origins along one axis of length L: one window when L == side, else n = ceil((L - overlap) / (side - overlap)) windows at
+// round-half-up(i (L - side) / (n - 1)) -- the first starts at 0, the last ends at L, neighbours overlap by at least `overlap`.
+static std::vector<int> window_origins(int L, int side, int overlap) {
+    std::vector<int> o(1, 0);
+    if (L == side) return o;
+    const int n = (L - overlap + (side - overlap) - 1) / (side - overlap);
+    o.resize(n);
+    for (int i = 0; i < n; ++i) o[i] = (int)((2LL * i * (L - side) + (n - 1)) / (2LL * (n - 1)));
+    return o;
+}
+// Blend weights [n][side] of the n windows of one axis: min(i + 1, side - i, ramp) / ramp with ramp = max(overlap, 1); the ramp towards a
+// border of the canvas (no neighbour there) is dropped, so a single window weighs 1 everywhere.
+static std::vector<float> window_weights(int n, int side, int overlap) {
+    const int ramp = std::max(overlap, 1);
+    std::vector<float> w((size_t)n * side);
+    for (int k = 0; k < n; ++k)
+        for (int i = 0; i < side; ++i) {
+            int m = ramp;
+            if (k > 0) m = std::min(m, i + 1);
+            if (k < n - 1) m = std::min(m, side - i);
+            w[(size_t)k * side + i] = (float)m / (float)ramp;
+        }
+    return w;
+}
+
+struct sr3_windowed {
+    sr3_engine* e = nullptr;               // borrowed: runs Bw = e->B windows of e->H x e->W per pass
+    int B = 0, H = 0, W = 0, N = 0;        // canvas batch and size; windows of all images
+    std::vector<int> oy, ox;
+    std::vector<float> wy, wx;
+    DevAllocs mem;
+    WindowGeom g{};
+    float *x = nullptr, *cond = nullptr, *noise = nullptr, *means = nullptr;
+    WindowCtl* ctl_dev = nullptr;
+    WindowCtl ctl{};
+    uint64_t seed = 0, first_index = 0;
+    float* snapshots = nullptr; int snapshot_cap = 0;
+    cudaGraphExec_t graph = nullptr;
+    cudaStream_t cap_stream = nullptr;
+
+    ~sr3_windowed() {
+        if (graph) cudaGraphExecDestroy(graph);
+        if (cap_stream) cudaStreamDestroy(cap_stream);
+    }
+    size_t canvas_elems() const { return (size_t)B * e->cfg.channels * H * W; }
+
+    void init(sr3_engine* eng, int batch, int height, int width, int overlap_h, int overlap_w) {
+        e = eng; B = batch; H = height; W = width;
+        const int wh = e->H, ww = e->W, C = e->cfg.channels;
+        // checked before anything is allocated
+        REQUIRE(B >= 1, "batch must be >= 1");
+        REQUIRE(H >= wh && W >= ww, "canvas %dx%d is smaller than the window %dx%d (canvases are not padded)", H, W, wh, ww);
+        REQUIRE(overlap_h >= 0 && overlap_h < wh && overlap_w >= 0 && overlap_w < ww, "overlap %dx%d must be at least 0 and below the window %dx%d",
+                overlap_h, overlap_w, wh, ww);
+        REQUIRE((long long)B * H * W < (1LL << 31) && (long long)H * W < (1LL << 31), "canvas too large");
+        oy = window_origins(H, wh, overlap_h); ox = window_origins(W, ww, overlap_w);
+        wy = window_weights((int)oy.size(), wh, overlap_h); wx = window_weights((int)ox.size(), ww, overlap_w);
+        N = B * (int)(oy.size() * ox.size());
+        CK(cudaSetDevice(e->dev));
+        const size_t cb = canvas_elems() * sizeof(float);
+        x = static_cast<float*>(mem.alloc(cb)); noise = static_cast<float*>(mem.alloc(cb));
+        if (e->cond_c) cond = static_cast<float*>(mem.alloc((size_t)B * e->cond_c * H * W * sizeof(float)));
+        means = static_cast<float*>(mem.alloc((size_t)N * C * wh * ww * sizeof(float)));
+        ctl_dev = static_cast<WindowCtl*>(mem.alloc(sizeof(WindowCtl)));
+        int* oyd = static_cast<int*>(mem.alloc(oy.size() * sizeof(int))); int* oxd = static_cast<int*>(mem.alloc(ox.size() * sizeof(int)));
+        float* wyd = static_cast<float*>(mem.alloc(wy.size() * sizeof(float))); float* wxd = static_cast<float*>(mem.alloc(wx.size() * sizeof(float)));
+        CK(cudaMemcpy(oyd, oy.data(), oy.size() * sizeof(int), cudaMemcpyHostToDevice));
+        CK(cudaMemcpy(oxd, ox.data(), ox.size() * sizeof(int), cudaMemcpyHostToDevice));
+        CK(cudaMemcpy(wyd, wy.data(), wy.size() * sizeof(float), cudaMemcpyHostToDevice));
+        CK(cudaMemcpy(wxd, wx.data(), wx.size() * sizeof(float), cudaMemcpyHostToDevice));
+        g.B = B; g.C = C; g.H = H; g.W = W; g.wh = wh; g.ww = ww; g.ny = (int)oy.size(); g.nx = (int)ox.size();
+        g.oy = oyd; g.ox = oxd; g.wy = wyd; g.wx = wxd;
+        CK(cudaStreamCreateWithFlags(&cap_stream, cudaStreamNonBlocking));
+    }
+
+    // One canvas step: advance the canvas timestep, then per pass of Bw windows gather -> the engine's step (mean-only form) -> store of
+    // the pass's means; then the merge.  Slots of the last pass beyond the window list repeat the last window (finite, never stored).
+    void begin_step(cudaStream_t st) { launch_k(step_begin_kernel, dim3(1), dim3(32), 0, st, static_cast<float4*>(nullptr), 0LL, &ctl_dev->step); }
+    void gather(int first, cudaStream_t st) {
+        WindowGather p{};
+        p.g = g; p.cond = cond; p.x = x; p.first = first; p.n_total = N; p.Bw = e->B;
+        p.in_buf = e->in_buf; p.in_ld = e->in_C * e->PW; p.cond_c = e->cond_c; p.lo_off = e->precise ? e->in_C : 0;
+        p.x_state = e->x_state; p.wctl = ctl_dev; p.ectl = e->ctl_dev;
+        const long long total = 1LL * e->B * g.wh * (g.ww / 4);
+        launch_k(window_gather_kernel, dim3((int)std::min<long long>((total + 255) / 256, num_sms() * 8LL)), dim3(256), 0, st, p);
+    }
+    void store_means(int first, cudaStream_t st) {
+        const size_t win = (size_t)g.C * g.wh * g.ww;
+        CK(cudaMemcpyAsync(means + first * win, e->mean_buf, std::min(e->B, N - first) * win * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    }
+    void merge(cudaStream_t st) {
+        WindowMerge m{};
+        m.g = g; m.means = means; m.x = x; m.noise = noise; m.tab = e->post_tab; m.tab_T = e->T_cap; m.ctl = ctl_dev;
+        const long long total = 1LL * B * H * W;
+        launch_k(window_merge_kernel, dim3((int)std::min<long long>((total + 255) / 256, num_sms() * 8LL)), dim3(256), 0, st, m);
+    }
+    void record_step(cudaStream_t st) {
+        begin_step(st);
+        for (int first = 0; first < N; first += e->B) {
+            gather(first, st);
+            e->record_step(st);
+            store_means(first, st);
+        }
+        merge(st);
+    }
+    void run_step(cudaStream_t st) {
+        if (!graph) {
+            cudaGraph_t gr;
+            CK(cudaStreamBeginCapture(cap_stream, cudaStreamCaptureModeThreadLocal));
+            record_step(cap_stream);
+            CK(cudaStreamEndCapture(cap_stream, &gr));
+            CK(cudaGraphInstantiate(&graph, gr, 0));
+            CK(cudaGraphDestroy(gr));
+        }
+        CK(cudaGraphLaunch(graph, st));
+    }
+    // Control blocks of a run of steps starting at timestep t: the engine computes clipped posterior means only (its own noise add is
+    // discarded: update_state = 0, z read from its zeroed noise buffer); the canvas block carries the timestep, the noise source and the key.
+    void push_ctl(int t, bool injected, cudaStream_t st) {
+        StepCtl& c = e->ctl; memset(&c, 0, sizeof(c));
+        c.nl_from_table = 1; c.out_mode = 1; c.write_mean = 1; c.update_state = 0; c.use_noise_buf = 1; c.clip = 1; c.t_next = t;
+        CK(cudaMemsetAsync(e->noise_buf, 0, e->img_bytes(), st));
+        e->push_ctl(st);
+        memset(&ctl, 0, sizeof(ctl));
+        ctl.step.t_next = t; ctl.step.use_noise_buf = injected ? 1 : 0; ctl.step.seed = seed; ctl.step.sample_offset = first_index;
+        ctl.snapshots = snapshots; ctl.snapshot_cap = snapshot_cap; ctl.T = e->T;
+        CK(cudaMemcpyAsync(ctl_dev, &ctl, sizeof(WindowCtl), cudaMemcpyHostToDevice, st));
     }
 };
 
@@ -2261,6 +2397,107 @@ int sr3_super_resolution_host(sr3_engine* e, const float* cond_host, const float
     if (rc) return rc;
     CK(cudaMemcpyAsync(final_host, e->x_state, ib, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
+    API_END
+}
+
+int sr3_windowed_create(sr3_engine* e, int batch, int height, int width, int overlap_h, int overlap_w, sr3_windowed** out) {
+    API_BEGIN
+    REQUIRE(e && out, "null argument");
+    std::unique_ptr<sr3_windowed> w(new sr3_windowed());
+    w->init(e, batch, height, width, overlap_h, overlap_w);
+    *out = w.release();
+    API_END
+}
+void sr3_windowed_destroy(sr3_windowed* w) { delete w; }
+int sr3_windowed_begin(sr3_windowed* w, const float* cond, const float* x_T, uint64_t seed, uint64_t first_index, void* stream) {
+    API_BEGIN
+    REQUIRE(w && x_T, "null argument");
+    REQUIRE(w->e->T > 0, "set_new_noise_schedule has not been called");
+    if (w->e->cfg.conditional) REQUIRE(cond != nullptr, "condition_x is required by a conditional model");
+    else REQUIRE(cond == nullptr, "condition_x given to an unconditional model");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    CK(cudaSetDevice(w->e->dev));
+    if (cond) CK(cudaMemcpyAsync(w->cond, cond, (size_t)w->B * w->e->cond_c * w->H * w->W * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    CK(cudaMemcpyAsync(w->x, x_T, w->canvas_elems() * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    w->seed = seed; w->first_index = first_index;
+    API_END
+}
+int sr3_windowed_set_snapshots(sr3_windowed* w, float* snapshots, int snapshot_cap) {
+    API_BEGIN
+    REQUIRE(w && snapshot_cap >= 0 && (snapshots || snapshot_cap == 0), "bad snapshot buffer");
+    w->snapshots = snapshots; w->snapshot_cap = snapshot_cap;
+    API_END
+}
+int sr3_windowed_steps(sr3_windowed* w, int t_start, int steps, const float* noises, void* stream) {
+    API_BEGIN
+    REQUIRE(w, "null argument");
+    sr3_engine* e = w->e;
+    REQUIRE(t_start < e->T && steps >= 0 && t_start - steps + 1 >= 0, "bad step range t_start=%d steps=%d T=%d", t_start, steps, e->T);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    CK(cudaSetDevice(e->dev));
+    e->check_params();
+    w->push_ctl(t_start, noises != nullptr, st);
+    const size_t n = w->canvas_elems();
+    for (int i = 0; i < steps; ++i) {
+        if (noises) CK(cudaMemcpyAsync(w->noise, noises + (size_t)(t_start - i) * n, n * sizeof(float), cudaMemcpyDeviceToDevice, st));
+        w->run_step(st);
+    }
+    API_END
+}
+int sr3_windowed_read_state(sr3_windowed* w, float* x_out, void* stream) {
+    API_BEGIN
+    REQUIRE(w && x_out, "null argument");
+    CK(cudaMemcpyAsync(x_out, w->x, w->canvas_elems() * sizeof(float), cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(stream)));
+    API_END
+}
+int sr3_windowed_grid(const sr3_windowed* w, int* ny, int* nx, int* origins_y, int* origins_x, float* weights_y, float* weights_x) {
+    API_BEGIN
+    REQUIRE(w && ny && nx, "null argument");
+    *ny = (int)w->oy.size(); *nx = (int)w->ox.size();
+    if (origins_y) memcpy(origins_y, w->oy.data(), w->oy.size() * sizeof(int));
+    if (origins_x) memcpy(origins_x, w->ox.data(), w->ox.size() * sizeof(int));
+    if (weights_y) memcpy(weights_y, w->wy.data(), w->wy.size() * sizeof(float));
+    if (weights_x) memcpy(weights_x, w->wx.data(), w->wx.size() * sizeof(float));
+    API_END
+}
+// Eager (non-graph) canvas steps at timestep t with CUDA events around the gathers, the engine passes and the merge: ms[3] = their device
+// time per step, averaged over `reps` steps after one warm-up.  Overwrites the canvas state with the steps' results.
+int sr3_windowed_profile_step(sr3_windowed* w, int t, int reps, float* ms, void* stream) {
+    API_BEGIN
+    REQUIRE(w && ms && reps >= 1, "bad argument");
+    sr3_engine* e = w->e;
+    REQUIRE(e->T > 0 && t >= 0 && t < e->T, "bad t");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    CK(cudaSetDevice(e->dev));
+    const int Bw = e->B, passes = (w->N + Bw - 1) / Bw;
+    std::vector<cudaEvent_t> ev(3 * passes + 2);
+    for (auto& x : ev) CK(cudaEventCreate(&x));
+    double acc[3] = {0, 0, 0};
+    for (int r = 0; r < reps + 1; ++r) {
+        w->push_ctl(t, false, st);
+        w->begin_step(st);
+        for (int pi = 0; pi < passes; ++pi) {
+            CK(cudaEventRecord(ev[3 * pi], st));
+            w->gather(pi * Bw, st);
+            CK(cudaEventRecord(ev[3 * pi + 1], st));
+            for (auto& op : e->ops) op(st);
+            CK(cudaEventRecord(ev[3 * pi + 2], st));
+            w->store_means(pi * Bw, st);
+        }
+        CK(cudaEventRecord(ev[3 * passes], st));
+        w->merge(st);
+        CK(cudaEventRecord(ev[3 * passes + 1], st));
+        CK(cudaStreamSynchronize(st));
+        if (r == 0) continue;
+        float v = 0;
+        for (int pi = 0; pi < passes; ++pi) {
+            CK(cudaEventElapsedTime(&v, ev[3 * pi], ev[3 * pi + 1])); acc[0] += v;
+            CK(cudaEventElapsedTime(&v, ev[3 * pi + 1], ev[3 * pi + 2])); acc[1] += v;
+        }
+        CK(cudaEventElapsedTime(&v, ev[3 * passes], ev[3 * passes + 1])); acc[2] += v;
+    }
+    for (int k = 0; k < 3; ++k) ms[k] = (float)(acc[k] / reps);
+    for (auto& x : ev) cudaEventDestroy(x);
     API_END
 }
 

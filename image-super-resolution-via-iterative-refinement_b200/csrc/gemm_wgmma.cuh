@@ -29,6 +29,7 @@
 #include <cuda.h>
 #include <type_traits>
 #include "ptx.cuh"
+#include "sampling_noise.cuh"
 
 namespace sr3 {
 
@@ -167,26 +168,6 @@ __host__ __device__ constexpr int gemm_smem_bytes(int block_n, int a_stage_bytes
     return stages * gemm_stage_bytes(block_n, a_stage_bytes, b_taps) + gemm_epi_bytes(resid) + 1024 /*align slack*/ + gemm_aux_bytes(num_k);
 }
 
-// ---------------------------------------------------------------- Philox4x32-10 + Box-Muller
-__device__ __forceinline__ void philox4x32_10(uint32_t (&c)[4], uint32_t k0, uint32_t k1) {
-#pragma unroll
-    for (int r = 0; r < 10; ++r) {
-        const uint32_t hi0 = __umulhi(0xD2511F53u, c[0]), lo0 = 0xD2511F53u * c[0];
-        const uint32_t hi1 = __umulhi(0xCD9E8D57u, c[2]), lo1 = 0xCD9E8D57u * c[2];
-        const uint32_t n0 = hi1 ^ c[1] ^ k0, n1 = lo1, n2 = hi0 ^ c[3] ^ k1, n3 = lo0;
-        c[0] = n0; c[1] = n1; c[2] = n2; c[3] = n3;
-        k0 += 0x9E3779B9u; k1 += 0xBB67AE85u;
-    }
-}
-__device__ __forceinline__ void box_muller(uint32_t a, uint32_t b, float& z0, float& z1) {
-    const float u1 = (static_cast<float>(a) + 1.0f) * 2.3283064365386963e-10f;   // (0, 1]
-    const float u2 = static_cast<float>(b) * 2.3283064365386963e-10f;            // [0, 1)
-    const float r = sqrtf(-2.0f * logf(u1));
-    float s, c;
-    sincospif(2.0f * u2, &s, &c);
-    z0 = r * c; z1 = r * s;
-}
-
 // GroupNorm statistics are accumulated with fp64 atomics.  Every contribution is first rounded to a multiple of 2^-20, so as long as
 // a sum stays below 2^33 (|x|_rms < 180 over a 512x512 channel) every addition is EXACT: the result does not depend on the order in
 // which the CTAs arrive -- repeat runs are bit identical -- and E[x^2] - mean^2 is evaluated in fp64 by the consumer (no fp32
@@ -227,12 +208,13 @@ __device__ __forceinline__ void final_epilogue(const GemmParams& p, const float 
     }
     const int t = ctl.t_cur;
     const float c1 = q.tab[t], c2 = q.tab[q.T + t], pc1 = q.tab[2 * q.T + t], pc2 = q.tab[3 * q.T + t];
-    const float sigma = (t > 0) ? expf(0.5f * q.tab[4 * q.T + t]) : 0.0f;
+    const float sigma = posterior_sigma(q.tab, q.T, t);
     float z[4] = {0.f, 0.f, 0.f, 0.f};
     if (t > 0) {
         if (ctl.use_noise_buf) {
             for (int c = 0; c < q.C; ++c) z[c] = q.noise_buf[(static_cast<long long>(img) * q.C + c) * plane + pix];
         } else {
+            // (sampling_noise4 of sampling_noise.cuh, spelled out: this kernel's code is kept instruction for instruction)
             uint32_t ctr[4] = {static_cast<uint32_t>(pix), static_cast<uint32_t>(ctl.sample_offset + img), static_cast<uint32_t>(t),
                                static_cast<uint32_t>((ctl.sample_offset + img) >> 32)};
             philox4x32_10(ctr, static_cast<uint32_t>(ctl.seed), static_cast<uint32_t>(ctl.seed >> 32));
@@ -247,7 +229,7 @@ __device__ __forceinline__ void final_epilogue(const GemmParams& p, const float 
         if (ctl.clip) x0 = fminf(fmaxf(x0, -1.0f), 1.0f);
         const float mean = __fadd_rn(__fmul_rn(pc1, x0), __fmul_rn(pc2, xt));
         if (ctl.write_mean) q.mean_out[idx] = mean;
-        const float xn = __fadd_rn(mean, __fmul_rn(z[c], sigma));
+        const float xn = posterior_sample(mean, z[c], sigma);
         if (ctl.update_state) {
             q.x_state[idx] = xn;
             __nv_bfloat16* ib = q.in_buf + (static_cast<long long>(img) * plane + pix) * q.in_C + q.in_coff + c;

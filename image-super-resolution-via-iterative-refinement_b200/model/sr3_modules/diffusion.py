@@ -156,6 +156,64 @@ class GaussianDiffusion(nn.Module):
     def super_resolution(self, x_in, continous=False, **kw):
         return self.p_sample_loop(x_in, continous, **kw)
 
+    # ---- windowed sampling: canvases of any size, see DESIGN.md 3.9
+    WINDOW_PASS_SIZES = (16, 8, 4, 2, 1)      # windows per engine pass: the largest one not above the window count whose engine fits
+
+    def _windowed_sampler(self, batch, height, width, window=None, overlap=None):
+        """The canvas sampler for [batch, C, height, width] (sr3_windowed_*).  Every argument is checked before anything is allocated:
+        `window` by _native.check_image_size (UnsupportedSizeError), then the overlaps and the canvas size (ValueError)."""
+        from ... import _native
+        wh, ww = (self.image_size, self.image_size) if window is None else (int(window[0]), int(window[1]))
+        _native.check_image_size(len(self.denoise_fn.arch["channel_mults"]), wh, ww)
+        if overlap is None:
+            overlap = (wh // 4, ww // 4)
+        ovh, ovw = (int(overlap), int(overlap)) if isinstance(overlap, int) else (int(overlap[0]), int(overlap[1]))
+        for ov, side in ((ovh, wh), (ovw, ww)):
+            if not 0 <= ov < side:
+                raise ValueError("overlap %d must be at least 0 and below the window side %d" % (ov, side))
+        if height < wh or width < ww:
+            raise ValueError("canvas %dx%d is smaller than the window %dx%d (canvases are not padded)" % (height, width, wh, ww))
+        n = batch * len(_native.window_grid(height, wh, ovh)) * len(_native.window_grid(width, ww, ovw))
+        sizes = [s for s in self.WINDOW_PASS_SIZES if s <= n] or [min(self.WINDOW_PASS_SIZES)]
+        eng = None
+        for i, bw in enumerate(sizes):
+            try:
+                eng = self._engine(bw, wh, ww)
+                break
+            except RuntimeError as e:          # an engine of this batch does not fit the device: run fewer windows per pass
+                if "out of memory" not in str(e) or i == len(sizes) - 1:
+                    raise
+        key = (batch, height, width, ovh, ovw)
+        cached = getattr(self, "_windowed", None)
+        if cached is None or cached[0] != key or cached[1].engine is not eng:
+            self._windowed = None              # release the previous canvas before the new one is allocated
+            self._windowed = cached = (key, _native.WindowedSampler(eng, batch, height, width, ovh, ovw))
+        return cached[1]
+
+    @torch.no_grad()
+    def super_resolution_windowed(self, x_in, window=None, overlap=None, continous=False, x_T=None, noises=None, seed=None, first_index=0):
+        """super_resolution for a conditioning image x_in [B, C, H, W] of ANY size H >= window height, W >= window width: the UNet runs on
+        overlapping `window` = (wh, ww) crops (default image_size x image_size; any size _native.check_image_size accepts) whose posterior
+        means are blended on the canvas inside every reverse step, so there is one x_t and one noise draw per canvas pixel and no seam.
+        `overlap`: least overlap of neighbouring windows in pixels, an int or (rows, columns), default a quarter of the window side.
+        With window == (H, W) this is super_resolution bit for bit.  Return conventions and the extra keyword arguments are
+        p_sample_loop's."""
+        device = self.betas.device
+        if not self.conditional:
+            shape, cond = tuple(x_in), None
+        else:
+            cond = x_in.to(device)
+            shape = tuple(cond.shape)
+        sampler = self._windowed_sampler(shape[0], shape[2], shape[3], window, overlap)
+        img = torch.randn(shape, device=device) if x_T is None else x_T.to(device)
+        if seed is None:
+            seed = int(torch.randint(0, 2 ** 62, (1,)).item())
+        final, snaps = sampler.sample_loop(cond, img, noises, seed, first_index, want_snapshots=continous)
+        if continous:
+            first = cond if self.conditional else img
+            return torch.cat([first, snaps.reshape(-1, *shape[1:])], dim=0)
+        return final[-1]
+
     def q_sample(self, x_start, continuous_sqrt_alpha_cumprod, noise=None):
         noise = torch.randn_like(x_start) if noise is None else noise
         return continuous_sqrt_alpha_cumprod * x_start + (1 - continuous_sqrt_alpha_cumprod ** 2).sqrt() * noise

@@ -58,12 +58,16 @@ def sharded_sample(sample_fn: Callable[[Optional[torch.Tensor], torch.Tensor, in
     return gather_shards(local, n, group)
 
 
-def sharded_super_resolution(netG, x_in: torch.Tensor, x_T: Optional[torch.Tensor] = None, seed: int = 0, group=None) -> torch.Tensor:
+def sharded_super_resolution(netG, x_in: torch.Tensor, x_T: Optional[torch.Tensor] = None, seed: int = 0, group=None, window=None,
+                             overlap=None) -> torch.Tensor:
     """Batch-sharded `GaussianDiffusion.super_resolution` (reference: model/sr3_modules/diffusion.py:176-210 run on GPU 0 only,
     model/model.py:60-78): returns the [B,3,H,W] finished images x_0 on every rank, at the size of `x_in` (any size the engine accepts).
 
     `x_in` / `x_T` are the GLOBAL (host or device) tensors; each rank copies and samples only its slice; the Philox noise streams are keyed
-    by the global sample index (`first_index`), so the images do not depend on the number of ranks."""
+    by the global sample index (`first_index`), so the images do not depend on the number of ranks.
+
+    `window` / `overlap` (either one given): every rank runs `GaussianDiffusion.super_resolution_windowed`'s loop on its slice instead, for
+    `x_in` of any size; its noise is keyed by the global sample index and the pixel's index in the canvas, so this too is rank independent."""
     dev = netG.betas.device
     if x_T is None:
         g = torch.Generator().manual_seed(seed)
@@ -72,6 +76,9 @@ def sharded_super_resolution(netG, x_in: torch.Tensor, x_T: Optional[torch.Tenso
     def fn(c, xt, first):
         if c.shape[0] == 0:
             return torch.empty((0,) + tuple(xt.shape[1:]), device=dev)
+        if window is not None or overlap is not None:
+            sampler = netG._windowed_sampler(c.shape[0], c.shape[2], c.shape[3], window, overlap)
+            return sampler.sample_loop(c.to(dev, non_blocking=True), xt.to(dev, non_blocking=True), None, seed, first, want_snapshots=False)[0]
         # images of the net's image_size keep the plain `_engine(batch)` call (all a stand-in net without an image_size offers); other
         # sizes name theirs
         size, image_size = tuple(c.shape[2:]), getattr(netG, "image_size", None)

@@ -180,6 +180,38 @@ int sr3_p_sample_loop_begin(sr3_engine* e, const float* condition_x, const float
 int sr3_p_sample_steps(sr3_engine* e, int t_start, int steps, void* stream);
 int sr3_read_state(sr3_engine* e, float* x_out, void* stream);
 
+/* ---- windowed sampling: super-resolve a canvas of ANY size H >= window height, W >= window width with an engine of a supported window
+ * size.  Each image of the canvas [B,3,H,W] is covered by overlapping windows (per axis: one window when the side equals the window's, else
+ * n = ceil((L - overlap) / (side - overlap)) windows at origins round-half-up(i (L - side) / (n - 1))); the windows of all images form one list,
+ * walked in passes of the engine's batch.  Every reverse step t merges the windows on the canvas:
+ *   mean(p)    = sum_n w_n(p) mean_n(p) / sum_n w_n(p)   over the windows covering p in ascending index, fp32, mean_n = the clipped posterior
+ *                mean of p_mean_variance on the window's crops of x_t and the condition;
+ *   x_{t-1}(p) = mean(p) + exp(0.5 logvar_t) z(p)  (t > 0),  z from Philox keyed by (seed, first_sample_index + b, pixel index IN THE CANVAS, t)
+ *                or from `noises`.
+ * w_n(p) = wy(y) wx(x), w(i) = min(i + 1, side - i, ramp) / ramp with ramp = max(overlap, 1), the ramp towards a canvas border dropped.
+ * A canvas of the window's size has one window of weight 1 and reproduces sr3_p_sample_loop bit for bit.  The result does not depend on the
+ * engine's batch, and repeat runs are bit identical.  A whole canvas step is one CUDA graph (captured at the first step).
+ * The canvas object owns the canvas state, a copy of the condition, the window means, the tables and the graph; it BORROWS the engine, which
+ * must outlive it and must not run anything else between sr3_windowed_steps calls that belong together. */
+typedef struct sr3_windowed sr3_windowed;
+/* Fails before any allocation when the canvas is smaller than the engine's image size or an overlap is not in [0, side). */
+int sr3_windowed_create(sr3_engine* e, int batch, int height, int width, int overlap_h, int overlap_w, sr3_windowed** out);
+void sr3_windowed_destroy(sr3_windowed* w);
+/* condition_x, x_T: DEVICE [B,3,H,W] (copied); as sr3_p_sample_loop_begin. */
+int sr3_windowed_begin(sr3_windowed* w, const float* condition_x, const float* x_T, uint64_t seed, uint64_t first_sample_index, void* stream);
+/* Where the following steps keep x_{t-1} of every t with t % (1 | T/10) == 0 (the `continous=True` images): DEVICE [snapshot_cap][B,3,H,W]
+ * owned by the caller, first kept image first; NULL / 0: none. */
+int sr3_windowed_set_snapshots(sr3_windowed* w, float* snapshots, int snapshot_cap);
+/* `steps` canvas steps from timestep t_start down, graph launches only.  noises: optional DEVICE [T][B,3,H,W], noises[t] used at step t. */
+int sr3_windowed_steps(sr3_windowed* w, int t_start, int steps, const float* noises, void* stream);
+int sr3_windowed_read_state(sr3_windowed* w, float* x_out, void* stream);
+/* The window grid: *ny, *nx windows per axis; optional HOST outputs origins_y [ny], origins_x [nx], weights_y [ny][window height],
+ * weights_x [nx][window width]. */
+int sr3_windowed_grid(const sr3_windowed* w, int* ny, int* nx, int* origins_y, int* origins_x, float* weights_y, float* weights_x);
+/* Profiling: eager canvas steps at timestep t (Philox noise), CUDA events around the launches; ms[3] = device time per step of the gathers,
+ * of the engine passes and of the merge, averaged over `reps` steps after one warm-up.  Advances the canvas state. */
+int sr3_windowed_profile_step(sr3_windowed* w, int t, int reps, float* ms, void* stream);
+
 /* core/metrics.py:8-34 `tensor2img` on the device: src fp32 DEVICE [n][C][H][W] -> clamp to [min_v, max_v] -> [0, 1] -> * 255, round half
  * to even -> uint8 DEVICE, HWC.  n == 1: dst [H][W][C].  n > 1: the images are tiled like torchvision.utils.make_grid(nrow, padding 2,
  * pad_value 0), which is what the reference does for 4-D input: dst [rows*(H+2)+2][cols*(W+2)+2][C], cols = min(nrow, n).
