@@ -67,6 +67,7 @@ _SIGS = {
     "sr3_train_block_params": (c_int, [c_void_p, c_int, POINTER(c_int), c_int, POINTER(c_int)]),
     "sr3_train_backward_profile": (c_int, [c_void_p, c_float, POINTER(c_void_p), c_int, POINTER(c_float), c_void_p]),
     "sr3_train_set_dropout_mask": (c_int, [c_void_p, c_char_p, c_void_p]),
+    "sr3_test_train_film_state": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_int), POINTER(c_int), c_void_p]),
     "sr3_train_num_dropout_layers": (c_int, [c_void_p]),
     "sr3_train_dropout_layer_name": (c_int, [c_void_p, c_int, c_char_p, c_int]),
     "sr3_adam_step": (c_int, [c_void_p, c_int, c_float, c_float, c_float, c_float, c_int, c_float, c_void_p]),
@@ -213,6 +214,7 @@ class Engine:
         self.channels = cfg["channels"]
         self.in_channel = cfg["in_channel"]
         self.out_channel = cfg["out_channel"]
+        self.inner_channel = cfg["inner_channel"]
         self.image_size = cfg["image_size"]
         self.height = int(cfg["image_size"] if height is None else height)
         self.width = int(cfg["image_size"] if width is None else width)
@@ -429,6 +431,19 @@ class Engine:
         with torch.cuda.device(self.device):
             _check(lib().sr3_train_unet_backward(self._h, _ptr(deps), arr, len(grads), _ptr(dx), _ptr(dnl), _stream()))
         return dx, dnl
+
+    def film_state(self):
+        """Tests: copies of the FiLM state of this training engine's latest forward and backward, one row per image the plan allocates
+        (the batch, padded): {"tau": [rows, inner], "dfilm": [rows, F], "dtau": [rows, inner]}.  sr3_test_train_film_state."""
+        rows, F = c_int(), c_int()
+        with torch.cuda.device(self.device):
+            _check(lib().sr3_test_train_film_state(self._h, None, None, None, ctypes.byref(rows), ctypes.byref(F), _stream()))
+            inner = self.inner_channel
+            out = {"tau": torch.empty(rows.value, inner, device=self.device), "dfilm": torch.empty(rows.value, F.value, device=self.device),
+                   "dtau": torch.empty(rows.value, inner, device=self.device)}
+            _check(lib().sr3_test_train_film_state(self._h, _ptr(out["tau"]), _ptr(out["dfilm"]), _ptr(out["dtau"]), ctypes.byref(rows),
+                                                   ctypes.byref(F), _stream()))
+        return out
 
     def train_backward_profile(self, grad_scale, grads):
         """{kind: ms} of one backward, CUDA events around every op."""

@@ -1739,6 +1739,10 @@ struct sr3_engine {
         CK(cudaGetDeviceProperties(&prop, dev));
         REQUIRE(prop.major == 9 && prop.minor == 0, "sr3_b200 needs an sm_90 GPU (found sm_%d%d); there is no fallback path", prop.major, prop.minor);
         REQUIRE(cfg.inner_channel % 64 == 0, "inner_channel must be a multiple of 64 (got %d)", cfg.inner_channel);
+        // the FiLM / noise-level MLP backward holds every image's embedding in one block's shared memory: refuse a training batch it
+        // cannot hold now, not at the end of the first backward
+        REQUIRE(!train || (film_bwd_smem(B, cfg.inner_channel) <= FILM_BWD_SMEM_MAX && embed_bwd_smem(B, cfg.inner_channel) <= FILM_BWD_SMEM_MAX),
+                "FiLM / noise-level MLP backward: batch %d too large for one block's shared memory", B);
         REQUIRE(cfg.in_channel <= 64, "in_channel must be <= 64");
         for (int i = 0; i < cfg.n_mults; ++i) REQUIRE((cfg.inner_channel * cfg.channel_mults[i]) % (2 * cfg.norm_groups) == 0 || (cfg.inner_channel * cfg.channel_mults[i]) % cfg.norm_groups == 0, "norm_groups must divide the channel counts");
         inner = cfg.inner_channel; H = height; W = width;
@@ -2140,6 +2144,19 @@ int sr3_train_set_dropout_mask(sr3_engine* e, const char* block_name, const unsi
     for (size_t i = 0; i < e->drop_names.size(); ++i)
         if (e->drop_names[i] == block_name) { e->drop_host[i].mask = mask_nchw; found = true; }
     REQUIRE(found, "no dropout layer named %s", block_name);
+    API_END
+}
+int sr3_test_train_film_state(const sr3_engine* e, float* tau, float* dfilm, float* dtau, int* rows, int* F, void* stream) {
+    API_BEGIN
+    REQUIRE(e && rows && F, "null argument");
+    REQUIRE(e->train, "engine was not created with sr3_engine_create_train");
+    *rows = e->Bp; *F = e->F;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    CK(cudaSetDevice(e->dev));
+    if (tau) CK(cudaMemcpyAsync(tau, e->tau, (size_t)e->Bp * e->inner * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    if (dfilm) CK(cudaMemcpyAsync(dfilm, e->dfilm, (size_t)e->Bp * e->F * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    if (dtau) CK(cudaMemcpyAsync(dtau, e->dtau, (size_t)e->Bp * e->inner * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    CK(cudaStreamSynchronize(st));
     API_END
 }
 int sr3_train_num_dropout_layers(const sr3_engine* e) { return e ? (int)e->drop_names.size() : 0; }

@@ -155,6 +155,12 @@ int sr3_train_backward_profile(sr3_engine* e, float grad_scale, float* const* gr
 /* Tests: replace the Philox dropout mask of ResnetBlock `block_name` ("downs.1.res_block.block2", the module that owns the nn.Dropout) by a
  * keep-mask, uint8 DEVICE [B][C][H][W] (1 = keep), e.g. the one the reference drew; NULL restores Philox. */
 int sr3_train_set_dropout_mask(sr3_engine* e, const char* block_name, const unsigned char* mask_nchw);
+/* Tests, read-only: the FiLM state of a training engine's latest forward and backward, copied into DEVICE fp32 buffers of *rows images
+ * (*rows = the batch the plan allocates: the batch, padded to even or, for a 4x4 lowest level, to a multiple of 8): tau [rows][inner] (the
+ * noise-level embedding), dfilm [rows][F] (the per-image channel sums of the gradient of every ResnetBlock's FiLM output, the blocks'
+ * slices in downs / mid / ups order, F their summed output channels) and dtau [rows][inner] (its gradient).  Any of the three may be NULL;
+ * *rows and *F are always written. */
+int sr3_test_train_film_state(const sr3_engine* e, float* tau, float* dfilm, float* dtau, int* rows, int* F, void* stream);
 int sr3_train_num_dropout_layers(const sr3_engine* e);
 int sr3_train_dropout_layer_name(const sr3_engine* e, int index, char* name, int name_cap);
 /* torch.optim.Adam(lr, betas, eps, weight_decay 0) step `step` (1-based) over a DEVICE table of n_tensors records

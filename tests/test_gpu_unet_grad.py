@@ -2,20 +2,22 @@
 set_differentiable(True)) runs the bf16 training plan, and backward() gives the gradients of x, the noise level and every parameter
 (sr3_train_unet_forward / sr3_train_unet_backward).
 
-Against the oracle's fp32 autograd on the CPU (itself pinned to the reference in tests/test_oracle_unet_grad.py): eps within 1e-2, dx and
-d noise_level within 2e-2 relative L2 over the batch, every parameter gradient within tests/test_gpu_train.py's bounds.  Also: equivalence
-with p_losses' backward, the three new kernels against fp64, the guards against stale or repeated backwards, and the unchanged default."""
+Against the oracle's fp32 autograd on the CPU (itself pinned to the reference in tests/test_oracle_unet_grad.py): eps within 1e-2, dx
+within 2e-2 relative L2 over the batch, d noise_level per image within the bound of dtau conditioned by Cauchy-Schwarz (compare), every
+parameter gradient within tests/test_gpu_train.py's bounds.  Also: equivalence with p_losses' backward, the three new kernels against
+fp64, the guards against stale or repeated backwards, and the unchanged default."""
 import numpy as np
 import pytest
 import torch
 
 import _train_util as tu
 import _unet_grad_inputs as ui
+from oracle import sr3_oracle as orc
 from test_oracle_unet_grad import golden, oracle_grads, unpack_masks  # noqa: F401  (golden: module fixture)
 
 pytestmark = pytest.mark.gpu
 EPS_TOL = 1e-2
-INPUT_TOL = 2e-2         # dx and d noise_level
+INPUT_TOL = 2e-2         # dx
 # relative L2 per parameter tensor.  tests/test_gpu_train.py holds loss gradients to 2e-2 (3e-2 for five-level nets); here the upstream
 # gradient is an arbitrary fp32 tensor that the load rounds to bf16 (an L1 / L2 loss gradient loses little or nothing there), and the
 # backward is not run-to-run reproducible (fp32 atomics, DESIGN.md §3.6): the unconditional case measured 1.84e-2 and 2.00e-2 in two runs.
@@ -44,40 +46,75 @@ def ours(net, x, nl, G, train_mode=False):
 
 
 def oracle_of(net, unet, name, x, nl, G, masks=None, p=0.0):
+    """oracle_grads, and dtau [B, inner]: the gradient reaching the output of the oracle's noise-level MLP (row b is what an oracle run on
+    image b alone gives as grad(noise_level_mlp.3.bias): the UNet is separable per image)."""
     _, image_size, _, _, _, _ = ui.ALL[name]
     sd = {k: v.detach().cpu() for k, v in net.denoise_fn.state_dict().items()}
     torch.set_num_threads(min(16, torch.get_num_threads()))
-    return oracle_grads(sd, tu.oracle_cfg(unet, image_size), x, nl, G, masks, p)
+    taus, mlp = [], orc.noise_level_mlp
+
+    def kept(*args):
+        t = mlp(*args)
+        t.retain_grad()
+        taus.append(t)
+        return t
+    orc.noise_level_mlp = kept
+    try:
+        r = oracle_grads(sd, tu.oracle_cfg(unet, image_size), x, nl, G, masks, p)
+    finally:
+        orc.noise_level_mlp = mlp
+    assert len(taus) == 1
+    return r + (taus[0].grad.reshape(x.shape[0], -1),)
 
 
-def compare(name, o, r, label=None):
+def dnl_bounds(sd, nl, rdtau):
+    """c_b = d tau_b / d noise_level_b [B, inner] in fp64 by forward-mode autograd through the oracle's noise-level MLP, and the per-image
+    scale ||c_b|| ||rdtau_b|| of the conditioned d noise_level bound."""
+    sd64 = {k: v.double() for k, v in sd.items() if k.startswith("noise_level_mlp.")}
+    inner = rdtau.shape[1]
+    n = nl.double().view(-1, 1)
+    _, c = torch.func.jvp(lambda t: orc.noise_level_mlp(sd64, t, inner).reshape(n.shape[0], inner), (n,), (torch.ones_like(n),))
+    return c, c.norm(dim=1) * rdtau.double().norm(dim=1)
+
+
+def compare(name, net, nl, o, r, label=None):
+    """eps and dx within EPS_TOL / INPUT_TOL relative L2, every parameter gradient within GRAD_TOL (FIVE_LEVEL_TOL), and d noise_level per
+    image within tol ||c_b|| ||dtau_b^ref||: by Cauchy-Schwarz on d noise_level_b = c_b^T dtau_b with dtau_b held to tol
+    (tests/test_gpu_noise_level_grad.py, test_noise_level_chain_matches_oracle).  A relative L2 bound over the batch's 2 or 3 scalars
+    is ill-conditioned: it is larger than the error of dtau by ||c_b|| ||dtau_b|| / |c_b^T dtau_b|, which grows without bound as c_b
+    and dtau_b turn orthogonal."""
     eps, dx, dnl, grads = o
-    reps, rdx, rdnl, rgrads = r
+    reps, rdx, rdnl, rgrads, rdtau = r
+    five = len(ui.ALL[name][0]["channel_multiplier"]) == 5
+    tol = FIVE_LEVEL_TOL if five else GRAD_TOL
+    _, scale = dnl_bounds({k: v.detach().cpu() for k, v in net.denoise_fn.state_dict().items()}, nl, rdtau)
+    dnl_ratio = (dnl.double() - rdnl.double()).abs().view(-1) / scale
     errs = {"eps": tu.rel(eps, reps), "dx": tu.rel(dx, rdx), "dnl": tu.rel(dnl, rdnl)}
     rows = tu.compare(grads, rgrads)
     worst = sorted(rows, key=lambda row: -row[1])[:3]
-    print(label or name, {k: f"{v:.2e}" for k, v in errs.items()}, "worst grads:", [(n, f"{e:.2e}") for n, e, _, _ in worst])
+    print(label or name, {k: f"{v:.2e}" for k, v in errs.items()}, "d noise_level error / (|c| |dtau|):", [f"{v:.2e}" for v in dnl_ratio.tolist()],
+          "worst grads:", [(n, f"{e:.2e}") for n, e, _, _ in worst])
     assert dnl.shape == rdnl.shape
-    assert errs["eps"] <= EPS_TOL and errs["dx"] <= INPUT_TOL and errs["dnl"] <= INPUT_TOL, errs
-    five = len(ui.ALL[name][0]["channel_multiplier"]) == 5
-    bad = [(n, e, c) for n, e, c, _ in rows if e >= (FIVE_LEVEL_TOL if five else GRAD_TOL)]
+    assert errs["eps"] <= EPS_TOL and errs["dx"] <= INPUT_TOL, errs
+    assert (dnl_ratio <= tol).all(), (dnl_ratio, tol)
+    bad = [(n, e, c) for n, e, c, _ in rows if e >= tol]
     assert not bad, bad[:10]
 
 
 @pytest.mark.timeout(1200)
 @pytest.mark.parametrize("name", sorted(ui.ALL))
-def test_unet_gradients_match_oracle(name):
+def test_unet_gradients_match_oracle_with_conditioned_dnl(name):
     """The tiny net at 32x32 (256-token attention) and 32x64 (512), the 4x4-level net at batch 3, an unconditional net, the 16->64 net at
-    64x64: eps, dx, d noise_level and every parameter gradient against the oracle's fp32 autograd."""
+    64x64: eps, dx, d noise_level (per image, conditioned: compare) and every parameter gradient against the oracle's fp32 autograd."""
     net, unet = build(name)
     x, nl, G = ui.inputs(name)
     o = ours(net, x, nl, G)
     b, h, w = ui.ALL[name][3:]
     assert o[1].shape == x.shape and o[2].shape == (b, 1)
-    compare(name, o, oracle_of(net, unet, name, x, nl, G))
+    compare(name, net, nl, o, oracle_of(net, unet, name, x, nl, G))
 
 
-def test_unet_gradients_with_reference_dropout_masks(golden):  # noqa: F811
+def test_unet_gradients_with_reference_dropout_masks_conditioned_dnl(golden):  # noqa: F811
     """train() mode with the reference's own nn.Dropout masks injected: against the oracle on the same masks, and eps against the golden."""
     d = golden["dropout"]
     name = d["case"]
@@ -91,7 +128,7 @@ def test_unet_gradients_with_reference_dropout_masks(golden):  # noqa: F811
     x, nl, G = ui.inputs(name)
     o = ours(net, x, nl, G, train_mode=True)
     assert tu.rel(o[0], d["eps"]) <= EPS_TOL
-    compare(name, o, oracle_of(net, unet, name, x, nl, G, masks, d["p"]), label=name + "/dropout")
+    compare(name, net, nl, o, oracle_of(net, unet, name, x, nl, G, masks, d["p"]), label=name + "/dropout")
 
 
 def test_train_mode_dropout_follows_torch_seed():
