@@ -572,7 +572,8 @@ class Engine:
         return lib().sr3_engine_workspace_bytes(self._h)
 
     def read_activation(self, name):
-        """fp32 output of a top-level UNet layer of the last forward, returned NCHW like a reference forward hook."""
+        """fp32 output of a top-level UNet layer of the last forward, returned NCHW like a reference forward hook.  For a layer with
+        self-attention that is the attention's output; "<layer>.res_block" ("mid.0.res_block") is its ResnetBlock's output."""
         numel = c_int64()
         shape = (c_int * 4)()
         _check(lib().sr3_engine_read_activation(self._h, name.encode(), c_void_p(0), 0, ctypes.byref(numel), shape, _stream()))

@@ -1439,7 +1439,7 @@ struct sr3_engine {
         bf16* a2 = static_cast<bf16*>(role("a2", (size_t)Bp * Hh * Ww * cout * 2 * PW));
         Act h; h.C = cout; h.H = Hh; h.W = Ww; h.stats = new_stats(cout);
         h.p = static_cast<float*>(role("h", (size_t)Bp * Hh * Ww * cout * 4));
-        Act y = new_act(cout, Hh, Ww, L.attn ? "" : L.name);
+        Act y = new_act(cout, Hh, Ww, L.attn ? p : L.name);
 
         add_prep(x, skip, g1, b1, G, true, a1, raw);
         float* mr1 = last_mr;

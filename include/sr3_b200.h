@@ -258,7 +258,8 @@ int64_t sr3_engine_workspace_bytes(const sr3_engine* e);
 int sr3_engine_profile_step(sr3_engine* e, int t, int reps, int cap, int* kinds, float* ms, double* flops, double* bytes, int* n_ops,
                             void* stream);
 /* Debug tap: copy the fp32 NHWC output of top-level layer `name` ("downs.3", "mid.0", ...) of the last forward to dst
- * (DEVICE, [B,H,W,C]); returns C*H*W*B through *numel. */
+ * (DEVICE, [B,H,W,C]); returns C*H*W*B through *numel.  The tap of a layer with self-attention is the attention's output; the output of
+ * its ResnetBlock, the attention's input, is the tap "<layer>.res_block" ("mid.0.res_block"). */
 int sr3_engine_read_activation(sr3_engine* e, const char* name, float* dst, int64_t cap, int64_t* numel, int shape_bhwc[4], void* stream);
 
 /* Stand-alone tile GEMM for unit tests: D[M,N] = A[M,K] * B[N,K]^T (bf16 row-major DEVICE inputs, fp32 output), M%128==0,
