@@ -96,6 +96,10 @@ _SIGS = {
     "sr3_windowed_read_state": (c_int, [c_void_p, c_void_p, c_void_p]),
     "sr3_windowed_grid": (c_int, [c_void_p, POINTER(c_int), POINTER(c_int), POINTER(c_int), POINTER(c_int), POINTER(c_float), POINTER(c_float)]),
     "sr3_windowed_profile_step": (c_int, [c_void_p, c_int, c_int, POINTER(c_float), c_void_p]),
+    "sr3_windowed_create_range": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, POINTER(c_int), POINTER(c_void_p)]),
+    "sr3_windowed_phase_begin": (c_int, [c_void_p, c_int, c_void_p]),
+    "sr3_windowed_phase_means": (c_int, [c_void_p, c_void_p]),
+    "sr3_windowed_phase_merge": (c_int, [c_void_p, c_void_p]),
     "sr3_engine_profile_step": (c_int, [c_void_p, c_int, c_int, c_int, POINTER(c_int), POINTER(c_float), POINTER(c_double), POINTER(c_double),
                                         POINTER(c_int), c_void_p]),
     "sr3_pil_bicubic_tables": (c_int, [c_int, c_int, POINTER(c_int), POINTER(c_int), c_int, POINTER(c_int)]),
@@ -615,16 +619,35 @@ def window_weights(n, side, overlap):
 
 class WindowedSampler:
     """A canvas [batch, C, height, width] sampled by overlapping windows of `engine`'s image size, merged inside every reverse step
-    (sr3_windowed_*).  Borrows the engine (engine.batch windows run per pass) and keeps it alive."""
+    (sr3_windowed_*).  Borrows the engine (engine.batch windows run per pass) and keeps it alive.
 
-    def __init__(self, engine, batch, height, width, overlap_h, overlap_w):
+    With `window_range` = (n0, n1) the sampler runs only windows [n0, n1) of the list (sr3_windowed_create_range): their means go to
+    `self.means`, an arena [N, C, wh, ww] of all N windows, NaN until written, into whose slots the means of other windows are copied or
+    received between phase_means() and phase_merge(); `bands` ([(y0, y1)] per image) limits the merge to those rows."""
+
+    def __init__(self, engine, batch, height, width, overlap_h, overlap_w, window_range=None, bands=None):
         self.engine = engine
         self.device = engine.device
         self.shape = (int(batch), engine.channels, int(height), int(width))
         self.overlap = (int(overlap_h), int(overlap_w))
+        self.window_range = None if window_range is None else (int(window_range[0]), int(window_range[1]))
+        self.means = None
         self._h = c_void_p()
         with torch.cuda.device(self.device):
-            _check(lib().sr3_windowed_create(engine._h, *self.shape[:1], *self.shape[2:], *self.overlap, ctypes.byref(self._h)))
+            if self.window_range is None:
+                _check(lib().sr3_windowed_create(engine._h, *self.shape[:1], *self.shape[2:], *self.overlap, ctypes.byref(self._h)))
+            else:
+                n = self.shape[0] * len(window_grid(height, engine.height, overlap_h)) * len(window_grid(width, engine.width, overlap_w))
+                if not 0 <= self.window_range[0] < self.window_range[1] <= n:
+                    raise ValueError("window range %s is not a non-empty part of the %d windows" % (self.window_range, n))
+                bt = None
+                if bands is not None:
+                    if len(bands) != self.shape[0]:
+                        raise ValueError("bands has %d entries for %d images" % (len(bands), self.shape[0]))
+                    bt = (c_int * (2 * self.shape[0]))(*[int(v) for yb in bands for v in yb])
+                self.means = torch.full((n, engine.channels, engine.height, engine.width), float("nan"), device=self.device)
+                _check(lib().sr3_windowed_create_range(engine._h, *self.shape[:1], *self.shape[2:], *self.overlap, *self.window_range,
+                                                       _ptr(self.means), bt, ctypes.byref(self._h)))
         self._keep = None
 
     def __del__(self):
@@ -685,6 +708,21 @@ class WindowedSampler:
         self.begin(condition_x, x_T, seed, first_index)
         self.steps(T - 1, T, noises, snaps)
         return self.read_state(), snaps
+
+    def phase_begin(self, t_start):
+        """Start a run of split steps from timestep t_start down (Philox noise keyed by begin()'s seed and first_index)."""
+        with torch.cuda.device(self.device):
+            _check(lib().sr3_windowed_phase_begin(self._h, int(t_start), _stream()))
+
+    def phase_means(self):
+        """Phase (a) of a step: advance the timestep, run this canvas's windows, store their means into the arena."""
+        with torch.cuda.device(self.device):
+            _check(lib().sr3_windowed_phase_means(self._h, _stream()))
+
+    def phase_merge(self):
+        """Phase (b) of the step: merge the arena's means (over the band) into x_{t-1}."""
+        with torch.cuda.device(self.device):
+            _check(lib().sr3_windowed_phase_merge(self._h, _stream()))
 
     def profile_step(self, t, reps=3):
         """{"gather", "engine", "merge"}: device ms per eager canvas step (CUDA events)."""

@@ -1888,25 +1888,33 @@ static std::vector<float> window_weights(int n, int side, int overlap) {
 struct sr3_windowed {
     sr3_engine* e = nullptr;               // borrowed: runs Bw = e->B windows of e->H x e->W per pass
     int B = 0, H = 0, W = 0, N = 0;        // canvas batch and size; windows of all images
+    int n0 = 0, n1 = 0;                    // the windows this canvas runs: [n0, n1) of the list (all of them unless created for a range)
+    bool ranged = false;                   // created by sr3_windowed_create_range: steps run as the two phases only
     std::vector<int> oy, ox;
     std::vector<float> wy, wx;
     DevAllocs mem;
     WindowGeom g{};
     float *x = nullptr, *cond = nullptr, *noise = nullptr, *means = nullptr;
+    const int* band = nullptr; int band_rows = 0;      // optional device [B][2] rows the merge computes (a ranged canvas's band)
     WindowCtl* ctl_dev = nullptr;
     WindowCtl ctl{};
     uint64_t seed = 0, first_index = 0;
     float* snapshots = nullptr; int snapshot_cap = 0;
-    cudaGraphExec_t graph = nullptr;
+    cudaGraphExec_t graph = nullptr, graph_means = nullptr, graph_merge = nullptr;
     cudaStream_t cap_stream = nullptr;
+    int phase_steps_left = 0; bool merge_due = false;  // host-side order of the phase calls
 
     ~sr3_windowed() {
-        if (graph) cudaGraphExecDestroy(graph);
+        for (cudaGraphExec_t g : {graph, graph_means, graph_merge})
+            if (g) cudaGraphExecDestroy(g);
         if (cap_stream) cudaStreamDestroy(cap_stream);
     }
     size_t canvas_elems() const { return (size_t)B * e->cfg.channels * H * W; }
 
-    void init(sr3_engine* eng, int batch, int height, int width, int overlap_h, int overlap_w) {
+    // A ranged canvas (first >= 0) runs windows [first, end) only, stores their means into the caller's arena `ext_means` [N][C][wh][ww]
+    // and merges only the rows of `bands` (HOST [B][2], nullptr: all rows).
+    void init(sr3_engine* eng, int batch, int height, int width, int overlap_h, int overlap_w, int first = -1, int end = -1,
+              float* ext_means = nullptr, const int* bands = nullptr) {
         e = eng; B = batch; H = height; W = width;
         const int wh = e->H, ww = e->W, C = e->cfg.channels;
         // checked before anything is allocated
@@ -1918,11 +1926,27 @@ struct sr3_windowed {
         oy = window_origins(H, wh, overlap_h); ox = window_origins(W, ww, overlap_w);
         wy = window_weights((int)oy.size(), wh, overlap_h); wx = window_weights((int)ox.size(), ww, overlap_w);
         N = B * (int)(oy.size() * ox.size());
+        n0 = 0; n1 = N;
+        if (first >= 0) {
+            REQUIRE(first < end && end <= N, "window range [%d, %d) is not a non-empty part of the %d windows", first, end, N);
+            REQUIRE(ext_means != nullptr, "a window range needs the caller's means arena");
+            if (bands)
+                for (int b = 0; b < B; ++b)
+                    REQUIRE(0 <= bands[2 * b] && bands[2 * b] <= bands[2 * b + 1] && bands[2 * b + 1] <= H, "band of image %d is rows [%d, %d) of %d",
+                            b, bands[2 * b], bands[2 * b + 1], H);
+            n0 = first; n1 = end; ranged = true;
+        }
         CK(cudaSetDevice(e->dev));
         const size_t cb = canvas_elems() * sizeof(float);
         x = static_cast<float*>(mem.alloc(cb)); noise = static_cast<float*>(mem.alloc(cb));
         if (e->cond_c) cond = static_cast<float*>(mem.alloc((size_t)B * e->cond_c * H * W * sizeof(float)));
-        means = static_cast<float*>(mem.alloc((size_t)N * C * wh * ww * sizeof(float)));
+        means = ranged ? ext_means : static_cast<float*>(mem.alloc((size_t)N * C * wh * ww * sizeof(float)));
+        if (ranged && bands) {
+            int* bd = static_cast<int*>(mem.alloc((size_t)2 * B * sizeof(int)));
+            CK(cudaMemcpy(bd, bands, (size_t)2 * B * sizeof(int), cudaMemcpyHostToDevice));
+            band = bd;
+            for (int b = 0; b < B; ++b) band_rows = std::max(band_rows, bands[2 * b + 1] - bands[2 * b]);
+        }
         ctl_dev = static_cast<WindowCtl*>(mem.alloc(sizeof(WindowCtl)));
         int* oyd = static_cast<int*>(mem.alloc(oy.size() * sizeof(int))); int* oxd = static_cast<int*>(mem.alloc(ox.size() * sizeof(int)));
         float* wyd = static_cast<float*>(mem.alloc(wy.size() * sizeof(float))); float* wxd = static_cast<float*>(mem.alloc(wx.size() * sizeof(float)));
@@ -1940,7 +1964,7 @@ struct sr3_windowed {
     void begin_step(cudaStream_t st) { launch_k(step_begin_kernel, dim3(1), dim3(32), 0, st, static_cast<float4*>(nullptr), 0LL, &ctl_dev->step); }
     void gather(int first, cudaStream_t st) {
         WindowGather p{};
-        p.g = g; p.cond = cond; p.x = x; p.first = first; p.n_total = N; p.Bw = e->B;
+        p.g = g; p.cond = cond; p.x = x; p.first = first; p.n_total = n1; p.Bw = e->B;
         p.in_buf = e->in_buf; p.in_ld = e->in_C * e->PW; p.cond_c = e->cond_c; p.lo_off = e->precise ? e->in_C : 0;
         p.x_state = e->x_state; p.wctl = ctl_dev; p.ectl = e->ctl_dev;
         const long long total = 1LL * e->B * g.wh * (g.ww / 4);
@@ -1948,34 +1972,43 @@ struct sr3_windowed {
     }
     void store_means(int first, cudaStream_t st) {
         const size_t win = (size_t)g.C * g.wh * g.ww;
-        CK(cudaMemcpyAsync(means + first * win, e->mean_buf, std::min(e->B, N - first) * win * sizeof(float), cudaMemcpyDeviceToDevice, st));
+        CK(cudaMemcpyAsync(means + first * win, e->mean_buf, std::min(e->B, n1 - first) * win * sizeof(float), cudaMemcpyDeviceToDevice, st));
     }
     void merge(cudaStream_t st) {
         WindowMerge m{};
         m.g = g; m.means = means; m.x = x; m.noise = noise; m.tab = e->post_tab; m.tab_T = e->T_cap; m.ctl = ctl_dev;
-        const long long total = 1LL * B * H * W;
+        m.band = band; m.band_rows = band_rows;
+        const long long total = 1LL * B * (band ? band_rows : H) * W;
         launch_k(window_merge_kernel, dim3((int)std::min<long long>((total + 255) / 256, num_sms() * 8LL)), dim3(256), 0, st, m);
     }
-    void record_step(cudaStream_t st) {
+    // Phase (a) of a step: the timestep advance and the passes over this canvas's windows, their means stored into the arena.
+    void record_means(cudaStream_t st) {
         begin_step(st);
-        for (int first = 0; first < N; first += e->B) {
+        for (int first = n0; first < n1; first += e->B) {
             gather(first, st);
             e->record_step(st);
             store_means(first, st);
         }
+    }
+    void record_step(cudaStream_t st) {
+        record_means(st);
         merge(st);
     }
-    void run_step(cudaStream_t st) {
-        if (!graph) {
+    template <class F> void launch_graph(cudaGraphExec_t& exec, F record, cudaStream_t st) {
+        if (!exec) {
             cudaGraph_t gr;
             CK(cudaStreamBeginCapture(cap_stream, cudaStreamCaptureModeThreadLocal));
-            record_step(cap_stream);
+            record(cap_stream);
             CK(cudaStreamEndCapture(cap_stream, &gr));
-            CK(cudaGraphInstantiate(&graph, gr, 0));
+            CK(cudaGraphInstantiate(&exec, gr, 0));
             CK(cudaGraphDestroy(gr));
         }
-        CK(cudaGraphLaunch(graph, st));
+        CK(cudaGraphLaunch(exec, st));
     }
+    void run_step(cudaStream_t st) { launch_graph(graph, [this](cudaStream_t s) { record_step(s); }, st); }
+    // The two phases of a step as separate graphs, so that means of windows other canvases ran can be written into the arena between them.
+    void run_means(cudaStream_t st) { launch_graph(graph_means, [this](cudaStream_t s) { record_means(s); }, st); }
+    void run_merge(cudaStream_t st) { launch_graph(graph_merge, [this](cudaStream_t s) { merge(s); }, st); }
     // Control blocks of a run of steps starting at timestep t: the engine computes clipped posterior means only (its own noise add is
     // discarded: update_state = 0, z read from its zeroed noise buffer); the canvas block carries the timestep, the noise source and the key.
     void push_ctl(int t, bool injected, cudaStream_t st) {
@@ -2448,6 +2481,7 @@ int sr3_windowed_set_snapshots(sr3_windowed* w, float* snapshots, int snapshot_c
 int sr3_windowed_steps(sr3_windowed* w, int t_start, int steps, const float* noises, void* stream) {
     API_BEGIN
     REQUIRE(w, "null argument");
+    REQUIRE(!w->ranged, "a canvas that runs a window range steps through sr3_windowed_phase_means / _merge");
     sr3_engine* e = w->e;
     REQUIRE(t_start < e->T && steps >= 0 && t_start - steps + 1 >= 0, "bad step range t_start=%d steps=%d T=%d", t_start, steps, e->T);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -2459,6 +2493,44 @@ int sr3_windowed_steps(sr3_windowed* w, int t_start, int steps, const float* noi
         if (noises) CK(cudaMemcpyAsync(w->noise, noises + (size_t)(t_start - i) * n, n * sizeof(float), cudaMemcpyDeviceToDevice, st));
         w->run_step(st);
     }
+    API_END
+}
+int sr3_windowed_create_range(sr3_engine* e, int batch, int height, int width, int overlap_h, int overlap_w, int first_window, int end_window,
+                              float* means, const int* bands, sr3_windowed** out) {
+    API_BEGIN
+    REQUIRE(e && out && first_window >= 0, "bad argument");
+    std::unique_ptr<sr3_windowed> w(new sr3_windowed());
+    w->init(e, batch, height, width, overlap_h, overlap_w, first_window, end_window, means, bands);
+    *out = w.release();
+    API_END
+}
+int sr3_windowed_phase_begin(sr3_windowed* w, int t_start, void* stream) {
+    API_BEGIN
+    REQUIRE(w, "null argument");
+    sr3_engine* e = w->e;
+    REQUIRE(t_start >= 0 && t_start < e->T, "bad t_start=%d T=%d", t_start, e->T);
+    CK(cudaSetDevice(e->dev));
+    e->check_params();
+    w->push_ctl(t_start, false, static_cast<cudaStream_t>(stream));
+    w->phase_steps_left = t_start + 1; w->merge_due = false;
+    API_END
+}
+int sr3_windowed_phase_means(sr3_windowed* w, void* stream) {
+    API_BEGIN
+    REQUIRE(w, "null argument");
+    REQUIRE(!w->merge_due && w->phase_steps_left > 0, "sr3_windowed_phase_means out of order (%d steps left, merge %s)", w->phase_steps_left,
+            w->merge_due ? "due" : "not due");
+    CK(cudaSetDevice(w->e->dev));
+    w->run_means(static_cast<cudaStream_t>(stream));
+    w->merge_due = true; --w->phase_steps_left;
+    API_END
+}
+int sr3_windowed_phase_merge(sr3_windowed* w, void* stream) {
+    API_BEGIN
+    REQUIRE(w && w->merge_due, "sr3_windowed_phase_merge without sr3_windowed_phase_means before it");
+    CK(cudaSetDevice(w->e->dev));
+    w->run_merge(static_cast<cudaStream_t>(stream));
+    w->merge_due = false;
     API_END
 }
 int sr3_windowed_read_state(sr3_windowed* w, float* x_out, void* stream) {
@@ -2486,7 +2558,7 @@ int sr3_windowed_profile_step(sr3_windowed* w, int t, int reps, float* ms, void*
     REQUIRE(e->T > 0 && t >= 0 && t < e->T, "bad t");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     CK(cudaSetDevice(e->dev));
-    const int Bw = e->B, passes = (w->N + Bw - 1) / Bw;
+    const int Bw = e->B, passes = (w->n1 - w->n0 + Bw - 1) / Bw;
     std::vector<cudaEvent_t> ev(3 * passes + 2);
     for (auto& x : ev) CK(cudaEventCreate(&x));
     double acc[3] = {0, 0, 0};
@@ -2495,11 +2567,11 @@ int sr3_windowed_profile_step(sr3_windowed* w, int t, int reps, float* ms, void*
         w->begin_step(st);
         for (int pi = 0; pi < passes; ++pi) {
             CK(cudaEventRecord(ev[3 * pi], st));
-            w->gather(pi * Bw, st);
+            w->gather(w->n0 + pi * Bw, st);
             CK(cudaEventRecord(ev[3 * pi + 1], st));
             for (auto& op : e->ops) op(st);
             CK(cudaEventRecord(ev[3 * pi + 2], st));
-            w->store_means(pi * Bw, st);
+            w->store_means(w->n0 + pi * Bw, st);
         }
         CK(cudaEventRecord(ev[3 * passes], st));
         w->merge(st);

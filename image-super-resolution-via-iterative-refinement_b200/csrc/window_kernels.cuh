@@ -93,17 +93,20 @@ __global__ void __launch_bounds__(256) window_gather_kernel(const WindowGather p
 
 struct WindowMerge {
     WindowGeom g;
-    const float* means;      // window-mean arena [B * ny * nx][C][wh][ww]
+    const float* means;      // window-mean arena [B * ny * nx][C][wh][ww]: every window covering a merged pixel must be present
     float* x;                // canvas state, overwritten with x_{t-1}
     const float* noise;      // canvas-shaped z of this step (read when step.use_noise_buf)
     const float* tab;        // the engine's [5][tab_T] schedule table
     int tab_T;
     const WindowCtl* ctl;
+    const int* band;         // optional [B][2]: only rows [y0, y1) of image b are merged (a rank's band); nullptr: every row
+    int band_rows;           // max over images of y1 - y0 (the launch covers B x band_rows x W pixels)
 };
 
 // One thread per canvas pixel, all (<= 4) channels: the Philox draw of a pixel yields the z of its channels.  The covering windows are found
 // from the two per-axis origin tables and accumulated in ascending window index with separately rounded multiplies and adds, so the sum is
-// the same whatever the launch shape and however many windows a pass ran: no atomics, repeat runs are bit identical.
+// the same whatever the launch shape and however many windows a pass ran: no atomics, repeat runs are bit identical.  With a band table
+// a pixel outside its image's band is neither read nor written, so a rank that holds only the means covering its band computes that band.
 __global__ void __launch_bounds__(256) window_merge_kernel(const WindowMerge p) {
     pdl_launch_dependents();
     pdl_wait();
@@ -119,10 +122,15 @@ __global__ void __launch_bounds__(256) window_merge_kernel(const WindowMerge p) 
         const int slot = (p.ctl->T - 1) / inter - t / inter;
         if (p.ctl->snapshots != nullptr && t % inter == 0 && slot < p.ctl->snapshot_cap) snap = p.ctl->snapshots + slot * (plane * g.C * g.B);
     }
-    const long long total = plane * g.B;
+    const long long bplane = p.band ? static_cast<long long>(p.band_rows) * g.W : plane;
+    const long long total = bplane * g.B;
     for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total; i += static_cast<long long>(gridDim.x) * blockDim.x) {
-        const int b = static_cast<int>(i / plane);
-        const long long pix = i - b * plane;
+        const int b = static_cast<int>(i / bplane);
+        long long pix = i - b * bplane;
+        if (p.band) {
+            pix += static_cast<long long>(p.band[2 * b]) * g.W;
+            if (pix >= static_cast<long long>(p.band[2 * b + 1]) * g.W) continue;
+        }
         const int y = static_cast<int>(pix / g.W), x = static_cast<int>(pix - static_cast<long long>(y) * g.W);
         float num[4] = {0.f, 0.f, 0.f, 0.f}, den = 0.f;
         for (int iy = 0; iy < g.ny; ++iy) {

@@ -159,9 +159,9 @@ class GaussianDiffusion(nn.Module):
     # ---- windowed sampling: canvases of any size, see DESIGN.md 3.9
     WINDOW_PASS_SIZES = (16, 8, 4, 2, 1)      # windows per engine pass: the largest one not above the window count whose engine fits
 
-    def _windowed_sampler(self, batch, height, width, window=None, overlap=None):
-        """The canvas sampler for [batch, C, height, width] (sr3_windowed_*).  Every argument is checked before anything is allocated:
-        `window` by _native.check_image_size (UnsupportedSizeError), then the overlaps and the canvas size (ValueError)."""
+    def _window_geometry(self, height, width, window=None, overlap=None):
+        """((wh, ww), (overlap_h, overlap_w)) of a canvas, checked before anything is allocated: `window` by _native.check_image_size
+        (UnsupportedSizeError), then the overlaps and the canvas size (ValueError)."""
         from ... import _native
         wh, ww = (self.image_size, self.image_size) if window is None else (int(window[0]), int(window[1]))
         _native.check_image_size(len(self.denoise_fn.arch["channel_mults"]), wh, ww)
@@ -173,22 +173,39 @@ class GaussianDiffusion(nn.Module):
                 raise ValueError("overlap %d must be at least 0 and below the window side %d" % (ov, side))
         if height < wh or width < ww:
             raise ValueError("canvas %dx%d is smaller than the window %dx%d (canvases are not padded)" % (height, width, wh, ww))
-        n = batch * len(_native.window_grid(height, wh, ovh)) * len(_native.window_grid(width, ww, ovw))
+        return (wh, ww), (ovh, ovw)
+
+    def _window_engine(self, n, wh, ww):
+        """The engine that runs `n` windows of wh x ww: the largest WINDOW_PASS_SIZES entry not above n whose engine fits."""
         sizes = [s for s in self.WINDOW_PASS_SIZES if s <= n] or [min(self.WINDOW_PASS_SIZES)]
-        eng = None
         for i, bw in enumerate(sizes):
             try:
-                eng = self._engine(bw, wh, ww)
-                break
+                return self._engine(bw, wh, ww)
             except RuntimeError as e:          # an engine of this batch does not fit the device: run fewer windows per pass
                 if "out of memory" not in str(e) or i == len(sizes) - 1:
                     raise
+
+    def _windowed_sampler(self, batch, height, width, window=None, overlap=None):
+        """The canvas sampler for [batch, C, height, width] (sr3_windowed_*).  Every argument is checked before anything is allocated
+        (_window_geometry)."""
+        from ... import _native
+        (wh, ww), (ovh, ovw) = self._window_geometry(height, width, window, overlap)
+        n = batch * len(_native.window_grid(height, wh, ovh)) * len(_native.window_grid(width, ww, ovw))
+        eng = self._window_engine(n, wh, ww)
         key = (batch, height, width, ovh, ovw)
         cached = getattr(self, "_windowed", None)
         if cached is None or cached[0] != key or cached[1].engine is not eng:
             self._windowed = None              # release the previous canvas before the new one is allocated
             self._windowed = cached = (key, _native.WindowedSampler(eng, batch, height, width, ovh, ovw))
         return cached[1]
+
+    def _windowed_range_sampler(self, batch, height, width, window, overlap, shard):
+        """A canvas sampler that runs only the windows of `shard` (a parallel.WindowShard of this geometry's plan), with its own means
+        arena and the shard's band: the sampler of one rank of a canvas sharded by window."""
+        from ... import _native
+        (wh, ww), (ovh, ovw) = self._window_geometry(height, width, window, overlap)
+        eng = self._window_engine(shard.n1 - shard.n0, wh, ww)
+        return _native.WindowedSampler(eng, batch, height, width, ovh, ovw, window_range=(shard.n0, shard.n1), bands=shard.bands)
 
     @torch.no_grad()
     def super_resolution_windowed(self, x_in, window=None, overlap=None, continous=False, x_T=None, noises=None, seed=None, first_index=0):

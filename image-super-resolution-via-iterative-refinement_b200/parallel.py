@@ -5,12 +5,17 @@ all-gather (SURVEY.md 8e).  The reference only offers nn.DataParallel for traini
 
 Noise comes from Philox streams keyed by the GLOBAL sample index, so the result does not depend on the number of ranks.
 
+A batch of fewer images than ranks (one large photograph) is sharded by WINDOW instead (window_shard_plan, DESIGN.md 5): every rank
+runs a contiguous range of the canvas's window list and exchanges the means of the windows along its band's edges with its neighbours once
+per reverse step; the result is the one-GPU windowed canvas bit for bit when every rank runs engines of the same shape.
+
 Training (SURVEY.md 8e, config 4) is plain data parallelism with ONE exchange step: every rank runs forward / backward on its slice of the
 batch, the parameter gradients are summed with NCCL all-reduces in buckets that are issued while the backward of the earlier layers is still
 running (the native backward is replayed layer by layer: sr3_train_backward_block), and Adam is applied redundantly on every rank.  The
 reference's own multi-GPU training is nn.DataParallel (model/networks.py:113-115: replicate + scatter + gather every forward).
 """
-from typing import Callable, Optional, Tuple
+import bisect
+from typing import Callable, List, NamedTuple, Optional, Sequence, Tuple
 
 import torch
 import torch.distributed as dist
@@ -67,11 +72,16 @@ def sharded_super_resolution(netG, x_in: torch.Tensor, x_T: Optional[torch.Tenso
     by the global sample index (`first_index`), so the images do not depend on the number of ranks.
 
     `window` / `overlap` (either one given): every rank runs `GaussianDiffusion.super_resolution_windowed`'s loop on its slice instead, for
-    `x_in` of any size; its noise is keyed by the global sample index and the pixel's index in the canvas, so this too is rank independent."""
+    `x_in` of any size; its noise is keyed by the global sample index and the pixel's index in the canvas, so this too is rank independent.
+    With fewer images than ranks the windows of the whole batch are sharded across the ranks instead (sharded_windowed_super_resolution),
+    so one large image runs on every GPU."""
     dev = netG.betas.device
     if x_T is None:
         g = torch.Generator().manual_seed(seed)
         x_T = torch.randn(tuple(x_in.shape), generator=g)
+    world = dist.get_world_size(group) if dist.is_initialized() else 1
+    if (window is not None or overlap is not None) and x_in.shape[0] < world:
+        return sharded_windowed_super_resolution(netG, x_in, x_T, seed, 0, window, overlap, group)
 
     def fn(c, xt, first):
         if c.shape[0] == 0:
@@ -87,6 +97,167 @@ def sharded_super_resolution(netG, x_in: torch.Tensor, x_T: Optional[torch.Tenso
         return final
 
     return sharded_sample(fn, x_in, x_T, group)
+
+
+# ---------------------------------------------------------------------------------------------------- windowed canvas, sharded by window
+class WindowShard(NamedTuple):
+    """One rank's part of a canvas sharded by window.  Window n of the list is (image n // (ny nx), row (n // nx) % ny, column n % nx)."""
+    n0: int                                 # owned windows [n0, n1) (n0 == n1: none)
+    n1: int
+    bands: List[Tuple[int, int]]            # per image: rows [y0, y1) the owned windows read, full width ((0, 0): none)
+    recv: List[Tuple[int, int, int]]        # (src rank, m0, m1): not-owned windows [m0, m1) whose rows meet a band, owned by src
+    send: List[Tuple[int, int, int]]        # (dst rank, m0, m1): the transpose of the other ranks' receive lists
+    rows: List[Tuple[int, int, int]]        # (image, y0, y1): the rows this rank contributes to the finished canvas
+
+
+def _pair(v):
+    return (int(v), int(v)) if isinstance(v, int) else (int(v[0]), int(v[1]))
+
+
+def window_shard_plan(batch: int, height: int, width: int, window, overlap, world: int) -> List[WindowShard]:
+    """Ownership and exchange plan of a canvas [batch, C, height, width] covered by `window` = (wh, ww) windows that overlap by `overlap`
+    (ints or pairs), on the grid of _native.window_grid, split over `world` ranks.  Rank r owns the balanced range shard_bounds(N, world, r)
+    of the N windows; its band in an image runs from its first owned window's origin row to its last one's origin row + wh.  Every
+    window covering a pixel of the band meets the band's rows, so the owned and received means are all a merge of the band reads.  The
+    output rows give every row of every image to exactly one rank whose band contains it."""
+    from ._native import window_grid
+    (wh, ww), (ovh, ovw) = _pair(window), _pair(overlap)
+    oy, ox = window_grid(height, wh, ovh), window_grid(width, ww, ovw)
+    ny, nx = len(oy), len(ox)
+    per = ny * nx
+    n = batch * per
+    if batch < 1 or world < 1:
+        raise ValueError("bad plan request: batch %d, world %d" % (batch, world))
+    starts = [shard_bounds(n, world, r)[0] for r in range(world)]
+
+    shards = []
+    for r in range(world):
+        n0, n1 = shard_bounds(n, world, r)
+        bands, recv = [(0, 0)] * batch, []
+        for b in range(batch):
+            lo, hi = max(n0, b * per), min(n1, (b + 1) * per)
+            if lo >= hi:
+                continue
+            y0, y1 = oy[(lo - b * per) // nx], oy[(hi - 1 - b * per) // nx] + wh
+            bands[b] = (y0, y1)
+            hit = [iy for iy in range(ny) if oy[iy] < y1 and oy[iy] + wh > y0]
+            for m in range(b * per + hit[0] * nx, b * per + (hit[-1] + 1) * nx):
+                if n0 <= m < n1:
+                    continue
+                src = bisect.bisect_right(starts, m) - 1        # ranks that own nothing start at n, past every window
+                if recv and recv[-1][0] == src and recv[-1][2] == m:
+                    recv[-1] = (src, recv[-1][1], m + 1)
+                else:
+                    recv.append((src, m, m + 1))
+        shards.append((n0, n1, bands, recv))
+    send = [[] for _ in range(world)]
+    for r, (_, _, _, recv) in enumerate(shards):
+        for src, m0, m1 in recv:
+            send[src].append((r, m0, m1))
+    rows = [[] for _ in range(world)]
+    for b in range(batch):
+        cur = 0
+        for r in range(world):
+            y0, y1 = shards[r][2][b]
+            if y1 > cur:
+                assert y0 <= cur, (b, r, y0, cur)          # bands start in rank order and leave no gap: the windows cover the canvas
+                rows[r].append((b, cur, y1))
+                cur = y1
+        assert cur == height, (b, cur, height)
+    return [WindowShard(n0, n1, bands, recv, send[r], rows[r]) for r, (n0, n1, bands, recv) in enumerate(shards)]
+
+
+def local_exchange(plan: Sequence[WindowShard], arenas: Sequence[Optional[torch.Tensor]]) -> Callable[[], None]:
+    """The exchange between the means arenas of len(plan) ranks emulated in one process (None: a rank that owns nothing): every receive
+    of the plan as a tensor copy from its owner's arena, on the current stream."""
+    copies = [(arenas[r][m0:m1], arenas[src][m0:m1]) for r, sh in enumerate(plan) for src, m0, m1 in sh.recv]
+
+    def run():
+        for dst, src in copies:
+            dst.copy_(src)
+    return run
+
+
+def p2p_exchange(plan: Sequence[WindowShard], rank: int, arena: Optional[torch.Tensor], group=None) -> Callable[[], None]:
+    """The exchange of this rank's slabs with torch.distributed point-to-point operations (NCCL on GPUs: queued behind and waited for on
+    the current stream, no host synchronisation).  Sends and receives of one pair are posted in ascending window order on both sides."""
+    peer = (lambda r: r) if group is None else (lambda r: dist.get_global_rank(group, r))
+    sh = plan[rank]
+    ops = [dist.P2POp(dist.isend, arena[m0:m1], peer(dst), group) for dst, m0, m1 in sh.send] + \
+          [dist.P2POp(dist.irecv, arena[m0:m1], peer(src), group) for src, m0, m1 in sh.recv]
+
+    def run():
+        if ops:
+            for w in dist.batch_isend_irecv(ops):
+                w.wait()
+    return run
+
+
+def sharded_windowed_loop(samplers: Sequence, exchange: Callable[[], None]) -> List[torch.Tensor]:
+    """The whole reverse loop of range samplers (_native.WindowedSampler with a window_range, begin() already called), every step:
+    phase (a) on every sampler, exchange(), phase (b) on every sampler.  Returns each sampler's final canvas state (its band rows hold
+    the result; other rows are whatever begin() put there)."""
+    if samplers:
+        T = samplers[0].engine.T
+        for s in samplers:
+            s.phase_begin(T - 1)
+        for _ in range(T):
+            for s in samplers:
+                s.phase_means()
+            exchange()
+            for s in samplers:
+                s.phase_merge()
+    return [s.read_state() for s in samplers]
+
+
+def assemble_rows(plan: Sequence[WindowShard], states: Sequence[Optional[torch.Tensor]]) -> torch.Tensor:
+    """The finished canvas from the states of emulated ranks: every row from the rank the plan gives it to."""
+    ref = next(s for s in states if s is not None)
+    out = torch.empty_like(ref)
+    for sh, st in zip(plan, states):
+        for b, y0, y1 in sh.rows:
+            out[b, :, y0:y1] = st[b, :, y0:y1]
+    return out
+
+
+def gather_rows(plan: Sequence[WindowShard], rank: int, state: Optional[torch.Tensor], shape, device, group=None) -> torch.Tensor:
+    """The finished canvas on every rank: each rank's output rows, all-gathered (padded to the longest) and placed; exact."""
+    B, C, H, W = shape
+    sizes = [sum(y1 - y0 for _, y0, y1 in sh.rows) * C * W for sh in plan]
+    buf = torch.zeros(max(sizes), dtype=torch.float32, device=device)
+    if sizes[rank]:
+        buf[:sizes[rank]] = torch.cat([state[b, :, y0:y1].reshape(-1) for b, y0, y1 in plan[rank].rows])
+    parts = [torch.empty_like(buf) for _ in plan]
+    dist.all_gather(parts, buf, group=group)
+    out = torch.empty(shape, dtype=torch.float32, device=device)
+    for sh, part in zip(plan, parts):
+        off = 0
+        for b, y0, y1 in sh.rows:
+            k = (y1 - y0) * C * W
+            out[b, :, y0:y1] = part[off:off + k].view(C, y1 - y0, W)
+            off += k
+    return out
+
+
+def sharded_windowed_super_resolution(netG, x_in: torch.Tensor, x_T: torch.Tensor, seed: int, first_index: int, window, overlap,
+                                      group=None) -> torch.Tensor:
+    """`GaussianDiffusion.super_resolution_windowed` of the whole batch with its windows sharded across the ranks of `group`: each rank
+    builds the same plan, runs its window range on an engine chosen from its own window count, exchanges the means its band needs every
+    step over point-to-point operations and ends with the whole finished [B, C, H, W] canvas."""
+    world = dist.get_world_size(group)
+    rank = dist.get_rank(group)
+    dev = netG.betas.device
+    B, _, H, W = x_in.shape
+    (wh, ww), ov = netG._window_geometry(H, W, window, overlap)
+    plan = window_shard_plan(B, H, W, (wh, ww), ov, world)
+    sh = plan[rank]
+    sampler = None
+    if sh.n1 > sh.n0:
+        sampler = netG._windowed_range_sampler(B, H, W, (wh, ww), ov, sh)
+        sampler.begin(x_in.to(dev, non_blocking=True), x_T.to(dev, non_blocking=True), seed, first_index)
+    dist.all_reduce(torch.zeros(1, device=dev), group=group)     # every rank joins the group's first operation before the point-to-point
+    states = sharded_windowed_loop([sampler] if sampler else [], p2p_exchange(plan, rank, sampler.means if sampler else None, group))
+    return gather_rows(plan, rank, states[0] if states else None, (B, netG.channels, H, W), dev, group)
 
 
 # ---------------------------------------------------------------------------------------------------------------- training

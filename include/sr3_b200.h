@@ -218,6 +218,23 @@ int sr3_windowed_grid(const sr3_windowed* w, int* ny, int* nx, int* origins_y, i
  * of the engine passes and of the merge, averaged over `reps` steps after one warm-up.  Advances the canvas state. */
 int sr3_windowed_profile_step(sr3_windowed* w, int t, int reps, float* ms, void* stream);
 
+/* ---- windowed sampling sharded by window (one canvas on several GPUs).  A ranged canvas runs only windows [first_window, end_window) of
+ * the list and stores their means into `means`, a DEVICE arena [N][3][window height][window width] of all N windows owned by the caller;
+ * the caller fills the slots of the other windows it needs (the ones covering its band) between the two phases of every step.  `bands`:
+ * optional HOST [batch][2] rows [y0, y1) per image the merge computes (copied; NULL: every row); the merge reads the means of every window
+ * that covers a pixel of the band and nothing else, and the gathers read only the rows of the range's windows, so rows outside the band
+ * may hold anything.  A step of a ranged canvas equals the same rows of a whole canvas's step bit for bit when the arena holds the same
+ * means.  sr3_windowed_steps refuses a ranged canvas; sr3_windowed_profile_step profiles its range.  Ranged canvases may share one engine
+ * when their phases are issued in order on one stream: every pass rewrites the engine's input and state. */
+int sr3_windowed_create_range(sr3_engine* e, int batch, int height, int width, int overlap_h, int overlap_w, int first_window, int end_window,
+                              float* means, const int* bands, sr3_windowed** out);
+/* Starts a run of steps from timestep t_start down (Philox noise); then per step: phase_means (timestep advance, passes over the range,
+ * means into the arena), the caller's exchange into the arena on or behind `stream`, phase_merge (merge of the band -> x_{t-1}).  Each phase
+ * is one CUDA graph (captured at its first call); neither synchronises the host.  Calls out of this order are refused. */
+int sr3_windowed_phase_begin(sr3_windowed* w, int t_start, void* stream);
+int sr3_windowed_phase_means(sr3_windowed* w, void* stream);
+int sr3_windowed_phase_merge(sr3_windowed* w, void* stream);
+
 /* core/metrics.py:8-34 `tensor2img` on the device: src fp32 DEVICE [n][C][H][W] -> clamp to [min_v, max_v] -> [0, 1] -> * 255, round half
  * to even -> uint8 DEVICE, HWC.  n == 1: dst [H][W][C].  n > 1: the images are tiled like torchvision.utils.make_grid(nrow, padding 2,
  * pad_value 0), which is what the reference does for 4-D input: dst [rows*(H+2)+2][cols*(W+2)+2][C], cols = min(nrow, n).
