@@ -113,6 +113,7 @@ _SIGS = {
     "sr3_engine_num_ops_per_step": (c_int, [c_void_p]),
     "sr3_engine_workspace_bytes": (c_int64, [c_void_p]),
     "sr3_engine_read_activation": (c_int, [c_void_p, c_char_p, c_void_p, c_int64, POINTER(c_int64), POINTER(c_int), c_void_p]),
+    "sr3_test_read_gradient": (c_int, [c_void_p, c_char_p, c_int, c_void_p, c_int64, POINTER(c_int64), POINTER(c_int), c_void_p]),
     "sr3_bench_conv": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, POINTER(c_float)]),
     "sr3_test_gemm": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "sr3_test_attention": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
@@ -584,6 +585,19 @@ class Engine:
         t = torch.empty(tuple(shape), device=self.device, dtype=torch.float32)
         _check(lib().sr3_engine_read_activation(self._h, name.encode(), _ptr(t), t.numel(), ctypes.byref(numel), shape, _stream()))
         return t.permute(0, 3, 1, 2).contiguous()
+
+    def read_gradient(self, name, form="g"):
+        """Tests: the gradient the latest backward of this training engine left for the tensor of tap `name` (read_activation's names).
+        form "g": fp32 NCHW [B,C,H,W]; "gb": its bf16 copy, widened to fp32, NCHW; "gsum": its per-image channel sums [B,C].
+        sr3_test_read_gradient."""
+        f = {"g": 0, "gb": 1, "gsum": 2}[form]
+        numel = c_int64()
+        shape = (c_int * 4)()
+        with torch.cuda.device(self.device):
+            _check(lib().sr3_test_read_gradient(self._h, name.encode(), f, c_void_p(0), 0, ctypes.byref(numel), shape, _stream()))
+            t = torch.empty(tuple(shape), device=self.device, dtype=torch.float32)
+            _check(lib().sr3_test_read_gradient(self._h, name.encode(), f, _ptr(t), t.numel(), ctypes.byref(numel), shape, _stream()))
+        return t.view(shape[0], shape[3]) if f == 2 else t.permute(0, 3, 1, 2).contiguous()
 
 
 def window_grid(length, side, overlap):

@@ -2640,6 +2640,38 @@ int sr3_engine_read_activation(sr3_engine* e, const char* name, float* dst, int6
     API_END
 }
 
+int sr3_test_read_gradient(sr3_engine* e, const char* name, int form, float* dst, int64_t cap, int64_t* numel, int shape_bhwc[4], void* stream) {
+    API_BEGIN
+    REQUIRE(e && name, "null argument");
+    REQUIRE(e->train, "engine was not created with sr3_engine_create_train: it keeps no gradients");
+    REQUIRE(form >= 0 && form <= 2, "bad gradient form %d (0 g, 1 gb, 2 gsum)", form);
+    auto it = e->taps.find(name);
+    REQUIRE(it != e->taps.end(), "no activation tap named %s", name);
+    const Act& a = it->second;
+    const int64_t n = form == 2 ? (int64_t)e->B * a.C : (int64_t)e->B * a.H * a.W * a.C;
+    if (numel) *numel = n;
+    if (shape_bhwc) {
+        shape_bhwc[0] = e->B; shape_bhwc[1] = form == 2 ? 1 : a.H; shape_bhwc[2] = form == 2 ? 1 : a.W; shape_bhwc[3] = a.C;
+    }
+    if (dst) {
+        REQUIRE(cap >= n, "destination too small");
+        cudaStream_t st = static_cast<cudaStream_t>(stream);
+        CK(cudaSetDevice(e->dev));
+        if (form == 0) CK(cudaMemcpyAsync(dst, a.g, n * 4, cudaMemcpyDeviceToDevice, st));
+        else if (form == 2) CK(cudaMemcpyAsync(dst, a.gsum, n * 4, cudaMemcpyDeviceToDevice, st));
+        else {   // widened on the host (bf16 is the top half of an fp32): a test read needs no kernel of its own
+            std::vector<uint16_t> hb(n);
+            std::vector<uint32_t> hf(n);
+            CK(cudaMemcpyAsync(hb.data(), a.gb, n * sizeof(uint16_t), cudaMemcpyDeviceToHost, st));
+            CK(cudaStreamSynchronize(st));
+            for (int64_t i = 0; i < n; ++i) hf[i] = (uint32_t)hb[i] << 16;
+            CK(cudaMemcpyAsync(dst, hf.data(), n * 4, cudaMemcpyHostToDevice, st));
+        }
+        CK(cudaStreamSynchronize(st));
+    }
+    API_END
+}
+
 int sr3_test_gemm(const void* a, const void* b, float* dptr, int M, int N, int K, int block_n, void* stream) {
     API_BEGIN
     REQUIRE(M % 128 == 0 && K % 64 == 0 && N % block_n == 0, "bad test gemm shape");

@@ -278,6 +278,12 @@ int sr3_engine_profile_step(sr3_engine* e, int t, int reps, int cap, int* kinds,
  * (DEVICE, [B,H,W,C]); returns C*H*W*B through *numel.  The tap of a layer with self-attention is the attention's output; the output of
  * its ResnetBlock, the attention's input, is the tap "<layer>.res_block" ("mid.0.res_block"). */
 int sr3_engine_read_activation(sr3_engine* e, const char* name, float* dst, int64_t cap, int64_t* numel, int shape_bhwc[4], void* stream);
+/* Tests, read-only: the gradient a training engine's latest backward left for the tensor of tap `name` (the names of
+ * sr3_engine_read_activation), the first B images, into DEVICE fp32 dst.  form 0: g, the fp32 gradient, NHWC [B,H,W,C]; form 1: gb, its
+ * bf16 copy (the operand of the producing layer's data and weight gradients), widened to fp32, [B,H,W,C]; form 2: gsum, its per-image
+ * channel sums (the bias gradients), [B,C] (shape_bhwc {B, 1, 1, C}).  *numel and shape_bhwc are written whether or not dst is given.
+ * Refused on an engine not created for training, which keeps no gradients.  Synchronises `stream`. */
+int sr3_test_read_gradient(sr3_engine* e, const char* name, int form, float* dst, int64_t cap, int64_t* numel, int shape_bhwc[4], void* stream);
 
 /* Stand-alone tile GEMM for unit tests: D[M,N] = A[M,K] * B[N,K]^T (bf16 row-major DEVICE inputs, fp32 output), M%128==0,
  * K%64==0, N%block_n==0. */

@@ -49,8 +49,21 @@ def state_dict(cfg, seed):
     return sd
 
 
+class _Round(torch.autograd.Function):
+    """bf16 rounding of an operand, with the pass-through backward of the plan's gradients: a product's gradient reaches the unrounded
+    value it was rounded from (tests/_layer_grad_ref.py differentiates these functions)."""
+    @staticmethod
+    def forward(ctx, v):
+        ctx.dtype = v.dtype
+        return v.to(torch.bfloat16).to(torch.float64)
+
+    @staticmethod
+    def backward(ctx, g):
+        return g.to(ctx.dtype)
+
+
 def bf(v):
-    return v.to(torch.bfloat16).to(torch.float64)
+    return _Round.apply(v)
 
 
 def operand(v, mode):
