@@ -26,7 +26,8 @@ def build_train_net(unet, image_size, seed, loss_type="l1", sched=SCHED, conditi
 
 
 def oracle_cfg(unet, image_size):
-    return orc.UNetConfig(in_channel=unet["in_channel"], out_channel=unet["out_channel"], inner_channel=unet["inner_channel"], norm_groups=32,
+    return orc.UNetConfig(in_channel=unet["in_channel"], out_channel=unet["out_channel"], inner_channel=unet["inner_channel"],
+                          norm_groups=unet.get("norm_groups", 32),
                           channel_mults=tuple(unet["channel_multiplier"]), attn_res=tuple(unet["attn_res"]), res_blocks=unet["res_blocks"],
                           dropout=unet["dropout"], image_size=image_size)
 

@@ -12,9 +12,11 @@ import torch
 pytestmark = pytest.mark.gpu
 
 U32 = 2.0 ** -24           # fp32 unit roundoff
-# (nz, Lt, HW, C): 8x8 and 4x4 images sharing a 128-token batch (precise mode and the training forward), 256-token batches, and the batches
-# of the 16->128 config at 128x256 (512 tokens) and at 512x512 (4096 tokens)
-UNFUSED = [(1, 128, 64, 128), (3, 128, 16, 256), (2, 256, 256, 512), (1, 512, 512, 512), (2, 1024, 1024, 256), (1, 4096, 4096, 512)]
+# (nz, Lt, HW, C): 8x8 and 4x4 images sharing a 128-token batch (precise mode and the training forward), 256-token batches, the batches
+# of the 16->128 config at 128x256 (512 tokens) and at 512x512 (4096 tokens), and the C = 1024 middle block of the 64->512 config at
+# 512x512 (1024 tokens) and at 128x128 (8x8, two images per batch)
+UNFUSED = [(1, 128, 64, 128), (3, 128, 16, 256), (2, 256, 256, 512), (1, 512, 512, 512), (2, 1024, 1024, 256), (1, 4096, 4096, 512),
+           (1, 1024, 1024, 1024), (2, 128, 64, 1024)]
 
 
 def rel(a, b):

@@ -1,8 +1,8 @@
 """Kernel-level tests of the training backward (csrc/train_kernels.cuh, csrc/train_plan.inc) against fp64 references on the CPU, through
 hooks that build their launches with the training plan's own helpers (engine.cu: gn_op / prep_launch / gn_bwd_launch, combine_launch,
 dgrad_pack_desc and the data-gradient ConvArgs, the attention-backward GemmDescs and WgradOut views, launch_film_bwd / launch_embed_bwd,
-launch_loss_grad).  Shapes follow the configs the project ships: channels 64 .. 1024 (the skip concats of the 16->128 config make 192, 384,
-768 and 1024), 4x4 .. 128x128 pixels, batches 1, 3 and 16.
+launch_loss_grad).  Shapes follow the configs the project ships: channels 64 .. 2048 (the skip concats of the 16->128 config make 192, 384,
+768 and 1024, those of the 64->512 config up to 2048 at 16 groups), 4x4 .. 512x512 pixels, batches 1, 3 and 16.
 
 Unless a test says otherwise a result is held to a relative L2 error and, element-wise, to 1e-4 (|ref| + rms(ref)); the first element out of
 bound is reported by its index ((image, pixel, channel) for activations).
@@ -77,6 +77,13 @@ GN_CASES = [
     (3, 12, 12, 128, 0, 32, True, False, False, 0.0, ("philox", 0.5, 7, 0)),
     (3, 8, 8, 512, 0, 32, True, False, False, 0.0, ("mask", 0.1)),
     (1, 32, 32, 64, 0, 32, True, False, False, 0.0, ("mask", 0.3)),
+    # 16 groups (sr_sr3_64_512)
+    (2, 32, 32, 1024, 1024, 16, True, True, True, 0.0, None),     # 2048: 512-thread blocks, 128-channel groups
+    (2, 32, 32, 1024, 512, 16, True, True, True, 0.0, None),      # 1536: 384 threads, group 10 = channels 960..1055 spans both
+    (2, 64, 64, 512, 256, 16, True, False, True, 0.0, None),      # 768: group 10 = channels 480..527 spans both
+    (1, 512, 512, 64, 0, 16, True, False, True, 0.0, None),       # 262 144 pixels, group size 4
+    (2, 32, 32, 256, 0, 16, True, True, True, 60.0, None),        # |mean| / std ~ 60
+    (2, 8, 8, 1024, 1024, 16, True, False, False, 0.0, ("philox", 0.2, 0x5EED0000C0FFEE, 9)),   # Philox at 2048 channels
 ]
 
 
@@ -284,7 +291,8 @@ def attention_operands(nz, Lt, HW, C, g):
     return qk, vT, P, dO, inside
 
 
-@pytest.mark.parametrize("nz,Lt,HW,C", [(2, 256, 256, 512), (2, 128, 64, 256), (1, 128, 16, 128), (3, 128, 16, 256)])
+@pytest.mark.parametrize("nz,Lt,HW,C", [(2, 256, 256, 512), (2, 128, 64, 256), (1, 128, 16, 128), (3, 128, 16, 256), (2, 128, 64, 1024),
+                                        (1, 128, 16, 1024)])
 def test_attention_backward_matches_fp64(nz, Lt, HW, C):
     """bwd_attention from the transposes to the bf16 copy of d(qkv): dP = dO V^T and dQ = dS K on the tile kernel, softmax_bwd_kernel over
     HW-token segments, dK = dS^T Q (Q read through the 16-wide view inside the q|k rows) and dV = P^T dO on the weight-gradient kernel.

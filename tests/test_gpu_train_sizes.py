@@ -63,6 +63,32 @@ def test_gradients_match_oracle_l2(name):
     assert not bad, bad[:10]
 
 
+SR64_512 = dict(in_channel=6, out_channel=3, inner_channel=64, norm_groups=16, channel_multiplier=[1, 2, 4, 8, 16], attn_res=[], res_blocks=1,
+                dropout=0.0)     # sr_sr3_64_512.json's UNet
+
+
+@pytest.mark.timeout(1800)
+def test_gradients_64_512_config_match_oracle_l2():
+    """sr_sr3_64_512's UNet (16 GroupNorm groups, concats up to 2048 channels, the C = 1024 middle attention) trained on a 128x128 batch of
+    2: the loss within 1e-2 and every one of its parameter gradients within GRAD_TOL of the oracle's fp32 autograd.  (Its 16-group
+    forward is pinned to the reference by the big_64_512 golden, tests/test_oracle.py.)"""
+    b, h = 2, 128
+    net = tu.build_train_net(SR64_512, 512, ti.SEED, "l2", ti.SCHED)
+    hr, sr, noise = ti.batch(b, h, h, 2000)
+    gamma = tu.draw_gamma(b, ti.NP_SEED)
+    lo, go = tu.ours_loss_and_grads(net, hr, sr, gamma, noise)
+    assert (b, h, h, "cuda:0", True, 3, "bf16", 0.0) in net.denoise_fn._engines
+    torch.set_num_threads(min(16, torch.get_num_threads()))
+    lr_, gr = tu.oracle_loss_and_grads(net, SR64_512, 512, hr, sr, gamma, noise, "l2")
+    assert abs(lo - lr_) / abs(lr_) < 1e-2, (lo, lr_)
+    assert set(go) == set(gr)
+    rows = tu.compare(go, gr)
+    worst = sorted(rows, key=lambda r: -r[1])[:5]
+    print(f"sr64_512 at {h}x{h}, {len(rows)} parameter tensors, loss {lo:.6g} vs {lr_:.6g}; worst:", [(n, f"{e:.2e}") for n, e, _, _ in worst])
+    bad = [(n, e, c) for n, e, c, _ in rows if e >= GRAD_TOL]
+    assert not bad, bad[:10]
+
+
 def test_gradients_unconditional_model_non_square():
     lo, go, lr_, gr = compare_with_oracle("tiny_64x32", conditional=False)
     assert abs(lo - lr_) / abs(lr_) < 1e-2, (lo, lr_)
@@ -162,11 +188,13 @@ def test_philox_dropout_at_a_non_square_size(name):
 
 # ------------------------------------------------------------------------------------------------ kernels at the new geometries
 @pytest.mark.timeout(600)
-@pytest.mark.parametrize("nz,Lt,HW,C", [(1, 512, 512, 256), (1, 1024, 1024, 128), (2, 512, 512, 512), (1, 4096, 4096, 128)])
+@pytest.mark.parametrize("nz,Lt,HW,C", [(1, 512, 512, 256), (1, 1024, 1024, 128), (2, 512, 512, 512), (1, 4096, 4096, 128),
+                                        (1, 1024, 1024, 1024)])
 def test_attention_backward_long_segments_match_fp64(nz, Lt, HW, C):
     """bwd_attention on one image per attention batch of 512 to 4096 tokens (the 16->128 net's attention level at 128x256, 256x256 and
-    512x512): the bounds of test_attention_backward_matches_fp64.  The row dot of the softmax backward and the dK / dV contractions now run
-    over up to 4096 terms in fp32, ~2^-24 sqrt(n) each: still far inside 2e-5."""
+    512x512; the 64->512 net's C = 1024 middle block at 512x512): the bounds of test_attention_backward_matches_fp64.  The row dot of
+    the softmax backward and the dK / dV contractions now run over up to 4096 terms in fp32, ~2^-24 sqrt(n) each: still far inside
+    2e-5."""
     from sr3_b200 import _native
     g = gen("attn", nz, Lt, HW, C)
     qk, vT, P, dO, inside = attention_operands(nz, Lt, HW, C, g)

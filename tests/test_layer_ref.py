@@ -13,9 +13,14 @@ from oracle import sr3_oracle as orc
 
 TINY = orc.UNetConfig(6, 3, 64, 32, (1, 2), (16,), 1, 0.0, 32)
 TINY4 = orc.UNetConfig(6, 3, 64, 32, (1, 2, 2), (), 1, 0.0, 16)
+# the geometry of sr_sr3_64_512 at three levels: 16 GroupNorm groups, no attention but the middle block's; its 192 and 384 concats have 12-
+# and 24-channel groups that straddle the boundary at 128 and 256
+G16 = orc.UNetConfig(6, 3, 64, 16, (1, 2, 4), (), 1, 0.0, 32)
 # (config, batch, height, width): attention at 16x16 (and one- / two-source, identity / res_conv blocks), at 8x8 (the same net on 16x16
-# images: its attention level is then 8x8), at 4x4 (the 4x4 middle of TINY4), and over 512 tokens (16x32 attention of 32x64 images)
-NETS = {"tiny_32x32": (TINY, 2, 32, 32), "tiny_16x16": (TINY, 3, 16, 16), "tiny4_16x16": (TINY4, 3, 16, 16), "tiny_32x64": (TINY, 2, 32, 64)}
+# images: its attention level is then 8x8), at 4x4 (the 4x4 middle of TINY4), over 512 tokens (16x32 attention of 32x64 images), and
+# 16 groups (G16, its 8x8 middle attention with C = 256)
+NETS = {"tiny_32x32": (TINY, 2, 32, 32), "tiny_16x16": (TINY, 3, 16, 16), "tiny4_16x16": (TINY4, 3, 16, 16), "tiny_32x64": (TINY, 2, 32, 64),
+        "g16_32x32": (G16, 2, 32, 32)}
 
 
 def rel(a, b):
@@ -54,14 +59,18 @@ def test_unrounded_layers_are_the_oracle(net):
         e = rel(ref, taps[tap])
         assert e < 1e-12, (name, tap, e)
         kinds.add((kind, skip is not None, kind == "res" and lref.residual(kind, spec, sd, taps[src]) is not None))
+    if name == "g16_32x32":    # 16 groups; concats whose group straddles the boundary (12 channels at 128 + 64, 24 at 256 + 128)
+        straddle = {(taps[src].shape[1], taps[skip].shape[1]) for tap, kind, spec, src, skip in lref.layer_inputs(cfg)
+                    if skip is not None and taps[src].shape[1] % ((taps[src].shape[1] + taps[skip].shape[1]) // cfg.norm_groups)}
+        assert cfg.norm_groups == 16 and straddle == {(128, 64), (256, 128)}, straddle
     if name == "tiny_32x32":   # every kind of layer; ResnetBlocks with one and two sources, identity and res_conv shortcuts
         assert kinds >= {("conv", False, False), ("res", False, True), ("res", False, False), ("res", True, False), ("attn", False, False),
                          ("down", False, False), ("up", False, False), ("final", False, False)}, kinds
 
 
 def test_attention_geometry_of_the_nets():
-    """The attention layers the cases above reach: C = 128 at 16x16, 8x8 and 4x4 (8, 2 images per 128-token batch on the device) and
-    over 512 tokens."""
+    """The attention layers the cases above reach: C = 128 at 16x16, 8x8 and 4x4 (8, 2 images per 128-token batch on the device), over
+    512 tokens, and C = 256 at 8x8 in the 16-group net's middle block."""
     sizes = {}
     for name, (cfg, _, h, w) in NETS.items():
         sizes[name] = set()
@@ -69,7 +78,8 @@ def test_attention_geometry_of_the_nets():
             if kind == "attn":
                 f = cfg.image_size // spec.res
                 sizes[name].add((h // f, w // f))
-    assert sizes == {"tiny_32x32": {(16, 16)}, "tiny_16x16": {(8, 8)}, "tiny4_16x16": {(4, 4)}, "tiny_32x64": {(16, 32)}}, sizes
+    assert sizes == {"tiny_32x32": {(16, 16)}, "tiny_16x16": {(8, 8)}, "tiny4_16x16": {(4, 4)}, "tiny_32x64": {(16, 32)},
+                     "g16_32x32": {(8, 8)}}, sizes
 
 
 def test_folded_upsample_is_conv_of_nearest_2x():
