@@ -100,6 +100,12 @@ _SIGS = {
     "sr3_windowed_phase_begin": (c_int, [c_void_p, c_int, c_void_p]),
     "sr3_windowed_phase_means": (c_int, [c_void_p, c_void_p]),
     "sr3_windowed_phase_merge": (c_int, [c_void_p, c_void_p]),
+    "sr3_stream_create": (c_int, [c_void_p, c_uint64, POINTER(c_void_p)]),
+    "sr3_stream_destroy": (None, [c_void_p]),
+    "sr3_stream_admit": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_uint64, c_void_p]),
+    "sr3_stream_step": (c_int, [c_void_p, c_void_p]),
+    "sr3_stream_retire": (c_int, [c_void_p, c_int, c_void_p, c_void_p]),
+    "sr3_stream_slot_state": (c_int, [c_void_p, POINTER(c_int), POINTER(c_int)]),
     "sr3_engine_profile_step": (c_int, [c_void_p, c_int, c_int, c_int, POINTER(c_int), POINTER(c_float), POINTER(c_double), POINTER(c_double),
                                         POINTER(c_int), c_void_p]),
     "sr3_pil_bicubic_tables": (c_int, [c_int, c_int, POINTER(c_int), POINTER(c_int), c_int, POINTER(c_int)]),
@@ -744,6 +750,90 @@ class WindowedSampler:
         with torch.cuda.device(self.device):
             _check(lib().sr3_windowed_profile_step(self._h, int(t), int(reps), ms, _stream()))
         return {"gather": ms[0], "engine": ms[1], "merge": ms[2]}
+
+
+def stream_plan(arrival_steps, slots, T):
+    """The slot plan of continuous batching: for request n arriving before step arrival_steps[n] (non-decreasing; any iterable, read
+    lazily, one value per request planned), yields (slot, admit_step, finish_step).  Requests are admitted first come first served, each
+    at the first step at which it has arrived, every earlier request has been admitted and a slot is free, into the lowest free slot; it
+    runs steps admit_step .. admit_step + T - 1 and its image is ready after step finish_step - 1 = admit_step + T - 1, so the slot is free
+    again from step finish_step on.  Pure host arithmetic: GaussianDiffusion.super_resolution_stream follows it step for step."""
+    slots, T = int(slots), int(T)
+    if slots < 1 or T < 1:
+        raise ValueError("stream_plan needs slots >= 1 and T >= 1, got slots=%d T=%d" % (slots, T))
+    free_at = [0] * slots
+    last_arrival, last_admit = 0, 0
+    for a in arrival_steps:
+        a = int(a)
+        if a < last_arrival:
+            raise ValueError("arrival steps must be non-decreasing: %d after %d" % (a, last_arrival))
+        last_arrival = a
+        k = max(a, last_admit, min(free_at))
+        slot = next(s for s in range(slots) if free_at[s] <= k)
+        free_at[slot] = k + T
+        last_admit = k
+        yield slot, k, k + T
+
+
+class StreamSampler:
+    """Continuous batching on `engine` (sr3_stream_*): its engine.batch images are slots, each running its own request at its own
+    timestep.  The online interface: a server calls admit() for a request when a slot is free, step() once per reverse step, and
+    retire() for every slot finished() lists.  Borrows the engine (and keeps it alive); nothing else may run on it while requests are in
+    flight."""
+
+    def __init__(self, engine, seed):
+        self.engine = engine
+        self.device = engine.device
+        self.slots = engine.batch
+        self.seed = int(seed)
+        self._h = c_void_p()
+        with torch.cuda.device(self.device):
+            _check(lib().sr3_stream_create(engine._h, self.seed, ctypes.byref(self._h)))
+
+    def __del__(self):
+        try:
+            if getattr(self, "_h", None):
+                lib().sr3_stream_destroy(self._h)
+                self._h = None
+        except Exception:
+            pass
+
+    def _image(self, t, channels, what):
+        t = _f32c(t, self.device)
+        want = (channels, self.engine.height, self.engine.width)
+        if tuple(t.shape) != want:
+            raise ValueError("%s has shape %s; this stream's slots are %s" % (what, tuple(t.shape), want))
+        return t
+
+    def admit(self, slot, condition_x, x_T, sample_index):
+        """Load a request ([C, H, W] condition, None for an unconditional model, and x_T) into free `slot`; its Philox draws are keyed by
+        the global `sample_index`."""
+        c = None if condition_x is None else self._image(condition_x, self.engine.in_channel - self.engine.channels, "condition_x")
+        x = self._image(x_T, self.engine.channels, "x_T")
+        with torch.cuda.device(self.device):
+            _check(lib().sr3_stream_admit(self._h, int(slot), _ptr(c), _ptr(x), int(sample_index), _stream()))
+
+    def step(self, n=1):
+        with torch.cuda.device(self.device):
+            for _ in range(int(n)):
+                _check(lib().sr3_stream_step(self._h, _stream()))
+
+    def slot_state(self):
+        """(t, state) per slot: state 0 free, 1 running (t = timestep of its next step), 2 finished, waiting for retire()."""
+        t, st = (c_int * self.slots)(), (c_int * self.slots)()
+        _check(lib().sr3_stream_slot_state(self._h, t, st))
+        return list(t), list(st)
+
+    def finished(self):
+        """The slots whose image is ready."""
+        return [s for s, v in enumerate(self.slot_state()[1]) if v == 2]
+
+    def retire(self, slot):
+        """x_0 [C, H, W] of finished `slot`; frees the slot."""
+        out = torch.empty(self.engine.channels, self.engine.height, self.engine.width, device=self.device, dtype=torch.float32)
+        with torch.cuda.device(self.device):
+            _check(lib().sr3_stream_retire(self._h, int(slot), _ptr(out), _stream()))
+        return out
 
 
 def bench_conv(B, H, W, Cin, Cout, k=3, stride=1, resid=False, stats=True, reps=20):

@@ -231,6 +231,95 @@ class GaussianDiffusion(nn.Module):
             return torch.cat([first, snaps.reshape(-1, *shape[1:])], dim=0)
         return final[-1]
 
+    # ---- continuous batching: a stream of requests, see DESIGN.md 3.10
+    def super_resolution_stream(self, requests, slots=16, seed=None, first_index=0):
+        """Super-resolve a stream of requests with continuous batching: a generator over `requests`, any iterable (read lazily, one
+        request per free slot) of (key, x_in) or (key, x_in, x_T) with x_in [C, H, W].  The engine runs `slots` images, each at its own
+        timestep; a request takes the lowest free slot at the next step (_native.stream_plan) and its (key, image [C, H, W]) is yielded
+        as soon as its T steps are done, so a new request waits for a free slot, not for a whole batch.  The n-th request's draws are
+        keyed by sample index first_index + n (x_T ~ randn when not given): its image is the one super_resolution computes for it at
+        that sample index.  Every request must have the first one's size (ValueError before it is admitted); a schedule change while
+        requests are in flight makes the next step raise."""
+        if not self.conditional:
+            raise ValueError("super_resolution_stream needs a conditional model; use sample_stream")
+        return self._stream(requests, slots, seed, first_index)
+
+    def sample_stream(self, n, slots=16, seed=None):
+        """sample() for n images of image_size through the continuous-batching engine; yields (index, image [C, H, W])."""
+        if self.conditional:
+            raise ValueError("sample_stream needs an unconditional model; use super_resolution_stream")
+        return self._stream(((i, None) for i in range(int(n))), slots, seed, 0)
+
+    def _stream_request(self, req, size):
+        """(key, cond, x_T or None, (H, W)) of one request, checked against the stream's size (None for the first request)."""
+        from ... import _native
+        if not isinstance(req, (tuple, list)) or len(req) not in (2, 3):
+            raise ValueError("a request is (key, x_in) or (key, x_in, x_T), got %r" % (type(req),))
+        key, x_in, x_T = (tuple(req) + (None,))[:3]
+        if self.conditional:
+            cond_c = self.denoise_fn.arch["in_channel"] - self.channels
+            if not torch.is_tensor(x_in) or x_in.dim() != 3 or x_in.shape[0] != cond_c:
+                raise ValueError("request %r: x_in must be [%d, H, W], got %s" % (key, cond_c, tuple(getattr(x_in, "shape", ()))))
+            hw = (int(x_in.shape[1]), int(x_in.shape[2]))
+        else:
+            hw = (self.image_size, self.image_size)
+        if size is None:
+            _native.check_image_size(len(self.denoise_fn.arch["channel_mults"]), *hw)
+        elif hw != size:
+            raise ValueError("request %r is %dx%d; this stream runs %dx%d (each size needs its own stream)" % (key, *hw, *size))
+        if x_T is not None and tuple(x_T.shape) != (self.channels,) + hw:
+            raise ValueError("request %r: x_T must be %s, got %s" % (key, (self.channels,) + hw, tuple(x_T.shape)))
+        return key, x_in, x_T, hw
+
+    @torch.no_grad()
+    def _stream(self, requests, slots, seed, first_index):
+        from ... import _native
+        slots = int(slots)
+        if slots < 1:
+            raise ValueError("slots must be >= 1, got %d" % slots)
+        device = self.betas.device
+        if seed is None:
+            seed = int(torch.randint(0, 2 ** 62, (1,)).item())
+        reqs = iter(requests)
+        size, sampler, plan = None, None, None
+        step, n, exhausted = 0, 0, False
+        running = {}                           # slot -> (key, finish step)
+        while True:
+            # the requests admitted at this step: one per free slot, all checked before the first of them is admitted
+            batch = []
+            while not exhausted and len(running) + len(batch) < slots:
+                try:
+                    req = next(reqs)
+                except StopIteration:
+                    exhausted = True
+                    break
+                key, cond, x_T, size = self._stream_request(req, size)
+                batch.append((key, cond, x_T))
+            if batch and sampler is None:
+                eng = self._engine(slots, *size)
+                if eng.T == 0:
+                    raise RuntimeError("set_new_noise_schedule has not been called")
+                sampler, T = _native.StreamSampler(eng, seed), eng.T
+                clock = [0]
+                plan = _native.stream_plan(iter(lambda: clock[0], None), slots, T)     # every request arrives when it is read
+            if batch and sampler.engine.T != T:
+                raise RuntimeError("sr3_b200: the noise schedule changed during the stream (n_timestep %d -> %d)" % (T, sampler.engine.T))
+            for key, cond, x_T in batch:
+                slot, admit, finish = next(plan)
+                assert admit == step and slot not in running, (slot, admit, step)
+                if x_T is None:
+                    x_T = torch.randn((self.channels,) + size, device=device)
+                sampler.admit(slot, cond, x_T, first_index + n)
+                n += 1
+                running[slot] = (key, finish)
+            if not running:
+                return
+            sampler.step()
+            step += 1
+            clock[0] = step
+            for slot in sorted(s for s, (_, f) in running.items() if f == step):
+                yield running.pop(slot)[0], sampler.retire(slot)
+
     def q_sample(self, x_start, continuous_sqrt_alpha_cumprod, noise=None):
         noise = torch.randn_like(x_start) if noise is None else noise
         return continuous_sqrt_alpha_cumprod * x_start + (1 - continuous_sqrt_alpha_cumprod ** 2).sqrt() * noise

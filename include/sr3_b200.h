@@ -235,6 +235,32 @@ int sr3_windowed_phase_begin(sr3_windowed* w, int t_start, void* stream);
 int sr3_windowed_phase_means(sr3_windowed* w, void* stream);
 int sr3_windowed_phase_merge(sr3_windowed* w, void* stream);
 
+/* ---- continuous batching: serve a stream of requests on one inference engine, every slot (one of the engine's B images) at its own
+ * timestep.  A slot takes a request (sr3_stream_admit), runs exactly T reverse steps, one per sr3_stream_step, and then holds x_0 until
+ * sr3_stream_retire copies it out and frees the slot.  A step is the engine's step graph in its UNet.forward form (eps of every image,
+ * noise level of slot s = sqrt_alphas_cumprod_prev[t_s + 1]) followed by one kernel that applies p_sample's posterior update to every
+ * running slot at its own t_s, with z from Philox keyed by (seed, the request's sample_index, pixel, t_s), and advances the slots.  Every
+ * UNet op is per image, so a request's x_0 equals what sr3_p_sample_loop computes for the same condition, x_T and sample index
+ * (first_sample_index + b = sample_index) at the same slot b, bit for bit, whatever the other slots hold.  No step synchronises the host
+ * or copies to it: the host mirrors the slot table, since every request takes exactly T steps.
+ * The stream BORROWS the engine (which must outlive it) and its buffers: nothing else may run on that engine while requests are in flight,
+ * and all calls of one stream go to one CUDA stream.  Creating a stream zeroes the engine's state and input; retiring a slot zeroes
+ * that slot's. */
+typedef struct sr3_stream sr3_stream;
+int sr3_stream_create(sr3_engine* e, uint64_t seed, sr3_stream** out);
+void sr3_stream_destroy(sr3_stream* s);
+/* Load one request into a free slot: condition_x (NULL for an unconditional model) and x_T DEVICE fp32 [3,H,W] at the engine's H x W
+ * (copied); its first step runs at t = T - 1.  Refused, with no slot changed: a slot out of range or busy (running, or finished and not
+ * retired), an engine with no schedule, a schedule changed since the requests in flight were admitted. */
+int sr3_stream_admit(sr3_stream* s, int slot, const float* condition_x, const float* x_T, uint64_t sample_index, void* stream);
+/* One reverse step of every running slot.  Refused when the engine has no schedule or sr3_engine_set_schedule was called while requests
+ * are in flight (they would finish on a mixed schedule). */
+int sr3_stream_step(sr3_stream* s, void* stream);
+/* Copy the x_0 of a finished slot to `out` (DEVICE fp32 [3,H,W]) and free the slot.  Refuses a running or free slot. */
+int sr3_stream_retire(sr3_stream* s, int slot, float* out, void* stream);
+/* HOST t[B], state[B]: state 0 free, 1 running (t = timestep of its next step), 2 finished and not yet retired (t = -1). */
+int sr3_stream_slot_state(const sr3_stream* s, int* t, int* state);
+
 /* core/metrics.py:8-34 `tensor2img` on the device: src fp32 DEVICE [n][C][H][W] -> clamp to [min_v, max_v] -> [0, 1] -> * 255, round half
  * to even -> uint8 DEVICE, HWC.  n == 1: dst [H][W][C].  n > 1: the images are tiled like torchvision.utils.make_grid(nrow, padding 2,
  * pad_value 0), which is what the reference does for 4-D input: dst [rows*(H+2)+2][cols*(W+2)+2][C], cols = min(nrow, n).
