@@ -24,7 +24,8 @@ its weight gradient contracts bf16(y.g) with bf16 of the nearest-2x input.
 rounded=False turns every rounding off (plain fp64); off={points} turns single gradient-rounding points off.  wrong= selects a wrong
 reference of the wiring: "gn_per_source" (GroupNorm statistics of a group that straddles the concat taken per source), "joint_softmax"
 (the softmax, forward and backward, over the whole 128-token attention batch instead of per image), "per_tap" (the Upsample data
-gradient with per-tap rounded weights)."""
+gradient with per-tap rounded weights), "gn_neighbour" (every GroupNorm of the layer, forward and backward, with the statistics of image
+(b + 1) mod B for image b: _layer_ref's gn_stats)."""
 import math
 
 import torch
@@ -120,6 +121,7 @@ def layer_grads(sd, cfg, kind, spec, x, skip, nl, gy, keep_scale=None, rounded=T
         return psd[name].view(1, -1, 1, 1)
 
     out, extra, g = None, {}, cfg.norm_groups
+    st = lref.neighbour(x.shape[0]) if wrong == "gn_neighbour" else None
     if kind == "conv":
         out = gr(conv(X, "downs.0.weight", 1), "gy") + bias("downs.0.bias")
     elif kind == "res":
@@ -128,11 +130,11 @@ def layer_grads(sd, cfg, kind, spec, x, skip, nl, gy, keep_scale=None, rounded=T
         if wrong == "gn_per_source":
             n1 = gn_per_source(xin, X.shape[1], psd[p + ".block1.block.0.weight"], psd[p + ".block1.block.0.bias"], g)
         else:
-            n1 = lref._gn(xin, psd, p + ".block1.block.0", g)
+            n1 = lref._gn(xin, psd, p + ".block1.block.0", g, st)
         film = _leaf(lref.film_rows(sd, p, nl, cfg.inner_channel), dev)
         extra["film"] = film
         h = gr(conv(lref._silu(n1), p + ".block1.block.3.weight", 1), "dh") + film[:, :, None, None]
-        a2 = lref._silu(lref._gn(h, psd, p + ".block2.block.0", g))
+        a2 = lref._silu(lref._gn(h, psd, p + ".block2.block.0", g, st))
         if keep_scale is not None:
             a2 = a2 * keep_scale.to(dev, torch.float64)
         br = conv(a2, p + ".block2.block.3.weight", 1)
@@ -144,7 +146,7 @@ def layer_grads(sd, cfg, kind, spec, x, skip, nl, gy, keep_scale=None, rounded=T
         p = spec.name + ".attn"
         B, C, H, W = X.shape
         HW = H * W
-        qkv = gr(conv(lref._gn(X, psd, p + ".norm", g), p + ".qkv.weight", 0), "dqkv").view(B, 3, C, HW).transpose(2, 3)
+        qkv = gr(conv(lref._gn(X, psd, p + ".norm", g, st), p + ".qkv.weight", 0), "dqkv").view(B, 3, C, HW).transpose(2, 3)
         q, k, v = r(qkv[:, 0]), r(qkv[:, 1]), r(qkv[:, 2])             # [B, HW, C]
         per = max(1, 128 // HW) if wrong == "joint_softmax" else 1     # images sharing one softmax
         os = []
@@ -180,7 +182,7 @@ def layer_grads(sd, cfg, kind, spec, x, skip, nl, gy, keep_scale=None, rounded=T
         res.update({n: psd[n].grad for n in names})
         return res
     else:
-        a = lref._silu(lref._gn(X, psd, "final_conv.block.0", g))
+        a = lref._silu(lref._gn(X, psd, "final_conv.block.0", g, st))
         out = gr(conv(a, "final_conv.block.3.weight", 1), "gy") + bias("final_conv.block.3.bias")
     out.backward(gy.to(dev, torch.float64))
     res = {"out": out.detach()}

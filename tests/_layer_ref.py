@@ -23,6 +23,10 @@ unfused=True (the training plan in bf16): P = bf16(softmax), O = bf16(P v).
 
 rounded=False turns every rounding off: what is left is plain fp64 arithmetic of the layer.
 
+gn_stats (a wrong reference): every GroupNorm of the layer normalises image b with the statistics of image gn_stats[b] (neighbour(B):
+those of image (b + 1) mod B), what a per-image statistics run restarted at the wrong row would give.  With the identity it is the
+default reference bit for bit.
+
 The functions run on the device of their inputs (the GPU test keeps its fp64 references on the GPU)."""
 import math
 
@@ -92,8 +96,21 @@ def _p(sd, name, like):
     return sd[name].to(device=like.device, dtype=torch.float64)
 
 
-def _gn(x, sd, prefix, groups):
-    return F.group_norm(x, groups, _p(sd, prefix + ".weight", x), _p(sd, prefix + ".bias", x), eps=EPS)
+def _gn(x, sd, prefix, groups, stats=None):
+    """GroupNorm of x; stats: image b normalised with the mean and variance of image stats[b] (a wrong reference).  That is GroupNorm of
+    the stats image plus the difference of the two images in its scale, an exact zero for stats[b] == b."""
+    gamma, beta = _p(sd, prefix + ".weight", x), _p(sd, prefix + ".bias", x)
+    if stats is None:
+        return F.group_norm(x, groups, gamma, beta, eps=EPS)
+    xs = x[list(stats)]
+    B, C = x.shape[:2]
+    rstd = torch.rsqrt(xs.reshape(B, groups, -1).var(-1, unbiased=False) + EPS).repeat_interleave(C // groups, 1)
+    return F.group_norm(xs, groups, gamma, beta, eps=EPS) + (x - xs) * (rstd * gamma)[:, :, None, None]
+
+
+def neighbour(b):
+    """The GroupNorm statistics of image (i + 1) mod b for image i (gn_stats)."""
+    return [(i + 1) % b for i in range(b)]
 
 
 def _silu(x):
@@ -123,15 +140,15 @@ def film_rows(sd, prefix, noise_level, inner):
             + _p(sd, prefix + ".block1.block.3.bias", nl))
 
 
-def res_block(sd, prefix, x, skip, film, groups, precision="bf16", rounded=True, keep_scale=None):
+def res_block(sd, prefix, x, skip, film, groups, precision="bf16", rounded=True, keep_scale=None, gn_stats=None):
     """ResnetBlock `prefix` on x [B, C0, H, W] (+ skip [B, C1, H, W]); film [B, cout] from film_rows; keep_scale: the scaled Dropout
     keep-mask [B, cout, H, W] of block2 (training plan), or None."""
     mode = _mode(precision, rounded)
     x = x.to(torch.float64)
     xin = x if skip is None else torch.cat([x, skip.to(torch.float64)], 1)
-    a1 = _silu(_gn(xin, sd, prefix + ".block1.block.0", groups))
+    a1 = _silu(_gn(xin, sd, prefix + ".block1.block.0", groups, gn_stats))
     h = product(_conv(1), a1, _p(sd, prefix + ".block1.block.3.weight", x), mode) + film.to(x.device, torch.float64)[:, :, None, None]
-    a2 = _silu(_gn(h, sd, prefix + ".block2.block.0", groups))
+    a2 = _silu(_gn(h, sd, prefix + ".block2.block.0", groups, gn_stats))
     if keep_scale is not None:
         a2 = a2 * keep_scale.to(x.device, torch.float64)
     y = product(_conv(1), a2, _p(sd, prefix + ".block2.block.3.weight", x), mode) + _bias(sd, prefix + ".block2.block.3.bias", x)
@@ -140,12 +157,12 @@ def res_block(sd, prefix, x, skip, film, groups, precision="bf16", rounded=True,
     return y + x
 
 
-def attention(sd, prefix, y, groups, precision="bf16", rounded=True, unfused=False):
+def attention(sd, prefix, y, groups, precision="bf16", rounded=True, unfused=False, gn_stats=None):
     """SelfAttention `prefix` ("mid.0.attn") on its ResnetBlock's output y [B, C, H, W]."""
     mode = _mode(precision, rounded)
     y = y.to(torch.float64)
     B, C, H, W = y.shape
-    n = _gn(y, sd, prefix + ".norm", groups)
+    n = _gn(y, sd, prefix + ".norm", groups, gn_stats)
     qkv = product(_conv(0), n, _p(sd, prefix + ".qkv.weight", y), mode).view(B, 3, C, H * W).transpose(2, 3)    # [B, 3, HW, C]
     q, k, v = qkv[:, 0], qkv[:, 1], qkv[:, 2]
     if mode == "bf16" and not unfused:
@@ -206,9 +223,9 @@ def upsample(sd, name, x, precision="bf16", rounded=True, fold=True):
     return out + b
 
 
-def final_block(sd, x, groups, precision="bf16", rounded=True):
+def final_block(sd, x, groups, precision="bf16", rounded=True, gn_stats=None):
     x = x.to(torch.float64)
-    a = _silu(_gn(x, sd, "final_conv.block.0", groups))
+    a = _silu(_gn(x, sd, "final_conv.block.0", groups, gn_stats))
     return product(_conv(1), a, _p(sd, "final_conv.block.3.weight", x), _mode(precision, rounded)) + _bias(sd, "final_conv.block.3.bias", x)
 
 
@@ -233,7 +250,7 @@ def layer_inputs(cfg):
     return out
 
 
-def layer_reference(sd, cfg, kind, spec, x, skip, nl, precision="bf16", rounded=True, unfused=False, keep_scale=None, film=None):
+def layer_reference(sd, cfg, kind, spec, x, skip, nl, precision="bf16", rounded=True, unfused=False, keep_scale=None, film=None, gn_stats=None):
     """One entry of layer_inputs evaluated on the given input (and skip) activations."""
     g = cfg.norm_groups
     if kind == "conv":
@@ -242,14 +259,14 @@ def layer_reference(sd, cfg, kind, spec, x, skip, nl, precision="bf16", rounded=
         p = spec.name + ".res_block"
         if film is None:
             film = film_rows(sd, p, nl, cfg.inner_channel)
-        return res_block(sd, p, x, skip, film, g, precision, rounded, keep_scale)
+        return res_block(sd, p, x, skip, film, g, precision, rounded, keep_scale, gn_stats)
     if kind == "attn":
-        return attention(sd, spec.name + ".attn", x, g, precision, rounded, unfused)
+        return attention(sd, spec.name + ".attn", x, g, precision, rounded, unfused, gn_stats)
     if kind == "down":
         return downsample(sd, spec.name, x, precision, rounded)
     if kind == "up":
         return upsample(sd, spec.name, x, precision, rounded)
-    return final_block(sd, x, g, precision, rounded)
+    return final_block(sd, x, g, precision, rounded, gn_stats)
 
 
 def residual(kind, spec, sd, x):

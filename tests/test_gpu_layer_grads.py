@@ -138,11 +138,11 @@ def bound_of(cls, k):
     return bound * f, elem * f
 
 
-def make_engine(name):
-    """A bf16 training engine of the case with its weights (lref.state_dict) and, for a case with Dropout, injected keep-masks.
-    -> (cfg, sd, engine, {ResnetBlock tap: scaled keep-mask, fp64 on the GPU})."""
+def make_engine(case):
+    """A bf16 training engine of a case tuple (CASES' form) with its weights (lref.state_dict) and, for a case with Dropout, injected
+    keep-masks.  -> (cfg, sd, engine, {ResnetBlock tap: scaled keep-mask, fp64 on the GPU})."""
     from sr3_b200 import _native
-    net, image_size, b, h, w, drop = CASES[name]
+    net, image_size, b, h, w, drop = case
     cfg = tgl.oracle_cfg(net, image_size)
     sd = lref.state_dict(cfg, 5)
     eng = _native.Engine(tgl.engine_cfg(cfg, image_size, "bf16"), b, torch.device("cuda", torch.cuda.current_device()),
@@ -162,13 +162,14 @@ def make_engine(name):
     return cfg, sd, eng, keeps
 
 
-def run_backward(name):
-    """One forward and one backward of the case: everything the engine leaves, in fp64 on the GPU."""
-    net, image_size, b, h, w, drop = CASES[name]
-    cfg, sd, eng, keeps = make_engine(name)
-    g = torch.Generator().manual_seed(tgl.case_seed(CASES, name))
+def run_backward(case, seed):
+    """One forward and one backward of a case tuple, inputs drawn from `seed`: everything the engine leaves, in fp64 on the GPU, and its
+    tile_schedules() (the forward's tile plan)."""
+    net, image_size, b, h, w, drop = case
+    cfg, sd, eng, keeps = make_engine(case)
+    g = torch.Generator().manual_seed(seed)
     x = torch.randn(b, cfg.in_channel, h, w, generator=g)
-    nl = torch.tensor(tgl.NOISE_LEVELS[:b])
+    nl = tgl.noise_levels(b)
     workspace = eng.workspace_bytes()
     eps, _ = eng.train_unet_forward(x.cuda(), nl.cuda())
     taps = {"input": x.cuda().double()}
@@ -181,9 +182,10 @@ def run_backward(name):
     dx, _ = eng.train_unet_backward(deps.cuda(), grads, want_dx=True)
     torch.cuda.synchronize()
     gt = {tap: {f: eng.read_gradient(tap, f).double() for f in ("g", "gb", "gsum")} for tap in taps if tap != "input"}
-    out = dict(cfg=cfg, sd={k: v.cuda() for k, v in sd.items()}, nl=nl.cuda(), keeps=keeps, taps=taps, gt=gt, deps=deps.cuda().double(),
+    out = dict(cfg=cfg, sd={k: v.cuda() for k, v in sd.items()}, nl=nl.cuda(), keeps=keeps, taps=taps, eps=eps.double(), gt=gt,
+               deps=deps.cuda().double(),
                dx=dx.double(), dfilm=eng.film_state()["dfilm"][:b].double(), pgrads={n: t.double() for (n, _), t in zip(table, grads)},
-               workspace=workspace)
+               workspace=workspace, plan=eng.tile_schedules())
     del eng
     return out
 
@@ -204,6 +206,21 @@ def elementwise(got, ref, resid, elem):
     i = tuple(bad[0].tolist())
     return ratio.max().item(), (f"{bad.shape[0]} elements past {elem:.0e} (|b| + rms(b)), first at index {i}: got {got[i].item():.7g}, "
                                 f"want {ref[i].item():.7g} (bound {elem * scale[i].item():.2e})")
+
+
+def identity_failures(gt):
+    """The exact identities of every tap's gradient {tap: {"g", "gb", "gsum"}}: gb == bf16(g) bit for bit, and gsum the pixel sums of g to
+    within 1e-5 of the sums of |g|.  -> the failures."""
+    failures = []
+    for tap, v in gt.items():
+        gg = v["g"]
+        assert torch.isfinite(gg).all(), tap
+        if not torch.equal(v["gb"], gg.float().to(torch.bfloat16).double()):
+            failures.append(f"{tap}: gb is not bf16(g) at {int((v['gb'] != gg.float().to(torch.bfloat16).double()).sum())} elements")
+        err = (v["gsum"] - gg.sum((2, 3))).abs() - 1e-5 * gg.abs().sum((2, 3))
+        if (err > 0).any():
+            failures.append(f"{tap}: gsum is not the pixel sums of g (first bad (image, channel) {tuple((err > 0).nonzero()[0].tolist())})")
+    return failures
 
 
 def param_class(kind, name):
@@ -263,19 +280,11 @@ def miss(q):
 @pytest.mark.parametrize("name", sorted(CASES))
 def test_every_layer_gradient_matches_its_fp64_reference(name):
     t0 = time.time()
-    r = run_backward(name)
+    r = run_backward(CASES[name], tgl.case_seed(CASES, name))
     cfg, sd, nl, keeps, taps = r["cfg"], r["sd"], r["nl"], r["keeps"], r["taps"]
     b = r["dx"].shape[0]
-    failures, rows, worst = [], [], {}
-    # exact identities of every tensor's gradient
-    for tap, v in r["gt"].items():
-        gg = v["g"]
-        assert torch.isfinite(gg).all(), tap
-        if not torch.equal(v["gb"], gg.float().to(torch.bfloat16).double()):
-            failures.append(f"{tap}: gb is not bf16(g) at {int((v['gb'] != gg.float().to(torch.bfloat16).double()).sum())} elements")
-        err = (v["gsum"] - gg.sum((2, 3))).abs() - 1e-5 * gg.abs().sum((2, 3))
-        if (err > 0).any():
-            failures.append(f"{tap}: gsum is not the pixel sums of g (first bad (image, channel) {tuple((err > 0).nonzero()[0].tolist())})")
+    rows, worst = [], {}
+    failures = identity_failures(r["gt"])     # exact identities of every tensor's gradient
     params = set(r["pgrads"])
     layers, refs, quantities = layer_checks(r)
     checked = set()
@@ -357,11 +366,11 @@ def test_block_params_are_final_after_their_flush(name):
     """sr3_train_block_params(i): the listed gradients are final once block i and a flush have run (what DataParallelTrainer all-reduces
     bucket by bucket), every parameter is listed at most once, and the unlisted ones are exactly those finish() writes."""
     net, image_size, b, h, w, drop = CASES[name]
-    cfg, sd, eng, keeps = make_engine(name)
+    cfg, sd, eng, keeps = make_engine(CASES[name])
     g = torch.Generator().manual_seed(3)
     hr = torch.rand(b, 3, h, w, generator=g).cuda() * 2 - 1
     sr = torch.rand(b, 3, h, w, generator=g).cuda() * 2 - 1 if cfg.in_channel != 3 else None
-    gamma = torch.tensor(tgl.NOISE_LEVELS[:b]).cuda()
+    gamma = tgl.noise_levels(b).cuda()
     noise = torch.randn(b, 3, h, w, generator=g).cuda()
     table = eng.param_table()
     names = [n for n, _ in table]

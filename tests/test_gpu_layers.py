@@ -104,6 +104,16 @@ CASES = {
 NOISE_LEVELS = (0.9, 0.2, 0.55)      # a different noise level per image: a FiLM row read from the wrong image shows
 
 
+def noise_levels(b):
+    """The noise levels of a batch of b, fp32: NOISE_LEVELS for b <= 3; past that b distinct levels in [0.05, 0.95] that alternate between
+    the two ends, 0.05 + k d and 0.95 - k d for images 2 k and 2 k + 1 (d = 0.45 / b): images i and i + 1 (which the wrong FiLM references
+    swap) are 0.9 - i d apart, more than 0.45."""
+    if b <= len(NOISE_LEVELS):
+        return torch.tensor(NOISE_LEVELS[:b])
+    d = 0.45 / b
+    return torch.tensor([0.05 + i // 2 * d if i % 2 == 0 else 0.95 - i // 2 * d for i in range(b)], dtype=torch.float32)
+
+
 def case_seed(cases, name):
     """The seed of a case's inputs: its place in sorted order, the sr64_512 cases after the others (so adding them kept every other
     case's inputs)."""
@@ -122,10 +132,10 @@ def engine_cfg(cfg, image_size, precision):
                 precision=precision)
 
 
-def run_engine(name):
-    """-> (cfg, state dict on the GPU, noise levels, {tap: fp64 NCHW} incl. "input" and "eps", {dropout block: scaled keep-mask})."""
+def make_engine(case):
+    """The engine of a case tuple (CASES' form) with the weights lref.state_dict(cfg, 5) and the schedule SCHED.  -> (cfg, sd, engine)."""
     from sr3_b200 import _native
-    net, image_size, b, h, w, precision, drop = CASES[name]
+    net, image_size, b, h, w, precision, drop = case
     cfg = oracle_cfg(net, image_size)
     sd = lref.state_dict(cfg, 5)
     eng = _native.Engine(engine_cfg(cfg, image_size, precision), b, torch.device("cuda", torch.cuda.current_device()), train_dropout=drop,
@@ -133,9 +143,17 @@ def run_engine(name):
     sch = orc.make_schedule(SCHED)
     eng.set_schedule(sch.buffers, sch.sqrt_alphas_cumprod_prev)
     eng.load_state_dict(sd)
-    g = torch.Generator().manual_seed(case_seed(CASES, name))
+    return cfg, sd, eng
+
+
+def run_engine(case, seed, tap_dtype=torch.float64):
+    """One forward of a case tuple, inputs drawn from `seed`.  -> (cfg, state dict on the GPU, noise levels, {tap: NCHW in tap_dtype}
+    incl. "input" and "eps", {dropout block: scaled keep-mask}, the engine's tile_schedules())."""
+    net, image_size, b, h, w, precision, drop = case
+    cfg, sd, eng = make_engine(case)
+    g = torch.Generator().manual_seed(seed)
     x = torch.randn(b, cfg.in_channel, h, w, generator=g)
-    nl = torch.tensor(NOISE_LEVELS[:b])
+    nl = noise_levels(b)
     masks = {}
     if drop is None:
         eps = eng.unet_forward(x.cuda(), nl.cuda())
@@ -151,13 +169,14 @@ def run_engine(name):
             eng.set_dropout_mask(k, keep.cuda().contiguous())
             masks[k] = _philox.scale_mask(keep, drop)
         eps, _ = eng.train_unet_forward(x.cuda(), nl.cuda())
-    taps = {"input": x.cuda().double(), "eps": eps.double()}
+    taps = {"input": x.cuda().to(tap_dtype), "eps": eps.to(tap_dtype)}
     for tap, _, _, _, _ in lref.layer_inputs(cfg):
         if tap != "eps":
-            taps[tap] = eng.read_activation(tap).double()
+            taps[tap] = eng.read_activation(tap).to(tap_dtype)
+    plan = eng.tile_schedules()
     torch.cuda.synchronize()
     del eng
-    return cfg, {k: v.cuda() for k, v in sd.items()}, nl.cuda(), taps, masks
+    return cfg, {k: v.cuda() for k, v in sd.items()}, nl.cuda(), taps, masks, plan
 
 
 def contraction(kind, cin, cout, tokens):
@@ -199,7 +218,7 @@ def elementwise(got, ref, resid, elem):
 def test_every_layer_matches_its_fp64_reference(name):
     t0 = time.time()
     net, image_size, b, h, w, precision, drop = CASES[name]
-    cfg, sd, nl, taps, masks = run_engine(name)
+    cfg, sd, nl, taps, masks, _ = run_engine(CASES[name], case_seed(CASES, name))
     unfused = drop is not None
     failures, rows, worst = [], [], {}
     first_res = None

@@ -127,3 +127,35 @@ def test_rounding_moves_every_layer(net):
         for k, v in m.items():
             lo, hi = PRECISE_MOVES if k == "fp32" else BF16_MOVES
             assert lo < v < hi, (name, tap, k, v)
+
+
+def test_groupnorm_of_the_next_image_moves_every_groupnorm_layer(net):
+    """gn_stats (image b normalised with the statistics of another image) moves every layer with a GroupNorm by more than 5 times its
+    bf16 rounding (measured 9x to 108x), and with the identity it is the default reference bit for bit."""
+    name, cfg, sd, nl, taps = net
+    b = nl.shape[0]
+    moves = {}
+    for tap, kind, spec, src, skip in lref.layer_inputs(cfg):
+        if kind not in ("res", "attn", "final"):
+            continue
+        x, sk = taps[src], None if skip is None else taps[skip]
+        resid = lref.residual(kind, spec, sd, x)
+        ref = lref.layer_reference(sd, cfg, kind, spec, x, sk, nl)
+        assert torch.equal(lref.layer_reference(sd, cfg, kind, spec, x, sk, nl, gn_stats=list(range(b))), ref), (name, tap)
+        rounding = branch_rel(ref, lref.layer_reference(sd, cfg, kind, spec, x, sk, nl, rounded=False), resid)
+        moves[tap] = branch_rel(lref.layer_reference(sd, cfg, kind, spec, x, sk, nl, gn_stats=lref.neighbour(b)), ref, resid) / rounding
+    print(name, "moves in units of the layer's bf16 rounding:", {t: f"{v:.0f}" for t, v in moves.items()})
+    assert all(v > 5 for v in moves.values()), (name, moves)
+
+
+def test_noise_levels():
+    """noise_levels(b): the levels of the batch-2 and -3 cases unchanged; b distinct levels in [0.05, 0.95] past that, neighbours more than
+    0.45 apart."""
+    import test_gpu_layers as tgl
+    for b in (1, 2, 3):
+        assert torch.equal(tgl.noise_levels(b), torch.tensor(tgl.NOISE_LEVELS[:b]))
+    for b in (4, 5, 8, 16, 32):
+        nl = tgl.noise_levels(b)
+        assert nl.dtype == torch.float32 and nl.shape == (b,) and len(set(nl.tolist())) == b
+        assert 0.05 - 1e-7 <= nl.min() and nl.max() <= 0.95 + 1e-7
+        assert (nl[1:] - nl[:-1]).abs().min() > 0.45, nl
