@@ -106,6 +106,12 @@ _SIGS = {
     "sr3_stream_step": (c_int, [c_void_p, c_void_p]),
     "sr3_stream_retire": (c_int, [c_void_p, c_int, c_void_p, c_void_p]),
     "sr3_stream_slot_state": (c_int, [c_void_p, POINTER(c_int), POINTER(c_int)]),
+    "sr3_wstream_create": (c_int, [c_void_p, c_uint64, c_int, c_int, POINTER(c_void_p)]),
+    "sr3_wstream_destroy": (None, [c_void_p]),
+    "sr3_wstream_admit": (c_int, [c_void_p, POINTER(c_int), c_int, c_void_p, c_void_p, c_int, c_int, c_uint64, POINTER(c_int), c_void_p]),
+    "sr3_wstream_step": (c_int, [c_void_p, c_void_p]),
+    "sr3_wstream_retire": (c_int, [c_void_p, c_int, c_void_p]),
+    "sr3_wstream_slot_state": (c_int, [c_void_p, POINTER(c_int), POINTER(c_int), POINTER(c_int)]),
     "sr3_engine_profile_step": (c_int, [c_void_p, c_int, c_int, c_int, POINTER(c_int), POINTER(c_float), POINTER(c_double), POINTER(c_double),
                                         POINTER(c_int), c_void_p]),
     "sr3_pil_bicubic_tables": (c_int, [c_int, c_int, POINTER(c_int), POINTER(c_int), c_int, POINTER(c_int)]),
@@ -757,22 +763,37 @@ def stream_plan(arrival_steps, slots, T):
     lazily, one value per request planned), yields (slot, admit_step, finish_step).  Requests are admitted first come first served, each
     at the first step at which it has arrived, every earlier request has been admitted and a slot is free, into the lowest free slot; it
     runs steps admit_step .. admit_step + T - 1 and its image is ready after step finish_step - 1 = admit_step + T - 1, so the slot is free
-    again from step finish_step on.  Pure host arithmetic: GaussianDiffusion.super_resolution_stream follows it step for step."""
+    again from step finish_step on.  Pure host arithmetic: GaussianDiffusion.super_resolution_stream follows it step for step.
+    windowed_stream_plan with one window per request."""
+    for slot_list, k, finish in windowed_stream_plan(((a, 1) for a in arrival_steps), slots, T):
+        yield slot_list[0], k, finish
+
+
+def windowed_stream_plan(requests, slots, T):
+    """The slot plan of continuous batching when a request takes several slots: for request n = (arrival_step, n_windows) (arrival steps
+    non-decreasing; any iterable, read lazily, one value per request planned), yields (slot_list, admit_step, finish_step).  First come
+    first served with head-of-line blocking: a request is admitted at the first step at which it has arrived, every earlier request has
+    been admitted and n_windows slots are free -- a later, smaller request never overtakes it -- into the n_windows lowest free slots; it
+    runs T steps and its slots are free again from finish_step = admit_step + T on.  Pure host arithmetic:
+    GaussianDiffusion.super_resolution_windowed_stream follows it step for step."""
     slots, T = int(slots), int(T)
     if slots < 1 or T < 1:
-        raise ValueError("stream_plan needs slots >= 1 and T >= 1, got slots=%d T=%d" % (slots, T))
-    free_at = [0] * slots
+        raise ValueError("stream plans need slots >= 1 and T >= 1, got slots=%d T=%d" % (slots, T))
+    free_at = [0] * slots                   # the step from which each slot is free
     last_arrival, last_admit = 0, 0
-    for a in arrival_steps:
-        a = int(a)
+    for a, n in requests:
+        a, n = int(a), int(n)
         if a < last_arrival:
             raise ValueError("arrival steps must be non-decreasing: %d after %d" % (a, last_arrival))
+        if not 1 <= n <= slots:
+            raise ValueError("a request of %d windows cannot run on %d slots" % (n, slots))
         last_arrival = a
-        k = max(a, last_admit, min(free_at))
-        slot = next(s for s in range(slots) if free_at[s] <= k)
-        free_at[slot] = k + T
+        k = max(a, last_admit, sorted(free_at)[n - 1])     # the first step at which n slots are free
+        taken = [s for s in range(slots) if free_at[s] <= k][:n]
+        for s in taken:
+            free_at[s] = k + T
         last_admit = k
-        yield slot, k, k + T
+        yield taken, k, k + T
 
 
 class StreamSampler:
@@ -834,6 +855,80 @@ class StreamSampler:
         with torch.cuda.device(self.device):
             _check(lib().sr3_stream_retire(self._h, int(slot), _ptr(out), _stream()))
         return out
+
+
+class WindowedStreamSampler:
+    """Continuous batching of canvases of any size on `engine` (sr3_wstream_*): every request is a canvas of ny x nx windows of the engine's
+    size (overlap_h x overlap_w, the windowed sampler's grid) that takes as many of the engine.batch slots and runs at its own timestep.
+    The online interface: a server calls admit() with free slots, step() once per reverse step and retire() for every request finished()
+    lists.  This object owns each request's canvas (x_t, and a copy of the condition) until retire(), which returns x_0; the native side
+    borrows them, so admission allocates nothing on the device.  Borrows the engine (and keeps it alive); nothing else may run on it while
+    requests are in flight."""
+
+    def __init__(self, engine, seed, overlap_h, overlap_w):
+        self.engine = engine
+        self.device = engine.device
+        self.slots = engine.batch
+        self.seed = int(seed)
+        self.overlap = (int(overlap_h), int(overlap_w))
+        self._canvases = {}                    # request id -> (x, condition)
+        self._h = c_void_p()
+        with torch.cuda.device(self.device):
+            _check(lib().sr3_wstream_create(engine._h, self.seed, *self.overlap, ctypes.byref(self._h)))
+
+    def __del__(self):
+        try:
+            if getattr(self, "_h", None):
+                lib().sr3_wstream_destroy(self._h)
+                self._h = None
+        except Exception:
+            pass
+
+    def windows(self, height, width):
+        """The number of windows (= slots) of a height x width canvas."""
+        return len(window_grid(height, self.engine.height, self.overlap[0])) * len(window_grid(width, self.engine.width, self.overlap[1]))
+
+    def admit(self, slots, condition_x, x_T, sample_index):
+        """Admit a request ([C_cond, H, W] condition and [C, H, W] x_T) into the free `slots`, one per window of its grid (row-major); its
+        Philox draws are keyed by the global `sample_index`.  Returns the request's id."""
+        if condition_x is None or condition_x.dim() != 3 or condition_x.shape[0] != self.engine.in_channel - self.engine.channels:
+            raise ValueError("condition_x must be [%d, H, W], got %s" % (self.engine.in_channel - self.engine.channels,
+                                                                          tuple(getattr(condition_x, "shape", ()))))
+        hw = tuple(condition_x.shape[1:])
+        if tuple(x_T.shape) != (self.engine.channels,) + hw:
+            raise ValueError("x_T has shape %s; the condition is %s" % (tuple(x_T.shape), (self.engine.channels,) + hw))
+        cond = torch.empty(condition_x.shape, device=self.device, dtype=torch.float32).copy_(condition_x)
+        x = torch.empty(x_T.shape, device=self.device, dtype=torch.float32).copy_(x_T)
+        sl = [int(s) for s in slots]
+        rid = c_int()
+        with torch.cuda.device(self.device):
+            _check(lib().sr3_wstream_admit(self._h, (c_int * max(len(sl), 1))(*sl), len(sl), _ptr(cond), _ptr(x), hw[0], hw[1],
+                                           int(sample_index), ctypes.byref(rid), _stream()))
+        self._canvases[rid.value] = (x, cond)
+        return rid.value
+
+    def step(self, n=1):
+        with torch.cuda.device(self.device):
+            for _ in range(int(n)):
+                _check(lib().sr3_wstream_step(self._h, _stream()))
+
+    def slot_state(self):
+        """(request, t, state) per slot: the request id (-1 free), its t (timestep of its next step, -1 once finished) and state 0 free,
+        1 running, 2 finished, waiting for retire()."""
+        r, t, st = (c_int * self.slots)(), (c_int * self.slots)(), (c_int * self.slots)()
+        _check(lib().sr3_wstream_slot_state(self._h, r, t, st))
+        return list(r), list(t), list(st)
+
+    def finished(self):
+        """The ids of the requests whose image is ready."""
+        r, _, st = self.slot_state()
+        return sorted({q for q, v in zip(r, st) if v == 2})
+
+    def retire(self, request):
+        """x_0 [C, H, W] of finished `request`; frees its slots."""
+        with torch.cuda.device(self.device):
+            _check(lib().sr3_wstream_retire(self._h, int(request), _stream()))
+        return self._canvases.pop(int(request))[0]
 
 
 def bench_conv(B, H, W, Cin, Cout, k=3, stride=1, resid=False, stats=True, reps=20):

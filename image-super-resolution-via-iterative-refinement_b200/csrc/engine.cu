@@ -24,6 +24,7 @@
 #include "train_kernels.cuh"
 #include "window_kernels.cuh"
 #include "stream_kernels.cuh"
+#include "window_stream_kernels.cuh"
 
 using namespace sr3;
 typedef __nv_bfloat16 bf16;
@@ -2118,6 +2119,130 @@ struct sr3_stream {
     }
 };
 
+// ------------------------------------------------------------------------------------------------ continuous batching of windowed canvases
+// The engine's B images are slots, one window each; a request is a canvas of any size whose ny x nx windows take as many slots and run at
+// the request's own timestep.  The caller owns each canvas (x_t, condition); the stream holds up to B request records, their window
+// geometry, the slot table and a means arena.  A step: wstream_gather_kernel -> the engine's step graph (UNet.forward form) ->
+// wstream_means_kernel -> wstream_merge_kernel.
+struct sr3_wstream {
+    sr3_engine* e = nullptr;               // borrowed
+    uint64_t seed = 0;
+    int overlap_h = 0, overlap_w = 0;
+    DevAllocs mem;
+    WStreamReq* reqs = nullptr;            // device [2][B]; the next step reads reqs + cur * B, its merge writes the other half
+    int cur = 0;
+    WStreamSlot* slot_dev = nullptr;       // device [B]
+    int *oy = nullptr, *ox = nullptr, *slot_of = nullptr;     // device [B records][B]
+    float *wy = nullptr, *wx = nullptr;    // device [B records][B][wh], [B records][B][ww]
+    float* means = nullptr;                // device [B][C][wh][ww]
+    std::vector<WStreamReq> host;          // exact mirror of the half the next step reads
+    std::vector<char> held;                // the record holds a request: running (host[r].active) or finished and not yet retired
+    std::vector<WStreamSlot> slots;        // mirror of slot_dev
+    int schedule_gen = 0;                  // e->schedule_gen when the requests in flight were admitted
+
+    bool any_running() const {
+        for (const WStreamReq& r : host) if (r.active) return true;
+        return false;
+    }
+    void init(sr3_engine* eng, uint64_t sd, int ovh, int ovw) {
+        e = eng; seed = sd; overlap_h = ovh; overlap_w = ovw;
+        REQUIRE(!e->train, "a windowed stream needs an inference engine (sr3_engine_create_sized)");
+        REQUIRE(e->cfg.conditional, "a windowed stream needs a conditional model");
+        REQUIRE(ovh >= 0 && ovh < e->H && ovw >= 0 && ovw < e->W, "overlap %dx%d must be at least 0 and below the window %dx%d", ovh, ovw, e->H, e->W);
+        CK(cudaSetDevice(e->dev));
+        const int B = e->B;
+        host.assign(B, WStreamReq{-1, 0, 0ull, nullptr, nullptr, 0, 0, 0, 0});
+        held.assign(B, 0);
+        slots.assign(B, WStreamSlot{-1, 0, 0});
+        reqs = static_cast<WStreamReq*>(mem.alloc(2 * B * sizeof(WStreamReq)));
+        slot_dev = static_cast<WStreamSlot*>(mem.alloc(B * sizeof(WStreamSlot)));
+        oy = static_cast<int*>(mem.alloc((size_t)B * B * sizeof(int)));
+        ox = static_cast<int*>(mem.alloc((size_t)B * B * sizeof(int)));
+        slot_of = static_cast<int*>(mem.alloc((size_t)B * B * sizeof(int)));
+        wy = static_cast<float*>(mem.alloc((size_t)B * B * e->H * sizeof(float)));
+        wx = static_cast<float*>(mem.alloc((size_t)B * B * e->W * sizeof(float)));
+        means = static_cast<float*>(mem.alloc(e->img_bytes()));
+        CK(cudaMemcpy(reqs, host.data(), B * sizeof(WStreamReq), cudaMemcpyHostToDevice));
+        CK(cudaMemcpy(reqs + B, host.data(), B * sizeof(WStreamReq), cudaMemcpyHostToDevice));
+        CK(cudaMemcpy(slot_dev, slots.data(), B * sizeof(WStreamSlot), cudaMemcpyHostToDevice));
+        CK(cudaMemset(e->x_state, 0, e->img_bytes()));
+        CK(cudaMemset(e->in_buf, 0, (size_t)B * e->H * e->W * e->in_C * e->PW * sizeof(bf16)));
+        CK(cudaMemset(e->nl_buf, 0, B * sizeof(float)));
+    }
+    void check_schedule() const {
+        REQUIRE(e->T > 0, "no noise schedule: call sr3_engine_set_schedule first");
+        REQUIRE(!any_running() || schedule_gen == e->schedule_gen,
+                "the noise schedule changed while requests are in flight; they cannot finish on a mixed schedule");
+    }
+    int admit(const int* sl, int n, const float* cond, float* x, int H, int W, uint64_t sample, cudaStream_t st) {
+        const int B = e->B, wh = e->H, ww = e->W;
+        check_schedule();
+        REQUIRE(x != nullptr && cond != nullptr, "null canvas");
+        REQUIRE(H >= wh && W >= ww, "canvas %dx%d is smaller than the window %dx%d (canvases are not padded)", H, W, wh, ww);
+        REQUIRE((long long)H * W < (1LL << 31), "canvas too large");
+        const std::vector<int> ry = window_origins(H, wh, overlap_h), rx = window_origins(W, ww, overlap_w);
+        const int ny = (int)ry.size(), nx = (int)rx.size();
+        REQUIRE(n == ny * nx, "a %dx%d canvas has %d windows (%d x %d), given %d slots", H, W, ny * nx, ny, nx, n);
+        REQUIRE(sl != nullptr, "null slot list");
+        for (int k = 0; k < n; ++k) {
+            REQUIRE(sl[k] >= 0 && sl[k] < B, "slot %d out of range [0, %d)", sl[k], B);
+            REQUIRE(slots[sl[k]].req < 0, "slot %d is busy (request %d)", sl[k], slots[sl[k]].req);
+            for (int j = 0; j < k; ++j) REQUIRE(sl[j] != sl[k], "slot %d listed twice", sl[k]);
+        }
+        int r = 0;
+        while (held[r]) ++r;                   // a free slot exists, so fewer than B requests are held
+        CK(cudaSetDevice(e->dev));
+        if (!any_running()) schedule_gen = e->schedule_gen;
+        const std::vector<float> gy = window_weights(ny, wh, overlap_h), gx = window_weights(nx, ww, overlap_w);
+        CK(cudaMemcpyAsync(oy + r * B, ry.data(), ny * sizeof(int), cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(ox + r * B, rx.data(), nx * sizeof(int), cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(wy + (size_t)r * B * wh, gy.data(), gy.size() * sizeof(float), cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(wx + (size_t)r * B * ww, gx.data(), gx.size() * sizeof(float), cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(slot_of + r * B, sl, n * sizeof(int), cudaMemcpyHostToDevice, st));
+        for (int k = 0; k < n; ++k) slots[sl[k]] = WStreamSlot{r, k / nx, k % nx};
+        CK(cudaMemcpyAsync(slot_dev, slots.data(), B * sizeof(WStreamSlot), cudaMemcpyHostToDevice, st));
+        host[r] = WStreamReq{e->T - 1, 1, (unsigned long long)sample, x, cond, H, W, ny, nx};
+        held[r] = 1;
+        CK(cudaMemcpyAsync(reqs + cur * B + r, &host[r], sizeof(WStreamReq), cudaMemcpyHostToDevice, st));
+        return r;
+    }
+    void step(cudaStream_t st) {
+        check_schedule();
+        CK(cudaSetDevice(e->dev));
+        StepCtl& c = e->ctl; memset(&c, 0, sizeof(c));
+        c.nl_from_table = 0; c.out_mode = 0;
+        e->push_ctl(st);
+        WStreamStep p{};
+        p.cur = reqs + cur * e->B; p.next = reqs + (cur ^ 1) * e->B; p.slots = slot_dev;
+        p.oy = oy; p.ox = ox; p.wy = wy; p.wx = wx; p.slot_of = slot_of;
+        p.B = e->B; p.C = e->cfg.channels; p.cond_c = e->cond_c; p.wh = e->H; p.ww = e->W;
+        p.in_buf = e->in_buf; p.in_ld = e->in_C * e->PW; p.lo_off = e->precise ? e->in_C : 0;
+        p.x_state = e->x_state; p.eps = e->eps_buf; p.means = means;
+        p.tab = e->post_tab; p.tab_T = e->T_cap; p.nl_table = e->nl_table; p.nl_buf = e->nl_buf; p.seed = seed;
+        const long long total = 1LL * e->B * e->H * e->W;
+        const dim3 grid((int)std::min<long long>((total + 255) / 256, num_sms() * 8LL));
+        launch_k(wstream_gather_kernel, grid, dim3(256), 0, st, p);
+        e->run_step(st);
+        launch_k(wstream_means_kernel, grid, dim3(256), 0, st, p);
+        launch_k(wstream_merge_kernel, grid, dim3(256), 0, st, p);
+        cur ^= 1;
+        for (WStreamReq& r : host)
+            if (r.active && --r.t < 0) r.active = 0;
+    }
+    void check_request(int r) const {
+        REQUIRE(r >= 0 && r < e->B && held[r], "request %d is not held by this stream", r);
+    }
+    void retire(int r, cudaStream_t st) {
+        check_request(r);
+        REQUIRE(!host[r].active, "request %d is still running (t = %d)", r, host[r].t);
+        CK(cudaSetDevice(e->dev));
+        for (WStreamSlot& s : slots)
+            if (s.req == r) s = WStreamSlot{-1, 0, 0};
+        CK(cudaMemcpyAsync(slot_dev, slots.data(), e->B * sizeof(WStreamSlot), cudaMemcpyHostToDevice, st));
+        held[r] = 0;
+    }
+};
+
 // ------------------------------------------------------------------------------------------------ C ABI
 #define API_BEGIN try {
 #define API_END                      \
@@ -2668,6 +2793,45 @@ int sr3_stream_slot_state(const sr3_stream* s, int* t, int* state) {
     for (int i = 0; i < (int)s->host.size(); ++i) {
         t[i] = s->host[i].t;
         state[i] = !s->held[i] ? 0 : s->host[i].active ? 1 : 2;
+    }
+    API_END
+}
+int sr3_wstream_create(sr3_engine* e, uint64_t seed, int overlap_h, int overlap_w, sr3_wstream** out) {
+    API_BEGIN
+    REQUIRE(e && out, "null argument");
+    std::unique_ptr<sr3_wstream> s(new sr3_wstream());
+    s->init(e, seed, overlap_h, overlap_w);
+    *out = s.release();
+    API_END
+}
+void sr3_wstream_destroy(sr3_wstream* s) { delete s; }
+int sr3_wstream_admit(sr3_wstream* s, const int* slots, int n_slots, const float* condition_x, float* x, int height, int width,
+                      uint64_t sample_index, int* request, void* stream) {
+    API_BEGIN
+    REQUIRE(s && request, "null argument");
+    *request = s->admit(slots, n_slots, condition_x, x, height, width, sample_index, static_cast<cudaStream_t>(stream));
+    API_END
+}
+int sr3_wstream_step(sr3_wstream* s, void* stream) {
+    API_BEGIN
+    REQUIRE(s, "null stream");
+    s->step(static_cast<cudaStream_t>(stream));
+    API_END
+}
+int sr3_wstream_retire(sr3_wstream* s, int request, void* stream) {
+    API_BEGIN
+    REQUIRE(s, "null stream");
+    s->retire(request, static_cast<cudaStream_t>(stream));
+    API_END
+}
+int sr3_wstream_slot_state(const sr3_wstream* s, int* request, int* t, int* state) {
+    API_BEGIN
+    REQUIRE(s && request && t && state, "null argument");
+    for (int i = 0; i < (int)s->slots.size(); ++i) {
+        const int r = s->slots[i].req;
+        request[i] = r;
+        t[i] = r < 0 ? -1 : s->host[r].t;
+        state[i] = r < 0 ? 0 : s->host[r].active ? 1 : 2;
     }
     API_END
 }

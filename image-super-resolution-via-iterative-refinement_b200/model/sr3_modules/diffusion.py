@@ -320,6 +320,101 @@ class GaussianDiffusion(nn.Module):
             for slot in sorted(s for s, (_, f) in running.items() if f == step):
                 yield running.pop(slot)[0], sampler.retire(slot)
 
+    # ---- continuous batching of canvases of any size, see DESIGN.md 3.11
+    def super_resolution_windowed_stream(self, requests, window=None, overlap=None, slots=16, seed=None, first_index=0):
+        """super_resolution_windowed for a stream of requests of ANY sizes, with continuous batching: a generator over `requests`, any
+        iterable (read lazily) of (key, x_in) or (key, x_in, x_T) with x_in [C, H, W], H and W at least the window's.  Every request is a
+        canvas of overlapping `window` crops (window and overlap as in super_resolution_windowed) that takes one of the engine's `slots`
+        per window and runs at its own timestep; windows of different requests share the batch.  A request is admitted first come first
+        served once its windows' slots are free (_native.windowed_stream_plan) and its (key, image [C, H, W]) is yielded as soon as its T
+        steps are done.  The n-th request's draws are keyed by sample index first_index + n (x_T ~ randn when not given): its image is
+        super_resolution_windowed(x_in[None], window, overlap, x_T=x_T[None], seed=seed, first_index=first_index + n) on the same engine
+        with its windows in the same slots, bit for bit (DESIGN.md 3.11: on some plans the slot a window runs in changes it within rounding).  A request is checked when it is read, before it is admitted (ValueError naming its key): its shape, a canvas smaller
+        than the window, more windows than `slots` (use super_resolution_windowed for it).  A schedule change while requests are in
+        flight makes the next step raise."""
+        if not self.conditional:
+            raise ValueError("super_resolution_windowed_stream needs a conditional model; use sample_stream")
+        slots = int(slots)
+        if slots < 1:
+            raise ValueError("slots must be >= 1, got %d" % slots)
+        wh, ww = (self.image_size, self.image_size) if window is None else (int(window[0]), int(window[1]))
+        geometry = self._window_geometry(wh, ww, (wh, ww), overlap)     # checks window and overlap now
+        return self._windowed_stream(requests, geometry, slots, seed, first_index)
+
+    def _windowed_stream_request(self, req, geometry, slots):
+        """(key, cond, x_T or None, (H, W), windows) of one request, checked against the stream's window and slot count."""
+        from ... import _native
+        if not isinstance(req, (tuple, list)) or len(req) not in (2, 3):
+            raise ValueError("a request is (key, x_in) or (key, x_in, x_T), got %r" % (type(req),))
+        key, x_in, x_T = (tuple(req) + (None,))[:3]
+        cond_c = self.denoise_fn.arch["in_channel"] - self.channels
+        if not torch.is_tensor(x_in) or x_in.dim() != 3 or x_in.shape[0] != cond_c:
+            raise ValueError("request %r: x_in must be [%d, H, W], got %s" % (key, cond_c, tuple(getattr(x_in, "shape", ()))))
+        hw = (int(x_in.shape[1]), int(x_in.shape[2]))
+        (wh, ww), (ovh, ovw) = geometry
+        if hw[0] < wh or hw[1] < ww:
+            raise ValueError("request %r: canvas %dx%d is smaller than the window %dx%d (canvases are not padded)" % (key, *hw, wh, ww))
+        n = len(_native.window_grid(hw[0], wh, ovh)) * len(_native.window_grid(hw[1], ww, ovw))
+        if n > slots:
+            raise ValueError("request %r: a %dx%d canvas has %d windows, more than the stream's %d slots; use super_resolution_windowed"
+                             % (key, *hw, n, slots))
+        if x_T is not None and tuple(x_T.shape) != (self.channels,) + hw:
+            raise ValueError("request %r: x_T must be %s, got %s" % (key, (self.channels,) + hw, tuple(x_T.shape)))
+        return key, x_in, x_T, hw, n
+
+    @torch.no_grad()
+    def _windowed_stream(self, requests, geometry, slots, seed, first_index):
+        from ... import _native
+        device = self.betas.device
+        if seed is None:
+            seed = int(torch.randint(0, 2 ** 62, (1,)).item())
+        reqs = iter(requests)
+        sampler, plan, pending = None, None, None
+        step, n, exhausted = 0, 0, False
+        running = {}                           # request id -> (n, key, slot list, finish step)
+        arrival = [None]                       # (arrival step, windows) of the request the plan reads next
+        while True:
+            # the requests admitted at this step, in order; a request that does not fit waits, and nothing is read past it
+            batch, free = [], slots - sum(len(r[2]) for r in running.values())
+            while not exhausted and (pending is not None or free > 0):
+                if pending is None:
+                    try:
+                        req = next(reqs)
+                    except StopIteration:
+                        exhausted = True
+                        break
+                    pending = (step,) + self._windowed_stream_request(req, geometry, slots)
+                if pending[5] > free:
+                    break
+                batch.append(pending)
+                free -= pending[5]
+                pending = None
+            if batch and sampler is None:
+                (wh, ww), (ovh, ovw) = geometry
+                eng = self._engine(slots, wh, ww)
+                if eng.T == 0:
+                    raise RuntimeError("set_new_noise_schedule has not been called")
+                sampler, T = _native.WindowedStreamSampler(eng, seed, ovh, ovw), eng.T
+                plan = _native.windowed_stream_plan(iter(lambda: arrival[0], None), slots, T)
+            if batch and sampler.engine.T != T:
+                raise RuntimeError("sr3_b200: the noise schedule changed during the stream (n_timestep %d -> %d)" % (T, sampler.engine.T))
+            for read_at, key, cond, x_T, size, windows in batch:
+                arrival[0] = (read_at, windows)
+                slot_list, admit, finish = next(plan)
+                busy = {s for r in running.values() for s in r[2]}
+                assert admit == step and not busy & set(slot_list), (slot_list, admit, step)
+                if x_T is None:
+                    x_T = torch.randn((self.channels,) + size, device=device)
+                rid = sampler.admit(slot_list, cond, x_T, first_index + n)
+                running[rid] = (n, key, slot_list, finish)
+                n += 1
+            if not running:
+                return
+            sampler.step()
+            step += 1
+            for rid in sorted((r for r, v in running.items() if v[3] == step), key=lambda r: running[r][0]):
+                yield running.pop(rid)[1], sampler.retire(rid)
+
     def q_sample(self, x_start, continuous_sqrt_alpha_cumprod, noise=None):
         noise = torch.randn_like(x_start) if noise is None else noise
         return continuous_sqrt_alpha_cumprod * x_start + (1 - continuous_sqrt_alpha_cumprod ** 2).sqrt() * noise

@@ -261,6 +261,42 @@ int sr3_stream_retire(sr3_stream* s, int slot, float* out, void* stream);
 /* HOST t[B], state[B]: state 0 free, 1 running (t = timestep of its next step), 2 finished and not yet retired (t = -1). */
 int sr3_stream_slot_state(const sr3_stream* s, int* t, int* state);
 
+/* ---- continuous batching of windowed canvases: serve a stream of conditional requests of ANY size (each at least the engine's H x W,
+ * the window) on one inference engine.  A request is a canvas whose ny x nx overlapping windows (the grid and fp32 blend weights of
+ * sr3_windowed_*, with the stream's overlap) take ny * nx of the engine's B slots, one window each; all windows of a request run at the
+ * request's own timestep, windows of different requests at different timesteps share the batch.  A request takes exactly T steps, one
+ * per sr3_wstream_step, and then waits for sr3_wstream_retire.  A step is: a gather of every slot's window crop of its canvas (idle slots
+ * get zeros), the engine's step graph in its UNet.forward form (noise level of slot s = sqrt_alphas_cumprod_prev[t + 1] of its request),
+ * the clipped posterior mean of every running slot at its request's t, and a merge that blends the means on each canvas and adds sigma_t z
+ * with z from Philox keyed by (seed, the request's sample_index, the pixel's index in its canvas, t), writing x_{t-1} into the canvas.
+ * Bit-exactness: a request's x_0 equals what sr3_windowed_* computes for that canvas alone as image 0 with first_sample_index =
+ * sample_index on an engine of the same shape with its windows in the same slots, bit for bit, whatever the other slots hold and whenever
+ * it was admitted (every UNet op is per image; the means and the merge are the windowed sampler's arithmetic operation for operation).
+ * Whether the slots matter depends on the plan: on a 4x4-lowest-level plan a window moved to another slot changes within rounding.
+ * No step synchronises the host, copies to it or allocates: the host mirrors the request table, since every request takes exactly T steps.
+ * The stream BORROWS the engine (which must outlive it; nothing else may run on it while requests are in flight, and all calls of one
+ * stream go to one CUDA stream) and every admitted canvas until its request is retired.  Creating a stream zeroes the engine's state
+ * and input.  Refused at creation: a training engine, an unconditional model, an overlap outside [0, window side). */
+typedef struct sr3_wstream sr3_wstream;
+int sr3_wstream_create(sr3_engine* e, uint64_t seed, int overlap_h, int overlap_w, sr3_wstream** out);
+void sr3_wstream_destroy(sr3_wstream* s);
+/* Admit one request into the n_slots free slots `slots` (HOST, window k of the grid, row-major, into slots[k]).  condition_x: DEVICE fp32
+ * [cond_c][height][width], x: DEVICE fp32 [3][height][width] holding x_T, overwritten with x_{t-1} by every step and holding x_0 once the
+ * request has finished; both are BORROWED until sr3_wstream_retire, nothing is copied but the window geometry.  *request = the request's
+ * id, its first step runs at t = T - 1.  Refused, with no slot or request changed: a slot out of range, busy or listed twice, n_slots other
+ * than the canvas's window count, a canvas smaller than the window, null canvases, an engine with no schedule, a schedule changed since
+ * the requests in flight were admitted. */
+int sr3_wstream_admit(sr3_wstream* s, const int* slots, int n_slots, const float* condition_x, float* x, int height, int width,
+                      uint64_t sample_index, int* request, void* stream);
+/* One reverse step of every running request.  Refused when the engine has no schedule or sr3_engine_set_schedule was called while
+ * requests are in flight (they would finish on a mixed schedule). */
+int sr3_wstream_step(sr3_wstream* s, void* stream);
+/* Free the slots of a finished request and end the borrow of its canvases (x holds x_0).  Refuses a running request or an id not held. */
+int sr3_wstream_retire(sr3_wstream* s, int request, void* stream);
+/* HOST request[B], t[B], state[B] per slot: the request it runs (-1: free), the request's t (timestep of its next step; -1 once finished)
+ * and state 0 free, 1 running, 2 finished and not yet retired. */
+int sr3_wstream_slot_state(const sr3_wstream* s, int* request, int* t, int* state);
+
 /* core/metrics.py:8-34 `tensor2img` on the device: src fp32 DEVICE [n][C][H][W] -> clamp to [min_v, max_v] -> [0, 1] -> * 255, round half
  * to even -> uint8 DEVICE, HWC.  n == 1: dst [H][W][C].  n > 1: the images are tiled like torchvision.utils.make_grid(nrow, padding 2,
  * pad_value 0), which is what the reference does for 4-D input: dst [rows*(H+2)+2][cols*(W+2)+2][C], cols = min(nrow, n).
