@@ -13,7 +13,8 @@
 // * B rows are output channels (or keys / head-dim for attention) of a K-major bf16 matrix, 2-D TMA box {64, BLOCK_N}.
 // * The stage table is built on the host (engine.cu): 3x3 taps, the 1x1 residual conv accumulated into the same
 //   tile and channel concats are all just more stages.
-// * Persistent CTAs (one per SM) walk a contiguous range of tiles.  Warp 8 = TMA producer; warps 0..7 = two consumer warpgroups that
+// * Persistent CTAs (one per SM) walk a contiguous range of tiles.  Warp 8 = TMA producer (its warpgroup runs on 40 registers per thread
+//   so that the consumers get 232, see GEMM_THREADS); warps 0..7 = two consumer warpgroups that
 //   issue the wgmma of their share of the tile (MH = 2: one 128-row half each; MH = 1: one half of the columns each; tiles of at most
 //   32 columns: warpgroup 0 alone) and then run the epilogue on it: accumulator -> per-warp 32 x 32 transposition in shared memory ->
 //   bias / FiLM -> residual (TMA prefetched into smem) -> fp32 tile staged in swizzled smem and written by TMA store (and/or bf16
@@ -140,9 +141,17 @@ struct GemmParams {
     long long lo_out_off, lo_t_off;
 };
 
-constexpr int GEMM_THREADS = 288;           // warps 0..7: two consumer warpgroups (MMA + epilogue), warp 8: TMA producer
+// warps 0..7: two consumer warpgroups (MMA + epilogue); warps 8..11: the producer warpgroup, of which warp 8 issues the TMA loads.
+// A block of 384 threads starts at 168 registers per thread (a sub-partition's 16384 registers over its three warps).  After the set-up
+// the producer warpgroup gives all but 40 back and the consumers take them (setmaxnreg): 2 x 128 x 232 + 128 x 40 = 64512 <= 65536, so
+// the accumulator and the epilogue of the widest tiles stay in registers.
+constexpr int GEMM_THREADS = 384;
 constexpr int GEMM_EPI_WARPS = 8;
 constexpr int GEMM_PRODUCER_WARP = 8;
+constexpr int GEMM_CONSUMER_REGS = 232;
+constexpr int GEMM_PRODUCER_REGS = 40;
+static_assert(GEMM_EPI_WARPS * 32 * GEMM_CONSUMER_REGS + (GEMM_THREADS - GEMM_EPI_WARPS * 32) * GEMM_PRODUCER_REGS <= 65536, "register file");
+static_assert(GEMM_THREADS == 384 && GEMM_PRODUCER_WARP == GEMM_EPI_WARPS, "setmaxnreg acts on whole warpgroups: 2 consumer + 1 producer");
 constexpr int GEMM_MAX_STAGES = 8;
 // per epilogue warp: 4 KB staging (accumulator transposition, then the fp32 chunk for the TMA store) [+ 2 x 4 KB residual staging when the layer has one]
 __host__ __device__ constexpr int gemm_epi_warp_bytes(bool resid) { return resid ? 12288 : 4096; }
@@ -418,37 +427,43 @@ __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmPa
     const int tile_begin = static_cast<int>((static_cast<long long>(total_tiles) * cta) / ncta);
     const int tile_end = static_cast<int>((static_cast<long long>(total_tiles) * (cta + 1)) / ncta);
 
-    if (warp == GEMM_PRODUCER_WARP) {
-        // ---------------------------------------------------- TMA producer warp (converged; one elected lane issues)
-        int s = 0;
-        uint32_t ph = 0;
-        for (int tile = tile_begin; tile < tile_end; ++tile) {
-            int w0, h0, b0, n0, z;
-            decode(tile, w0, h0, b0, n0, z);
-            const int brow = n0 + z * p.b_zrows;
-            const int zdw = p.z_phase ? (z & 1) : 0, zdh = p.z_phase ? (z >> 1) : 0;
-            const int sp = tile % ksplit;
-            const int k0 = (num_kt * sp) / ksplit, k1 = (num_kt * (sp + 1)) / ksplit;
-            for (int k = k0; k < k1; ++k) {
-                mbar_wait(empty_bar(s), ph ^ 1u);
-                if (elect_one_sync()) {
-                    const int pass = k / p.num_k;
-                    const StageDesc& e = ktab_s[k - pass * p.num_k];
-                    const int a_lo = (pass == 2) ? p.lo_a_chan[e.a_sel] : 0, b_lo = (pass == 1) ? p.lo_b_col : 0;
-                    const uint32_t a_dst = stage_base + s * stage_bytes;
-                    const int na = e.a_multi ? e.ntaps : 1;
-                    mbar_arrive_expect_tx(full_bar(s), na * p.a_box_bytes + e.ntaps * B_BYTES);
-                    for (int t = 0; t < na; ++t)
-                        tma_load_5d(a_dst + (e.a_multi ? e.tap[t].a_off : 0), &pm->a_map[e.a_sel], full_bar(s), e.tap[t].a_chan + a_lo, w0 + e.tap[t].dw + zdw, e.tap[t].p,
-                                    h0 + e.tap[t].dh + (e.a_multi ? zdh : 0), b0);     // tall halo boxes always start one row above the tile
-                    for (int t = 0; t < e.ntaps; ++t)
-                        tma_load_2d(a_dst + p.a_stage_bytes + t * B_BYTES, &pm->b_map, full_bar(s), e.tap[t].b_col + b_lo, brow);
+    // The warp roles split here.  No block-wide barrier may follow: warps 9..11 have nothing more to do, and named barriers 1..3 count the
+    // 256 consumer threads only.
+    if (warp >= GEMM_EPI_WARPS) {
+        setmaxnreg_dec<GEMM_PRODUCER_REGS>();
+        if (warp == GEMM_PRODUCER_WARP) {
+            // ---------------------------------------------------- TMA producer warp (converged; one elected lane issues)
+            int s = 0;
+            uint32_t ph = 0;
+            for (int tile = tile_begin; tile < tile_end; ++tile) {
+                int w0, h0, b0, n0, z;
+                decode(tile, w0, h0, b0, n0, z);
+                const int brow = n0 + z * p.b_zrows;
+                const int zdw = p.z_phase ? (z & 1) : 0, zdh = p.z_phase ? (z >> 1) : 0;
+                const int sp = tile % ksplit;
+                const int k0 = (num_kt * sp) / ksplit, k1 = (num_kt * (sp + 1)) / ksplit;
+                for (int k = k0; k < k1; ++k) {
+                    mbar_wait(empty_bar(s), ph ^ 1u);
+                    if (elect_one_sync()) {
+                        const int pass = k / p.num_k;
+                        const StageDesc& e = ktab_s[k - pass * p.num_k];
+                        const int a_lo = (pass == 2) ? p.lo_a_chan[e.a_sel] : 0, b_lo = (pass == 1) ? p.lo_b_col : 0;
+                        const uint32_t a_dst = stage_base + s * stage_bytes;
+                        const int na = e.a_multi ? e.ntaps : 1;
+                        mbar_arrive_expect_tx(full_bar(s), na * p.a_box_bytes + e.ntaps * B_BYTES);
+                        for (int t = 0; t < na; ++t)
+                            tma_load_5d(a_dst + (e.a_multi ? e.tap[t].a_off : 0), &pm->a_map[e.a_sel], full_bar(s), e.tap[t].a_chan + a_lo, w0 + e.tap[t].dw + zdw, e.tap[t].p,
+                                        h0 + e.tap[t].dh + (e.a_multi ? zdh : 0), b0);     // tall halo boxes always start one row above the tile
+                        for (int t = 0; t < e.ntaps; ++t)
+                            tma_load_2d(a_dst + p.a_stage_bytes + t * B_BYTES, &pm->b_map, full_bar(s), e.tap[t].b_col + b_lo, brow);
+                    }
+                    __syncwarp();
+                    if (++s == stages) { s = 0; ph ^= 1u; }
                 }
-                __syncwarp();
-                if (++s == stages) { s = 0; ph ^= 1u; }
             }
         }
-    } else if (warp < GEMM_EPI_WARPS) {
+    } else {
+        setmaxnreg_inc<GEMM_CONSUMER_REGS>();
         // ---------------------------------------------------- consumers: warpgroup g issues the wgmma of its share of the tile, then
         // every warp runs the epilogue of its 32-row quadrant q of that share, one 32-column chunk (item) at a time
         const int g = warp >> 2;
@@ -608,17 +623,7 @@ __device__ __forceinline__ void gemm_tile_body(const GemmParams& p, const GemmPa
                     unsigned int* ctr = p.counters + tile / ksplit;
                     const unsigned int old = atomicAdd(ctr, 1u);
                     const unsigned int target = (old / ksplit + 1u) * ksplit;              // the counter only ever grows
-                    uint64_t t0 = 0;
-                    for (uint32_t spins = 0;; ++spins) {
-                        unsigned int v;
-                        asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(ctr) : "memory");
-                        if (static_cast<int>(v - target) >= 0) break;
-                        if ((spins & 1023u) == 1023u) {
-                            const uint64_t now = globaltimer_ns();
-                            if (t0 == 0) t0 = now;
-                            if (now - t0 > 4000000000ull) __trap();   // no printf: a call in the kernel serialises its wgmma (see mbar_wait)
-                        }
-                    }
+                    spin_wait_reached(ctr, target);
                     __threadfence();
                 }
                 __syncwarp();

@@ -29,11 +29,12 @@ __device__ __forceinline__ bool elect_one_sync() {
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
-__device__ __forceinline__ uint64_t globaltimer_ns() {
-    uint64_t t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    return t;
-}
+// Warpgroup register reallocation: every thread of the warpgroup executes the same one.  dec hands registers back to the CTA's pool,
+// inc blocks until the pool holds enough; both counts are per thread, multiples of 8 in [24, 256].
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 
 // fp64 reduction on a GLOBAL address (no return value), spelled in PTX so that it is one red.global.add.f64 whatever the compiler
 // can prove about the pointer.
@@ -90,6 +91,28 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
         "trap;\n\t"
         "DONE:\n\t}" ::"r"(bar),
         "r"(parity)
+        : "memory");
+}
+
+// Bounded spin until the counter at `ctr` (global, acquire at gpu scope) has reached `target` (wrap-around compare), trapping after 4 s.
+// Loop, timeout and trap are one asm block, as in mbar_wait: written as a C++ loop around __trap(), it made ptxas keep the consumer
+// warpgroups of the split-K tile kernels at the 168 registers they start with, setmaxnreg notwithstanding, and spill.
+__device__ __forceinline__ void spin_wait_reached(const unsigned int* ctr, uint32_t target) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t.reg .u32 v;\n\t.reg .u64 t0, t1;\n\t"
+        "mov.u64 t0, %%globaltimer;\n\t"
+        "SPIN:\n\t"
+        "ld.acquire.gpu.global.u32 v, [%0];\n\t"
+        "sub.u32 v, v, %1;\n\t"
+        "setp.ge.s32 p, v, 0;\n\t"
+        "@p bra SPUN;\n\t"
+        "mov.u64 t1, %%globaltimer;\n\t"
+        "sub.u64 t1, t1, t0;\n\t"
+        "setp.lt.u64 p, t1, 4000000000;\n\t"
+        "@p bra SPIN;\n\t"
+        "trap;\n\t"
+        "SPUN:\n\t}" ::"l"(__cvta_generic_to_global(ctr)),
+        "r"(target)
         : "memory");
 }
 
