@@ -100,12 +100,6 @@ _SIGS = {
     "sr3_windowed_phase_begin": (c_int, [c_void_p, c_int, c_void_p]),
     "sr3_windowed_phase_means": (c_int, [c_void_p, c_void_p]),
     "sr3_windowed_phase_merge": (c_int, [c_void_p, c_void_p]),
-    "sr3_stream_create": (c_int, [c_void_p, c_uint64, POINTER(c_void_p)]),
-    "sr3_stream_destroy": (None, [c_void_p]),
-    "sr3_stream_admit": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_uint64, c_void_p]),
-    "sr3_stream_step": (c_int, [c_void_p, c_void_p]),
-    "sr3_stream_retire": (c_int, [c_void_p, c_int, c_void_p, c_void_p]),
-    "sr3_stream_slot_state": (c_int, [c_void_p, POINTER(c_int), POINTER(c_int)]),
     "sr3_wstream_create": (c_int, [c_void_p, c_uint64, c_int, c_int, POINTER(c_void_p)]),
     "sr3_wstream_destroy": (None, [c_void_p]),
     "sr3_wstream_admit": (c_int, [c_void_p, POINTER(c_int), c_int, c_void_p, c_void_p, c_int, c_int, c_uint64, POINTER(c_int), c_void_p]),
@@ -796,67 +790,6 @@ def windowed_stream_plan(requests, slots, T):
         yield taken, k, k + T
 
 
-class StreamSampler:
-    """Continuous batching on `engine` (sr3_stream_*): its engine.batch images are slots, each running its own request at its own
-    timestep.  The online interface: a server calls admit() for a request when a slot is free, step() once per reverse step, and
-    retire() for every slot finished() lists.  Borrows the engine (and keeps it alive); nothing else may run on it while requests are in
-    flight."""
-
-    def __init__(self, engine, seed):
-        self.engine = engine
-        self.device = engine.device
-        self.slots = engine.batch
-        self.seed = int(seed)
-        self._h = c_void_p()
-        with torch.cuda.device(self.device):
-            _check(lib().sr3_stream_create(engine._h, self.seed, ctypes.byref(self._h)))
-
-    def __del__(self):
-        try:
-            if getattr(self, "_h", None):
-                lib().sr3_stream_destroy(self._h)
-                self._h = None
-        except Exception:
-            pass
-
-    def _image(self, t, channels, what):
-        t = _f32c(t, self.device)
-        want = (channels, self.engine.height, self.engine.width)
-        if tuple(t.shape) != want:
-            raise ValueError("%s has shape %s; this stream's slots are %s" % (what, tuple(t.shape), want))
-        return t
-
-    def admit(self, slot, condition_x, x_T, sample_index):
-        """Load a request ([C, H, W] condition, None for an unconditional model, and x_T) into free `slot`; its Philox draws are keyed by
-        the global `sample_index`."""
-        c = None if condition_x is None else self._image(condition_x, self.engine.in_channel - self.engine.channels, "condition_x")
-        x = self._image(x_T, self.engine.channels, "x_T")
-        with torch.cuda.device(self.device):
-            _check(lib().sr3_stream_admit(self._h, int(slot), _ptr(c), _ptr(x), int(sample_index), _stream()))
-
-    def step(self, n=1):
-        with torch.cuda.device(self.device):
-            for _ in range(int(n)):
-                _check(lib().sr3_stream_step(self._h, _stream()))
-
-    def slot_state(self):
-        """(t, state) per slot: state 0 free, 1 running (t = timestep of its next step), 2 finished, waiting for retire()."""
-        t, st = (c_int * self.slots)(), (c_int * self.slots)()
-        _check(lib().sr3_stream_slot_state(self._h, t, st))
-        return list(t), list(st)
-
-    def finished(self):
-        """The slots whose image is ready."""
-        return [s for s, v in enumerate(self.slot_state()[1]) if v == 2]
-
-    def retire(self, slot):
-        """x_0 [C, H, W] of finished `slot`; frees the slot."""
-        out = torch.empty(self.engine.channels, self.engine.height, self.engine.width, device=self.device, dtype=torch.float32)
-        with torch.cuda.device(self.device):
-            _check(lib().sr3_stream_retire(self._h, int(slot), _ptr(out), _stream()))
-        return out
-
-
 class WindowedStreamSampler:
     """Continuous batching of canvases of any size on `engine` (sr3_wstream_*): every request is a canvas of ny x nx windows of the engine's
     size (overlap_h x overlap_w, the windowed sampler's grid) that takes as many of the engine.batch slots and runs at its own timestep.
@@ -889,15 +822,15 @@ class WindowedStreamSampler:
         return len(window_grid(height, self.engine.height, self.overlap[0])) * len(window_grid(width, self.engine.width, self.overlap[1]))
 
     def admit(self, slots, condition_x, x_T, sample_index):
-        """Admit a request ([C_cond, H, W] condition and [C, H, W] x_T) into the free `slots`, one per window of its grid (row-major); its
-        Philox draws are keyed by the global `sample_index`.  Returns the request's id."""
-        if condition_x is None or condition_x.dim() != 3 or condition_x.shape[0] != self.engine.in_channel - self.engine.channels:
-            raise ValueError("condition_x must be [%d, H, W], got %s" % (self.engine.in_channel - self.engine.channels,
-                                                                          tuple(getattr(condition_x, "shape", ()))))
-        hw = tuple(condition_x.shape[1:])
+        """Admit a request ([C_cond, H, W] condition, None for an unconditional model, and [C, H, W] x_T) into the free `slots`, one per
+        window of its grid (row-major); its Philox draws are keyed by the global `sample_index`.  Returns the request's id."""
+        cond_c = self.engine.in_channel - self.engine.channels
+        if condition_x is not None and (condition_x.dim() != 3 or condition_x.shape[0] != cond_c):
+            raise ValueError("condition_x must be [%d, H, W], got %s" % (cond_c, tuple(condition_x.shape)))
+        hw = tuple((x_T if condition_x is None else condition_x).shape[-2:])     # without a condition the size is x_T's
         if tuple(x_T.shape) != (self.engine.channels,) + hw:
-            raise ValueError("x_T has shape %s; the condition is %s" % (tuple(x_T.shape), (self.engine.channels,) + hw))
-        cond = torch.empty(condition_x.shape, device=self.device, dtype=torch.float32).copy_(condition_x)
+            raise ValueError("x_T has shape %s; this request needs %s" % (tuple(x_T.shape), (self.engine.channels,) + hw))
+        cond = None if condition_x is None else torch.empty(condition_x.shape, device=self.device, dtype=torch.float32).copy_(condition_x)
         x = torch.empty(x_T.shape, device=self.device, dtype=torch.float32).copy_(x_T)
         sl = [int(s) for s in slots]
         rid = c_int()

@@ -23,7 +23,6 @@
 #include "attn_long_wgmma.cuh"
 #include "train_kernels.cuh"
 #include "window_kernels.cuh"
-#include "stream_kernels.cuh"
 #include "window_stream_kernels.cuh"
 
 using namespace sr3;
@@ -2030,95 +2029,6 @@ struct sr3_windowed {
     }
 };
 
-// ------------------------------------------------------------------------------------------------ continuous batching
-// The engine's B images are the stream's slots and its buffers their state: x_state, the UNet input, nl_buf.  A step runs the engine's
-// own step graph with the UNet.forward control block (eps of every image into eps_buf, noise level nl_buf[b]) and then
-// slot_update_kernel, which applies each active slot's posterior update at the slot's own timestep and advances the slot table.
-struct sr3_stream {
-    sr3_engine* e = nullptr;               // borrowed
-    uint64_t seed = 0;
-    DevAllocs mem;
-    StreamSlot* table = nullptr;           // device [2][B]; the next step reads table + cur * B and writes the other half
-    int cur = 0;
-    std::vector<StreamSlot> host;          // exact mirror of the half the next step reads
-    std::vector<char> held;                // the slot holds a request: running (host[s].active) or finished and not yet retired
-    int schedule_gen = 0;                  // e->schedule_gen when the requests in flight were admitted
-
-    bool any_running() const {
-        for (const StreamSlot& s : host) if (s.active) return true;
-        return false;
-    }
-    void init(sr3_engine* eng, uint64_t sd) {
-        e = eng; seed = sd;
-        REQUIRE(!e->train, "a stream needs an inference engine (sr3_engine_create_sized)");
-        CK(cudaSetDevice(e->dev));
-        const int B = e->B;
-        host.assign(B, StreamSlot{-1, 0, 0ull});
-        held.assign(B, 0);
-        table = static_cast<StreamSlot*>(mem.alloc(2 * B * sizeof(StreamSlot)));
-        CK(cudaMemcpy(table, host.data(), B * sizeof(StreamSlot), cudaMemcpyHostToDevice));
-        CK(cudaMemcpy(table + B, host.data(), B * sizeof(StreamSlot), cudaMemcpyHostToDevice));
-        // idle slots run through the UNet too: start them from zeros rather than whatever the engine last computed
-        CK(cudaMemset(e->x_state, 0, e->img_bytes()));
-        CK(cudaMemset(e->in_buf, 0, (size_t)B * e->H * e->W * e->in_C * e->PW * sizeof(bf16)));
-        CK(cudaMemset(e->nl_buf, 0, B * sizeof(float)));
-    }
-    void check_slot(int slot) const { REQUIRE(slot >= 0 && slot < e->B, "slot %d out of range [0, %d)", slot, e->B); }
-    void check_schedule() const {
-        REQUIRE(e->T > 0, "no noise schedule: call sr3_engine_set_schedule first");
-        REQUIRE(!any_running() || schedule_gen == e->schedule_gen,
-                "the noise schedule changed while requests are in flight; they cannot finish on a mixed schedule");
-    }
-    void admit(int slot, const float* cond, const float* x_T, uint64_t sample, cudaStream_t st) {
-        check_slot(slot);
-        check_schedule();
-        REQUIRE(!held[slot], "slot %d is busy (%s)", slot, host[slot].active ? "running" : "finished, not yet retired");
-        REQUIRE(x_T != nullptr, "null x_T");
-        if (e->cfg.conditional) REQUIRE(cond != nullptr, "condition_x is required by a conditional model");
-        else REQUIRE(cond == nullptr, "condition_x given to an unconditional model");
-        CK(cudaSetDevice(e->dev));
-        if (!any_running()) schedule_gen = e->schedule_gen;
-        if (cond) e->load_nchw(cond, e->cond_c, 0, nullptr, st, slot);
-        e->load_nchw(x_T, e->cfg.channels, e->cond_c, e->x_state, st, slot);
-        CK(cudaMemcpyAsync(e->nl_buf + slot, e->nl_table + e->T, sizeof(float), cudaMemcpyDeviceToDevice, st));   // nl_table[t + 1], t = T - 1
-        host[slot] = StreamSlot{e->T - 1, 1, (unsigned long long)sample};
-        held[slot] = 1;
-        CK(cudaMemcpyAsync(table + cur * e->B + slot, &host[slot], sizeof(StreamSlot), cudaMemcpyHostToDevice, st));
-    }
-    void step(cudaStream_t st) {
-        check_schedule();
-        CK(cudaSetDevice(e->dev));
-        StepCtl& c = e->ctl; memset(&c, 0, sizeof(c));
-        c.nl_from_table = 0; c.out_mode = 0;
-        e->push_ctl(st);
-        e->run_step(st);
-        SlotUpdate p{};
-        p.eps = e->eps_buf; p.x_state = e->x_state;
-        p.in_buf = e->in_buf; p.in_ld = e->in_C * e->PW; p.in_coff = e->cond_c; p.lo_off = e->precise ? e->in_C : 0;
-        p.tab = e->post_tab; p.tab_T = e->T_cap; p.nl_table = e->nl_table; p.nl_buf = e->nl_buf;
-        p.cur = table + cur * e->B; p.next = table + (cur ^ 1) * e->B;
-        p.seed = seed; p.B = e->B; p.C = e->cfg.channels; p.H = e->H; p.W = e->W;
-        const long long total = 1LL * e->B * e->H * e->W;
-        launch_k(slot_update_kernel, dim3((int)std::min<long long>((total + 255) / 256, num_sms() * 8LL)), dim3(256), 0, st, p);
-        cur ^= 1;
-        for (StreamSlot& s : host)
-            if (s.active && --s.t < 0) s.active = 0;
-    }
-    void retire(int slot, float* out, cudaStream_t st) {
-        check_slot(slot);
-        REQUIRE(out != nullptr, "null output");
-        REQUIRE(held[slot], "slot %d holds no request", slot);
-        REQUIRE(!host[slot].active, "slot %d is still running (t = %d)", slot, host[slot].t);
-        CK(cudaSetDevice(e->dev));
-        const size_t chw = (size_t)e->cfg.channels * e->H * e->W;
-        const size_t in_img = (size_t)e->H * e->W * e->in_C * e->PW;
-        CK(cudaMemcpyAsync(out, e->x_state + slot * chw, chw * sizeof(float), cudaMemcpyDeviceToDevice, st));
-        CK(cudaMemsetAsync(e->x_state + slot * chw, 0, chw * sizeof(float), st));
-        CK(cudaMemsetAsync(e->in_buf + slot * in_img, 0, in_img * sizeof(bf16), st));
-        held[slot] = 0;
-    }
-};
-
 // ------------------------------------------------------------------------------------------------ continuous batching of windowed canvases
 // The engine's B images are slots, one window each; a request is a canvas of any size whose ny x nx windows take as many slots and run at
 // the request's own timestep.  The caller owns each canvas (x_t, condition); the stream holds up to B request records, their window
@@ -2147,7 +2057,6 @@ struct sr3_wstream {
     void init(sr3_engine* eng, uint64_t sd, int ovh, int ovw) {
         e = eng; seed = sd; overlap_h = ovh; overlap_w = ovw;
         REQUIRE(!e->train, "a windowed stream needs an inference engine (sr3_engine_create_sized)");
-        REQUIRE(e->cfg.conditional, "a windowed stream needs a conditional model");
         REQUIRE(ovh >= 0 && ovh < e->H && ovw >= 0 && ovw < e->W, "overlap %dx%d must be at least 0 and below the window %dx%d", ovh, ovw, e->H, e->W);
         CK(cudaSetDevice(e->dev));
         const int B = e->B;
@@ -2177,7 +2086,9 @@ struct sr3_wstream {
     int admit(const int* sl, int n, const float* cond, float* x, int H, int W, uint64_t sample, cudaStream_t st) {
         const int B = e->B, wh = e->H, ww = e->W;
         check_schedule();
-        REQUIRE(x != nullptr && cond != nullptr, "null canvas");
+        REQUIRE(x != nullptr, "null canvas");
+        if (e->cfg.conditional) REQUIRE(cond != nullptr, "condition_x is required by a conditional model");
+        else REQUIRE(cond == nullptr, "condition_x given to an unconditional model");
         REQUIRE(H >= wh && W >= ww, "canvas %dx%d is smaller than the window %dx%d (canvases are not padded)", H, W, wh, ww);
         REQUIRE((long long)H * W < (1LL << 31), "canvas too large");
         const std::vector<int> ry = window_origins(H, wh, overlap_h), rx = window_origins(W, ww, overlap_w);
@@ -2256,7 +2167,7 @@ struct sr3_wstream {
 extern "C" {
 
 const char* sr3_last_error(void) { return g_err.c_str(); }
-int sr3_abi_version(void) { return 4; }
+int sr3_abi_version(void) { return 5; }
 
 int sr3_engine_create_sized(const sr3_unet_config* cfg, int batch, int height, int width, int device, sr3_engine** out) {
     API_BEGIN
@@ -2758,42 +2669,6 @@ int sr3_windowed_read_state(sr3_windowed* w, float* x_out, void* stream) {
     API_BEGIN
     REQUIRE(w && x_out, "null argument");
     CK(cudaMemcpyAsync(x_out, w->x, w->canvas_elems() * sizeof(float), cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(stream)));
-    API_END
-}
-int sr3_stream_create(sr3_engine* e, uint64_t seed, sr3_stream** out) {
-    API_BEGIN
-    REQUIRE(e && out, "null argument");
-    std::unique_ptr<sr3_stream> s(new sr3_stream());
-    s->init(e, seed);
-    *out = s.release();
-    API_END
-}
-void sr3_stream_destroy(sr3_stream* s) { delete s; }
-int sr3_stream_admit(sr3_stream* s, int slot, const float* condition_x, const float* x_T, uint64_t sample_index, void* stream) {
-    API_BEGIN
-    REQUIRE(s, "null stream");
-    s->admit(slot, condition_x, x_T, sample_index, static_cast<cudaStream_t>(stream));
-    API_END
-}
-int sr3_stream_step(sr3_stream* s, void* stream) {
-    API_BEGIN
-    REQUIRE(s, "null stream");
-    s->step(static_cast<cudaStream_t>(stream));
-    API_END
-}
-int sr3_stream_retire(sr3_stream* s, int slot, float* out, void* stream) {
-    API_BEGIN
-    REQUIRE(s, "null stream");
-    s->retire(slot, out, static_cast<cudaStream_t>(stream));
-    API_END
-}
-int sr3_stream_slot_state(const sr3_stream* s, int* t, int* state) {
-    API_BEGIN
-    REQUIRE(s && t && state, "null argument");
-    for (int i = 0; i < (int)s->host.size(); ++i) {
-        t[i] = s->host[i].t;
-        state[i] = !s->held[i] ? 0 : s->host[i].active ? 1 : 2;
-    }
     API_END
 }
 int sr3_wstream_create(sr3_engine* e, uint64_t seed, int overlap_h, int overlap_w, sr3_wstream** out) {

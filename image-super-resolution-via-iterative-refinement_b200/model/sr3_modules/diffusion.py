@@ -242,16 +242,37 @@ class GaussianDiffusion(nn.Module):
         requests are in flight makes the next step raise."""
         if not self.conditional:
             raise ValueError("super_resolution_stream needs a conditional model; use sample_stream")
-        return self._stream(requests, slots, seed, first_index)
+        return self._stream(requests, None, slots, seed, first_index)
 
     def sample_stream(self, n, slots=16, seed=None):
         """sample() for n images of image_size through the continuous-batching engine; yields (index, image [C, H, W])."""
         if self.conditional:
             raise ValueError("sample_stream needs an unconditional model; use super_resolution_stream")
-        return self._stream(((i, None) for i in range(int(n))), slots, seed, 0)
+        return self._stream(((i, None) for i in range(int(n))), None, slots, seed, 0)
 
-    def _stream_request(self, req, size):
-        """(key, cond, x_T or None, (H, W)) of one request, checked against the stream's size (None for the first request)."""
+    def super_resolution_windowed_stream(self, requests, window=None, overlap=None, slots=16, seed=None, first_index=0):
+        """super_resolution_windowed for a stream of requests of ANY sizes, with continuous batching: a generator over `requests`, any
+        iterable (read lazily) of (key, x_in) or (key, x_in, x_T) with x_in [C, H, W], H and W at least the window's.  Every request is a
+        canvas of overlapping `window` crops (window and overlap as in super_resolution_windowed) that takes one of the engine's `slots`
+        per window and runs at its own timestep; windows of different requests share the batch.  A request is admitted first come first
+        served once its windows' slots are free (_native.windowed_stream_plan) and its (key, image [C, H, W]) is yielded as soon as its T
+        steps are done.  The n-th request's draws are keyed by sample index first_index + n (x_T ~ randn when not given): its image is
+        super_resolution_windowed(x_in[None], window, overlap, x_T=x_T[None], seed=seed, first_index=first_index + n) on the same engine
+        with its windows in the same slots, bit for bit (DESIGN.md 3.10: on some plans the slot a window runs in changes it within rounding).  A request is checked when it is read, before it is admitted (ValueError naming its key): its shape, a canvas smaller
+        than the window, more windows than `slots` (use super_resolution_windowed for it).  A schedule change while requests are in
+        flight makes the next step raise."""
+        if not self.conditional:
+            raise ValueError("super_resolution_windowed_stream needs a conditional model; use sample_stream")
+        slots = int(slots)
+        if slots < 1:
+            raise ValueError("slots must be >= 1, got %d" % slots)
+        wh, ww = (self.image_size, self.image_size) if window is None else (int(window[0]), int(window[1]))
+        geometry = self._window_geometry(wh, ww, (wh, ww), overlap)     # checks window and overlap now
+        return self._stream(requests, geometry, slots, seed, first_index)
+
+    def _stream_request(self, req, geometry, slots, single_size):
+        """(geometry, (key, cond, x_T or None, (H, W), windows)) of one request, checked against the stream's geometry and slot count.  A
+        single-size stream takes its geometry from its first request, one window of that size, and refuses every other size."""
         from ... import _native
         if not isinstance(req, (tuple, list)) or len(req) not in (2, 3):
             raise ValueError("a request is (key, x_in) or (key, x_in, x_T), got %r" % (type(req),))
@@ -263,94 +284,11 @@ class GaussianDiffusion(nn.Module):
             hw = (int(x_in.shape[1]), int(x_in.shape[2]))
         else:
             hw = (self.image_size, self.image_size)
-        if size is None:
-            _native.check_image_size(len(self.denoise_fn.arch["channel_mults"]), *hw)
-        elif hw != size:
-            raise ValueError("request %r is %dx%d; this stream runs %dx%d (each size needs its own stream)" % (key, *hw, *size))
-        if x_T is not None and tuple(x_T.shape) != (self.channels,) + hw:
-            raise ValueError("request %r: x_T must be %s, got %s" % (key, (self.channels,) + hw, tuple(x_T.shape)))
-        return key, x_in, x_T, hw
-
-    @torch.no_grad()
-    def _stream(self, requests, slots, seed, first_index):
-        from ... import _native
-        slots = int(slots)
-        if slots < 1:
-            raise ValueError("slots must be >= 1, got %d" % slots)
-        device = self.betas.device
-        if seed is None:
-            seed = int(torch.randint(0, 2 ** 62, (1,)).item())
-        reqs = iter(requests)
-        size, sampler, plan = None, None, None
-        step, n, exhausted = 0, 0, False
-        running = {}                           # slot -> (key, finish step)
-        while True:
-            # the requests admitted at this step: one per free slot, all checked before the first of them is admitted
-            batch = []
-            while not exhausted and len(running) + len(batch) < slots:
-                try:
-                    req = next(reqs)
-                except StopIteration:
-                    exhausted = True
-                    break
-                key, cond, x_T, size = self._stream_request(req, size)
-                batch.append((key, cond, x_T))
-            if batch and sampler is None:
-                eng = self._engine(slots, *size)
-                if eng.T == 0:
-                    raise RuntimeError("set_new_noise_schedule has not been called")
-                sampler, T = _native.StreamSampler(eng, seed), eng.T
-                clock = [0]
-                plan = _native.stream_plan(iter(lambda: clock[0], None), slots, T)     # every request arrives when it is read
-            if batch and sampler.engine.T != T:
-                raise RuntimeError("sr3_b200: the noise schedule changed during the stream (n_timestep %d -> %d)" % (T, sampler.engine.T))
-            for key, cond, x_T in batch:
-                slot, admit, finish = next(plan)
-                assert admit == step and slot not in running, (slot, admit, step)
-                if x_T is None:
-                    x_T = torch.randn((self.channels,) + size, device=device)
-                sampler.admit(slot, cond, x_T, first_index + n)
-                n += 1
-                running[slot] = (key, finish)
-            if not running:
-                return
-            sampler.step()
-            step += 1
-            clock[0] = step
-            for slot in sorted(s for s, (_, f) in running.items() if f == step):
-                yield running.pop(slot)[0], sampler.retire(slot)
-
-    # ---- continuous batching of canvases of any size, see DESIGN.md 3.11
-    def super_resolution_windowed_stream(self, requests, window=None, overlap=None, slots=16, seed=None, first_index=0):
-        """super_resolution_windowed for a stream of requests of ANY sizes, with continuous batching: a generator over `requests`, any
-        iterable (read lazily) of (key, x_in) or (key, x_in, x_T) with x_in [C, H, W], H and W at least the window's.  Every request is a
-        canvas of overlapping `window` crops (window and overlap as in super_resolution_windowed) that takes one of the engine's `slots`
-        per window and runs at its own timestep; windows of different requests share the batch.  A request is admitted first come first
-        served once its windows' slots are free (_native.windowed_stream_plan) and its (key, image [C, H, W]) is yielded as soon as its T
-        steps are done.  The n-th request's draws are keyed by sample index first_index + n (x_T ~ randn when not given): its image is
-        super_resolution_windowed(x_in[None], window, overlap, x_T=x_T[None], seed=seed, first_index=first_index + n) on the same engine
-        with its windows in the same slots, bit for bit (DESIGN.md 3.11: on some plans the slot a window runs in changes it within rounding).  A request is checked when it is read, before it is admitted (ValueError naming its key): its shape, a canvas smaller
-        than the window, more windows than `slots` (use super_resolution_windowed for it).  A schedule change while requests are in
-        flight makes the next step raise."""
-        if not self.conditional:
-            raise ValueError("super_resolution_windowed_stream needs a conditional model; use sample_stream")
-        slots = int(slots)
-        if slots < 1:
-            raise ValueError("slots must be >= 1, got %d" % slots)
-        wh, ww = (self.image_size, self.image_size) if window is None else (int(window[0]), int(window[1]))
-        geometry = self._window_geometry(wh, ww, (wh, ww), overlap)     # checks window and overlap now
-        return self._windowed_stream(requests, geometry, slots, seed, first_index)
-
-    def _windowed_stream_request(self, req, geometry, slots):
-        """(key, cond, x_T or None, (H, W), windows) of one request, checked against the stream's window and slot count."""
-        from ... import _native
-        if not isinstance(req, (tuple, list)) or len(req) not in (2, 3):
-            raise ValueError("a request is (key, x_in) or (key, x_in, x_T), got %r" % (type(req),))
-        key, x_in, x_T = (tuple(req) + (None,))[:3]
-        cond_c = self.denoise_fn.arch["in_channel"] - self.channels
-        if not torch.is_tensor(x_in) or x_in.dim() != 3 or x_in.shape[0] != cond_c:
-            raise ValueError("request %r: x_in must be [%d, H, W], got %s" % (key, cond_c, tuple(getattr(x_in, "shape", ()))))
-        hw = (int(x_in.shape[1]), int(x_in.shape[2]))
+        if single_size and geometry is None:
+            geometry = self._window_geometry(*hw, hw, 0)                # _native.check_image_size: UnsupportedSizeError
+        elif single_size and hw != geometry[0]:
+            # a larger request would otherwise become a canvas of several windows
+            raise ValueError("request %r is %dx%d; this stream runs %dx%d (each size needs its own stream)" % (key, *hw, *geometry[0]))
         (wh, ww), (ovh, ovw) = geometry
         if hw[0] < wh or hw[1] < ww:
             raise ValueError("request %r: canvas %dx%d is smaller than the window %dx%d (canvases are not padded)" % (key, *hw, wh, ww))
@@ -360,11 +298,16 @@ class GaussianDiffusion(nn.Module):
                              % (key, *hw, n, slots))
         if x_T is not None and tuple(x_T.shape) != (self.channels,) + hw:
             raise ValueError("request %r: x_T must be %s, got %s" % (key, (self.channels,) + hw, tuple(x_T.shape)))
-        return key, x_in, x_T, hw, n
+        return geometry, (key, x_in, x_T, hw, n)
 
     @torch.no_grad()
-    def _windowed_stream(self, requests, geometry, slots, seed, first_index):
+    def _stream(self, requests, geometry, slots, seed, first_index):
+        """The request loop of every stream.  geometry ((wh, ww), (overlap_h, overlap_w)), or None for a single-size stream."""
         from ... import _native
+        slots = int(slots)
+        if slots < 1:
+            raise ValueError("slots must be >= 1, got %d" % slots)
+        single_size = geometry is None
         device = self.betas.device
         if seed is None:
             seed = int(torch.randint(0, 2 ** 62, (1,)).item())
@@ -383,7 +326,8 @@ class GaussianDiffusion(nn.Module):
                     except StopIteration:
                         exhausted = True
                         break
-                    pending = (step,) + self._windowed_stream_request(req, geometry, slots)
+                    geometry, checked = self._stream_request(req, geometry, slots, single_size)
+                    pending = (step,) + checked
                 if pending[5] > free:
                     break
                 batch.append(pending)

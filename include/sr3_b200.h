@@ -235,34 +235,8 @@ int sr3_windowed_phase_begin(sr3_windowed* w, int t_start, void* stream);
 int sr3_windowed_phase_means(sr3_windowed* w, void* stream);
 int sr3_windowed_phase_merge(sr3_windowed* w, void* stream);
 
-/* ---- continuous batching: serve a stream of requests on one inference engine, every slot (one of the engine's B images) at its own
- * timestep.  A slot takes a request (sr3_stream_admit), runs exactly T reverse steps, one per sr3_stream_step, and then holds x_0 until
- * sr3_stream_retire copies it out and frees the slot.  A step is the engine's step graph in its UNet.forward form (eps of every image,
- * noise level of slot s = sqrt_alphas_cumprod_prev[t_s + 1]) followed by one kernel that applies p_sample's posterior update to every
- * running slot at its own t_s, with z from Philox keyed by (seed, the request's sample_index, pixel, t_s), and advances the slots.  Every
- * UNet op is per image, so a request's x_0 equals what sr3_p_sample_loop computes for the same condition, x_T and sample index
- * (first_sample_index + b = sample_index) at the same slot b, bit for bit, whatever the other slots hold.  No step synchronises the host
- * or copies to it: the host mirrors the slot table, since every request takes exactly T steps.
- * The stream BORROWS the engine (which must outlive it) and its buffers: nothing else may run on that engine while requests are in flight,
- * and all calls of one stream go to one CUDA stream.  Creating a stream zeroes the engine's state and input; retiring a slot zeroes
- * that slot's. */
-typedef struct sr3_stream sr3_stream;
-int sr3_stream_create(sr3_engine* e, uint64_t seed, sr3_stream** out);
-void sr3_stream_destroy(sr3_stream* s);
-/* Load one request into a free slot: condition_x (NULL for an unconditional model) and x_T DEVICE fp32 [3,H,W] at the engine's H x W
- * (copied); its first step runs at t = T - 1.  Refused, with no slot changed: a slot out of range or busy (running, or finished and not
- * retired), an engine with no schedule, a schedule changed since the requests in flight were admitted. */
-int sr3_stream_admit(sr3_stream* s, int slot, const float* condition_x, const float* x_T, uint64_t sample_index, void* stream);
-/* One reverse step of every running slot.  Refused when the engine has no schedule or sr3_engine_set_schedule was called while requests
- * are in flight (they would finish on a mixed schedule). */
-int sr3_stream_step(sr3_stream* s, void* stream);
-/* Copy the x_0 of a finished slot to `out` (DEVICE fp32 [3,H,W]) and free the slot.  Refuses a running or free slot. */
-int sr3_stream_retire(sr3_stream* s, int slot, float* out, void* stream);
-/* HOST t[B], state[B]: state 0 free, 1 running (t = timestep of its next step), 2 finished and not yet retired (t = -1). */
-int sr3_stream_slot_state(const sr3_stream* s, int* t, int* state);
-
-/* ---- continuous batching of windowed canvases: serve a stream of conditional requests of ANY size (each at least the engine's H x W,
- * the window) on one inference engine.  A request is a canvas whose ny x nx overlapping windows (the grid and fp32 blend weights of
+/* ---- continuous batching: serve a stream of requests of ANY size (each at least the engine's H x W, the window) on one inference
+ * engine, every request at its own timestep.  A request is a canvas whose ny x nx overlapping windows (the grid and fp32 blend weights of
  * sr3_windowed_*, with the stream's overlap) take ny * nx of the engine's B slots, one window each; all windows of a request run at the
  * request's own timestep, windows of different requests at different timesteps share the batch.  A request takes exactly T steps, one
  * per sr3_wstream_step, and then waits for sr3_wstream_retire.  A step is: a gather of every slot's window crop of its canvas (idle slots
@@ -272,20 +246,22 @@ int sr3_stream_slot_state(const sr3_stream* s, int* t, int* state);
  * Bit-exactness: a request's x_0 equals what sr3_windowed_* computes for that canvas alone as image 0 with first_sample_index =
  * sample_index on an engine of the same shape with its windows in the same slots, bit for bit, whatever the other slots hold and whenever
  * it was admitted (every UNet op is per image; the means and the merge are the windowed sampler's arithmetic operation for operation).
- * Whether the slots matter depends on the plan: on a 4x4-lowest-level plan a window moved to another slot changes within rounding.
+ * A window-sized request (one window, weight 1) in slot b equals what sr3_p_sample_loop computes for the same condition, x_T and
+ * first_sample_index + b = sample_index at image b, bit for bit.  Whether the slots matter depends on the plan: on a 4x4-lowest-level
+ * plan a window moved to another slot changes within rounding.
  * No step synchronises the host, copies to it or allocates: the host mirrors the request table, since every request takes exactly T steps.
  * The stream BORROWS the engine (which must outlive it; nothing else may run on it while requests are in flight, and all calls of one
  * stream go to one CUDA stream) and every admitted canvas until its request is retired.  Creating a stream zeroes the engine's state
- * and input.  Refused at creation: a training engine, an unconditional model, an overlap outside [0, window side). */
+ * and input.  Refused at creation: a training engine, an overlap outside [0, window side). */
 typedef struct sr3_wstream sr3_wstream;
 int sr3_wstream_create(sr3_engine* e, uint64_t seed, int overlap_h, int overlap_w, sr3_wstream** out);
 void sr3_wstream_destroy(sr3_wstream* s);
 /* Admit one request into the n_slots free slots `slots` (HOST, window k of the grid, row-major, into slots[k]).  condition_x: DEVICE fp32
- * [cond_c][height][width], x: DEVICE fp32 [3][height][width] holding x_T, overwritten with x_{t-1} by every step and holding x_0 once the
- * request has finished; both are BORROWED until sr3_wstream_retire, nothing is copied but the window geometry.  *request = the request's
+ * [cond_c][height][width] (NULL for an unconditional model), x: DEVICE fp32 [3][height][width] holding x_T, overwritten with x_{t-1} by
+ * every step and holding x_0 once the request has finished; both are BORROWED until sr3_wstream_retire, nothing is copied but the window geometry.  *request = the request's
  * id, its first step runs at t = T - 1.  Refused, with no slot or request changed: a slot out of range, busy or listed twice, n_slots other
- * than the canvas's window count, a canvas smaller than the window, null canvases, an engine with no schedule, a schedule changed since
- * the requests in flight were admitted. */
+ * than the canvas's window count, a canvas smaller than the window, a null x, a condition missing for a conditional model or given to an
+ * unconditional one, an engine with no schedule, a schedule changed since the requests in flight were admitted. */
 int sr3_wstream_admit(sr3_wstream* s, const int* slots, int n_slots, const float* condition_x, float* x, int height, int width,
                       uint64_t sample_index, int* request, void* stream);
 /* One reverse step of every running request.  Refused when the engine has no schedule or sr3_engine_set_schedule was called while

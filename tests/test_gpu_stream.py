@@ -1,5 +1,5 @@
-"""Continuous batching on the device (GaussianDiffusion.super_resolution_stream / sample_stream, _native.StreamSampler, sr3_stream_*):
-every slot of the engine at its own timestep, refilled as its image finishes (DESIGN.md 3.10).
+"""Continuous batching on the device (GaussianDiffusion.super_resolution_stream / sample_stream, and _native.WindowedStreamSampler with
+one-window requests): every slot of the engine at its own timestep, refilled as its image finishes (DESIGN.md 3.10).
 
 What is pinned, bit for bit (torch.equal): a request's image is the lockstep sampler's image for the same condition, x_T and sample index
 at the slot stream_plan gave it, whatever the other slots hold and whenever it was admitted; a stream leaves the engine as it found it;
@@ -88,7 +88,7 @@ def test_unconditional_sample_stream_is_the_lockstep_sampler(monkeypatch, precis
 
 @pytest.mark.timeout(900)
 @pytest.mark.parametrize("config,H,W", [("tiny", 32, 32), ("sr16_64", 64, 64)])
-def test_staggered_arrivals_are_independent_of_the_neighbours(monkeypatch, config, H, W):
+def test_staggered_one_window_requests_are_independent_of_the_neighbours(monkeypatch, config, H, W):
     """11 requests through 4 slots, arriving over the steps; driven through the online interface exactly as stream_plan says."""
     net = build(monkeypatch, config)
     T, N, seed, first = SCHED12["n_timestep"], 11, 99, 1000
@@ -96,18 +96,19 @@ def test_staggered_arrivals_are_independent_of_the_neighbours(monkeypatch, confi
     arrivals = [0, 0, 3, 5, 5, 9, 14, 15, 22, 30, 31]
     plan = list(_native.stream_plan(arrivals, B, T))
     assert len({a for _, a, _ in plan}) > 3 and len({s for s, _, _ in plan}) == B     # admitted at many steps, into every slot
-    s = _native.StreamSampler(net._engine(B, H, W), seed)
-    out = {}
+    s = _native.WindowedStreamSampler(net._engine(B, H, W), seed, 0, 0)
+    ids, out = {}, {}
     for k in range(max(f for _, _, f in plan)):
         for n, (slot, a, _) in enumerate(plan):
             if a == k:
-                s.admit(slot, cond[n], x_T[n], first + n)
+                ids[n] = s.admit([slot], cond[n], x_T[n], first + n)
         s.step()
         done = [n for n, (_, _, f) in enumerate(plan) if f == k + 1]
-        assert sorted(s.finished()) == sorted(plan[n][0] for n in done)
+        assert sorted(i for i, v in enumerate(s.slot_state()[2]) if v == 2) == sorted(plan[n][0] for n in done)
+        assert s.finished() == sorted(ids[n] for n in done)
         for n in done:
-            out[n] = s.retire(plan[n][0])
-    assert s.slot_state() == ([-1] * B, [0] * B)
+            out[n] = s.retire(ids[n])
+    assert s.slot_state() == ([-1] * B, [-1] * B, [0] * B)
     for n, (slot, _, _) in enumerate(plan):
         assert torch.equal(out[n], lockstep_at(net, cond, x_T, n, slot, first + n, seed)), n
 
@@ -148,35 +149,35 @@ def test_a_stream_leaves_no_state_behind(monkeypatch):
 
 
 @pytest.mark.timeout(900)
-def test_bad_calls_are_refused_and_change_no_slot(monkeypatch):
+def test_bad_one_window_calls_are_refused_and_change_no_slot(monkeypatch):
     net = build(monkeypatch, "tiny")
     cond, x_T = draws(B, 32, 32, 5)
-    s = _native.StreamSampler(net._engine(B, 32, 32), 1)
-    s.admit(1, cond[0], x_T[0], 0)
+    s = _native.WindowedStreamSampler(net._engine(B, 32, 32), 1, 0, 0)
+    r = s.admit([1], cond[0], x_T[0], 0)
     s.step(3)
     state = s.slot_state()
-    assert state == ([-1, 8, -1, -1], [0, 1, 0, 0])
+    assert state == ([-1, r, -1, -1], [-1, 8, -1, -1], [0, 1, 0, 0])
     with pytest.raises(RuntimeError, match="slot 4 out of range"):
-        s.admit(4, cond[1], x_T[1], 1)
+        s.admit([4], cond[1], x_T[1], 1)
     with pytest.raises(RuntimeError, match="slot -1 out of range"):
-        s.admit(-1, cond[1], x_T[1], 1)
+        s.admit([-1], cond[1], x_T[1], 1)
     with pytest.raises(RuntimeError, match="slot 1 is busy"):
-        s.admit(1, cond[1], x_T[1], 1)
-    with pytest.raises(RuntimeError, match="slot 1 is still running"):
-        s.retire(1)
-    with pytest.raises(RuntimeError, match="slot 0 holds no request"):
-        s.retire(0)
-    with pytest.raises(RuntimeError, match="condition_x is required"):
-        s.admit(0, None, x_T[1], 1)
-    with pytest.raises(ValueError, match="this stream's slots are"):
-        s.admit(0, cond[1, :, :16], x_T[1], 1)
+        s.admit([1], cond[1], x_T[1], 1)
+    with pytest.raises(RuntimeError, match="request %d is still running" % r):
+        s.retire(r)
+    with pytest.raises(RuntimeError, match="request %d is not held" % (r + 1)):
+        s.retire(r + 1)
+    with pytest.raises(RuntimeError, match="condition_x is required by a conditional model"):
+        s.admit([0], None, x_T[1], 1)
+    with pytest.raises(ValueError, match="x_T has shape"):
+        s.admit([0], cond[1, :, :16], x_T[1], 1)
     assert s.slot_state() == state
     # a schedule change with a request in flight: the next step (and any admit) is refused, nothing moves
     net.set_new_noise_schedule(dict(SCHED12, n_timestep=10), "cuda")
     with pytest.raises(RuntimeError, match="noise schedule changed while requests are in flight"):
         s.step()
     with pytest.raises(RuntimeError, match="noise schedule changed while requests are in flight"):
-        s.admit(0, cond[1], x_T[1], 1)
+        s.admit([0], cond[1], x_T[1], 1)
     assert s.slot_state() == state
     # the generator refuses to go on once the schedule it planned with has changed
     net.set_new_noise_schedule(SCHED12, "cuda")
@@ -189,14 +190,14 @@ def test_bad_calls_are_refused_and_change_no_slot(monkeypatch):
 
 
 @pytest.mark.timeout(900)
-def test_a_step_without_a_schedule_is_refused(monkeypatch):
+def test_a_one_window_stream_without_a_schedule_is_refused(monkeypatch):
     net = build(monkeypatch, "tiny")
     cfg = dict(net.denoise_fn.arch, channels=3, conditional=True, precision="bf16")
     eng = _native.Engine(cfg, B, torch.device("cuda"), height=32, width=32)     # never given a schedule
-    s = _native.StreamSampler(eng, 1)
+    s = _native.WindowedStreamSampler(eng, 1, 0, 0)
     cond, x_T = draws(1, 32, 32, 6)
     with pytest.raises(RuntimeError, match="no noise schedule"):
         s.step()
     with pytest.raises(RuntimeError, match="no noise schedule"):
-        s.admit(0, cond[0], x_T[0], 0)
-    assert s.slot_state() == ([-1] * B, [0] * B)
+        s.admit([0], cond[0], x_T[0], 0)
+    assert s.slot_state() == ([-1] * B, [-1] * B, [0] * B)

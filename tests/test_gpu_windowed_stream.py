@@ -1,6 +1,6 @@
 """Continuous batching of canvases of any size on the device (GaussianDiffusion.super_resolution_windowed_stream,
 _native.WindowedStreamSampler, sr3_wstream_*): every request's windows take slots of one engine and run at the request's own timestep
-(DESIGN.md 3.11).
+(DESIGN.md 3.10).
 
 What is pinned, bit for bit (torch.equal): a request's image is super_resolution_windowed of that request alone on the same engine,
 whatever its neighbours, whichever slots it got and whenever it was admitted; a window-sized request is super_resolution; a stream leaves
@@ -213,7 +213,7 @@ def test_bad_calls_are_refused_and_change_no_slot(monkeypatch):
 
 
 @pytest.mark.timeout(900)
-def test_a_step_without_a_schedule_is_refused(monkeypatch):
+def test_a_step_without_a_schedule_or_with_a_wrong_condition_is_refused(monkeypatch):
     slots = 4
     net = build(monkeypatch, "tiny", slots=slots)
     cfg = dict(net.denoise_fn.arch, channels=3, conditional=True, precision="bf16")
@@ -225,6 +225,14 @@ def test_a_step_without_a_schedule_is_refused(monkeypatch):
     with pytest.raises(RuntimeError, match="no noise schedule"):
         s.admit([0], c, x, 0)
     assert s.slot_state() == ([-1] * slots, [-1] * slots, [0] * slots)
-    with pytest.raises(RuntimeError, match="needs a conditional model"):
-        _native.WindowedStreamSampler(_native.Engine(dict(cfg, in_channel=3, conditional=False), slots, torch.device("cuda"),
-                                                     height=32, width=32), 1, 8, 8)
+    # an unconditional model streams too, and its requests carry no condition; a conditional model's requests must
+    unc = _native.WindowedStreamSampler(_native.Engine(dict(cfg, in_channel=3, conditional=False), slots, torch.device("cuda"),
+                                                       height=32, width=32), 1, 8, 8)
+    with pytest.raises(ValueError, match=r"condition_x must be \[0, H, W\]"):
+        unc.admit([0], c, x, 0)
+    assert unc.slot_state() == ([-1] * slots, [-1] * slots, [0] * slots)
+    del s
+    s = _native.WindowedStreamSampler(net._engine(slots, 32, 32), 1, 8, 8)
+    with pytest.raises(RuntimeError, match="condition_x is required by a conditional model"):
+        s.admit([0], None, x, 0)
+    assert s.slot_state() == ([-1] * slots, [-1] * slots, [0] * slots)

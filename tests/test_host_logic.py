@@ -28,7 +28,7 @@ def make_opt(unet, image_size, conditional=True, phase="val"):
 FULL = dict(in_channel=6, out_channel=3, inner_channel=64, channel_multiplier=[1, 2, 4, 8, 8], attn_res=[16], res_blocks=2, dropout=0.2)
 
 
-def test_library_exports_every_header_symbol():
+def test_library_exports_every_header_symbol_and_its_abi_version():
     header = open(os.path.join(ROOT, "include", "sr3_b200.h")).read()
     declared = set(re.findall(r"\b(sr3_[a-z0-9_]+)\s*\(", header))
     assert declared, "no declarations parsed"
@@ -36,7 +36,7 @@ def test_library_exports_every_header_symbol():
     for name in sorted(declared):
         assert hasattr(lib, name), f"{name} declared in sr3_b200.h but not exported by the library"
     assert declared == set(_native.EXPORTED_SYMBOLS), declared ^ set(_native.EXPORTED_SYMBOLS)
-    assert _native.lib().sr3_abi_version() == 4          # v4: the step-kernel entry points are gone
+    assert _native.lib().sr3_abi_version() == 5          # v5: the single-size stream entry points are gone
 
 
 def test_state_dict_layout_matches_reference_names_and_init():

@@ -130,19 +130,3 @@ def test_stream_without_a_gpu_fails_loudly():
     with pytest.raises((_native.NativeLibraryError, RuntimeError)):
         list(net.super_resolution_stream([(0, torch.zeros(3, 32, 32))], slots=2))
 
-
-def test_slot_update_kernel_does_not_spill():
-    """ptxas -v of slot_update_kernel (lib/build.log, built first if needed: nvcc needs no GPU): no stack frame, no spills."""
-    import importlib.util
-    import os
-    import re
-    pkg = os.path.dirname(_native.__file__)
-    spec = importlib.util.spec_from_file_location("sr3_b200_build_for_stream_test", os.path.join(pkg, "build.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    mod.build(force=False)
-    log = open(os.path.join(pkg, "lib", "build.log")).read()
-    props = re.findall(r"Function properties for \S*slot_update_kernel\S*\n\s*(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads",
-                       log)
-    assert props, "slot_update_kernel not found in the ptxas report"
-    assert all(p == ("0", "0", "0") for p in props), props

@@ -1,6 +1,6 @@
-"""Continuous batching (GaussianDiffusion.super_resolution_stream, sr3_stream_*) on the 16->128 config at 128x128 with 16 slots.
-Prints one JSON line:
-  * steady-state ms per step with every slot busy, the stream (engine step graph + slot_update_kernel) against sr3_p_sample_steps
+"""Continuous batching (GaussianDiffusion.super_resolution_stream: one-window requests on sr3_wstream_*) on the 16->128 config at
+128x128 with 16 slots.  Prints one JSON line:
+  * steady-state ms per step with every slot busy, the stream (gather + engine step graph + means + merge) against sr3_p_sample_steps
     (the lockstep sampler) on the same engine, the two arms alternated round by round (CUDA events around K steps; median and min..max);
   * request latency under Poisson arrivals at several loads for two policies, in steps from the deterministic plans (the lockstep policy
     starts a batch when the previous one ends, with the requests waiting at that moment; the continuous one is _native.stream_plan) and
@@ -101,16 +101,16 @@ def main():
         return e0.elapsed_time(e1) / args.steps
 
     def stream():
-        s = _native.StreamSampler(eng, 7)
+        s = _native.WindowedStreamSampler(eng, 7, 0, 0)
         for k in range(SLOTS):
-            s.admit(k, cond[k], x_T[k], k)
+            s.admit([k], cond[k], x_T[k], k)
         s.step(args.warmup)
         torch.cuda.synchronize()
         e0.record()
         s.step(args.steps)
         e1.record()
         torch.cuda.synchronize()
-        assert s.slot_state()[1] == [1] * SLOTS
+        assert s.slot_state()[2] == [1] * SLOTS
         assert torch.isfinite(eng.read_state()).all()
         return e0.elapsed_time(e1) / args.steps
 
