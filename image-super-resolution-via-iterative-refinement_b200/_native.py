@@ -123,6 +123,9 @@ _SIGS = {
     "sr3_bench_conv": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, POINTER(c_float)]),
     "sr3_test_gemm": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "sr3_test_attention": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    "sr3_test_attention_dn": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    "sr3_attention_dn": (c_int, [c_int, c_int, c_int, c_int, POINTER(c_int)]),
+    "sr3_bench_attention": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, POINTER(c_float)]),
     "sr3_test_conv_groupnorm": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
                                         c_int, c_void_p]),
     "sr3_test_conv": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
@@ -875,6 +878,29 @@ def test_attention(qk_bf16, vT_bf16, nz, Lt, HW, C):
     out = torch.empty(nz * Lt, C, device=qk_bf16.device, dtype=torch.bfloat16)
     _check(lib().sr3_test_attention(_ptr(qk_bf16), _ptr(vT_bf16), _ptr(out), nz, Lt, HW, C, _stream()))
     return out
+
+
+def test_attention_dn(qk_bf16, vT_bf16, nz, Lt, HW, C, dn):
+    """test_attention with attn_kernel's channel slice forced to dn (64, 128 or 256; 0 = the one the library picks)."""
+    out = torch.empty(nz * Lt, C, device=qk_bf16.device, dtype=torch.bfloat16)
+    _check(lib().sr3_test_attention_dn(_ptr(qk_bf16), _ptr(vT_bf16), _ptr(out), nz, Lt, HW, C, dn, _stream()))
+    return out
+
+
+def attention_dn(nz, Lt, C, sms=0):
+    """Output channels per CTA the fused attention core runs at for this shape on a GPU of `sms` SMs (0: the current device's)."""
+    dn = c_int()
+    _check(lib().sr3_attention_dn(nz, Lt, C, sms, ctypes.byref(dn)))
+    return dn.value
+
+
+def bench_attention(qk_bf16, vT_bf16, nz, Lt, HW, C, dn=0, reps=50):
+    """Average ms of one fused attention launch (one captured graph of `reps` launches) and its output."""
+    out = torch.empty(nz * Lt, C, device=qk_bf16.device, dtype=torch.bfloat16)
+    ms = c_float()
+    torch.cuda.synchronize()
+    _check(lib().sr3_bench_attention(_ptr(qk_bf16), _ptr(vT_bf16), _ptr(out), nz, Lt, HW, C, dn, reps, ctypes.byref(ms)))
+    return ms.value, out
 
 
 def test_gemm(a_bf16, b_bf16, block_n):

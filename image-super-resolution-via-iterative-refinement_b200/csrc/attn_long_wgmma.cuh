@@ -27,6 +27,7 @@
 
 namespace sr3 {
 
+constexpr int ATTNL_THREADS = 288;                       // two consumer warpgroups + the TMA producer warp (ATTN_PRODUCER_WARP)
 constexpr int ATTNL_KB = 128;                            // keys per block
 constexpr int ATTNL_DN = 128;                            // output channels per CTA
 constexpr int ATTNL_STAGES = 5;
@@ -34,7 +35,7 @@ constexpr int ATTNL_STAGE_BYTES = 16384 + 16384;         // S stage: q chunk 128
 constexpr int ATTNL_P_BYTES = 128 * ATTNL_KB * 2;        // P~: 128 rows x 128 keys, as two K chunks of 64
 constexpr int ATTNL_SMEM_BYTES = 1024 + GEMM_HDR_BYTES + ATTNL_STAGES * ATTNL_STAGE_BYTES + ATTNL_P_BYTES;
 
-__global__ void __launch_bounds__(ATTN_THREADS, 1) attn_long_kernel(const __grid_constant__ AttnParams p) {
+__global__ void __launch_bounds__(ATTNL_THREADS, 1) attn_long_kernel(const __grid_constant__ AttnParams p) {
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw = smem_u32(smem_raw);
     const uint32_t bar_base = (raw + 1023u) & ~1023u;                  // header: barriers

@@ -10,7 +10,12 @@
 // sequences (32x32 mid block of the 64->512 config, larger images) run attn_long_kernel (attn_long_wgmma.cuh).
 //
 // Operands (both produced by tile-kernel launches): qk [nz*Lt][2C] bf16 (q = columns [0,C), k = [C,2C)), vT [nz*C][Lt] bf16.
-// Warp roles: 8 = TMA producer, 0..7 = two warpgroups, each owning 64 query rows: S (64 x Lt) and O (64 x DN) in registers.
+// Warp roles, as in the tile kernel (gemm_wgmma.cuh): warps 0..7 are two consumer warpgroups, each owning 64 query rows with S (64 x Lt)
+// and then O (64 x DN) in registers; warps 8..11 are the producer warpgroup, of which warp 8 issues the TMA loads.  384 threads start at
+// 168 registers each; after the set-up the producer warpgroup drops to 40 and the consumers rise to 232 (setmaxnreg), so the 128-float
+// S row block of Lt = 256 and the 128-float O block of DN = 256 stay in registers instead of spilling.
+// DN (64, 128 or 256 of the C output channels per CTA) is picked per shape on the host (make_attn_op): it only decides which CTA
+// computes which columns, not how any column is summed.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda.h>
@@ -18,8 +23,13 @@
 
 namespace sr3 {
 
-constexpr int ATTN_THREADS = 288;
+constexpr int ATTN_THREADS = 384;
+constexpr int ATTN_CONSUMER_WARPS = 8;
 constexpr int ATTN_PRODUCER_WARP = 8;
+constexpr int ATTN_CONSUMER_REGS = 232;
+constexpr int ATTN_PRODUCER_REGS = 40;
+static_assert(ATTN_CONSUMER_WARPS * 32 * ATTN_CONSUMER_REGS + (ATTN_THREADS - ATTN_CONSUMER_WARPS * 32) * ATTN_PRODUCER_REGS <= 65536, "register file");
+static_assert(ATTN_THREADS == 384 && ATTN_PRODUCER_WARP == ATTN_CONSUMER_WARPS, "setmaxnreg acts on whole warpgroups: 2 consumer + 1 producer");
 constexpr int ATTN_STAGES = 3;
 constexpr int ATTN_STAGE_BYTES = 16384 + 32768;          // A: 128 rows x 64 | B: up to 256 rows x 64 (bf16, 128B-swizzled)
 constexpr int ATTN_P_BYTES = 65536;                      // P: 128 rows x up to 256 keys, as K chunks of 64
@@ -27,20 +37,24 @@ constexpr int ATTN_SMEM_BYTES = 1024 + GEMM_HDR_BYTES + ATTN_STAGES * ATTN_STAGE
 
 struct AttnParams {
     CUtensorMap qk_map;      // 2-D bf16 [nz*Lt rows][2C], box {64, 128}
-    CUtensorMap vt_map;      // 2-D bf16 [nz*C rows][Lt], box {64, 128}
+    CUtensorMap vt_map;      // 2-D bf16 [nz*C rows][Lt], box {64, min(dn, 128)}
     __nv_bfloat16* out;      // [nz*Lt][C]
     int C, Lt, HW, dn, nz;
     float scale_log2e;       // log2(e) / sqrt(C)
 };
 
-// One (attention batch z, query tile qt, channel slice dc) unit for Lt = LT keys and DN output channels: the body of attn_kernel (one
-// unit per CTA).  `pm` points at the parameters in the kernel parameter space (TMA descriptors are addressed through it).
+// One CTA = one (attention batch z, query tile qt, channel slice dc) unit for Lt = LT keys and DN output channels.
 template <int LT, int DN>
-__device__ __forceinline__ void attn_unit_t(const AttnParams& p, const AttnParams* pm, const uint32_t base_in, uint8_t* base_ptr_in,
-                                            const int qt, const int dc, const int z) {
-    const uint32_t bar_base = base_in;                                 // header (gemm_wgmma.cuh)
-    const uint32_t base = base_in + GEMM_HDR_BYTES;
-    uint8_t* base_ptr = base_ptr_in + GEMM_HDR_BYTES;
+__global__ void __launch_bounds__(ATTN_THREADS, 1) attn_kernel(const __grid_constant__ AttnParams p) {
+    static_assert((LT == 128 || LT == 256) && (DN == 64 || DN == 128 || DN == 256), "attn_kernel shape");
+    constexpr int VB = DN < 128 ? DN : 128;                            // rows of one vT box (vt_map)
+    extern __shared__ uint8_t smem_raw[];
+    const uint32_t raw = smem_u32(smem_raw);
+    const uint32_t bar_base = (raw + 1023u) & ~1023u;                  // header (gemm_wgmma.cuh): barriers
+    const uint32_t base = bar_base + GEMM_HDR_BYTES;
+    uint8_t* base_ptr = smem_raw + (base - raw);
+    const int n_dc = p.C / DN;
+    const int qt = blockIdx.x / n_dc, dc = blockIdx.x % n_dc, z = blockIdx.y;
     const uint32_t p_base = base + ATTN_STAGES * ATTN_STAGE_BYTES;
     uint8_t* p_ptr = base_ptr + ATTN_STAGES * ATTN_STAGE_BYTES;
     auto full_bar = [&](int s) { return bar_base + 8u * s; };
@@ -52,8 +66,8 @@ __device__ __forceinline__ void attn_unit_t(const AttnParams& p, const AttnParam
     constexpr int kc3 = LT / 64;     // K chunks of O = P v
 
     if (threadIdx.x == 0) {
-        tma_prefetch_desc(&pm->qk_map);
-        tma_prefetch_desc(&pm->vt_map);
+        tma_prefetch_desc(&p.qk_map);
+        tma_prefetch_desc(&p.vt_map);
         for (int s = 0; s < ATTN_STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 2); }   // empty: one arrive per warpgroup
         fence_mbar_init();
     }
@@ -61,8 +75,12 @@ __device__ __forceinline__ void attn_unit_t(const AttnParams& p, const AttnParam
     pdl_launch_dependents();
     pdl_wait();                  // q, k, vT come from the two preceding launches
 
-    if (warp == ATTN_PRODUCER_WARP) {
-        // ------------------------------------------------------------ TMA producer
+    // The warp roles split here.  No block-wide barrier may follow: warps 9..11 have nothing more to do, and named barriers 2 / 3 count
+    // the 128 threads of one consumer warpgroup.
+    if (warp >= ATTN_CONSUMER_WARPS) {
+        setmaxnreg_dec<ATTN_PRODUCER_REGS>();
+        if (warp != ATTN_PRODUCER_WARP) return;
+        // ------------------------------------------------------------ TMA producer warp (converged; one elected lane issues)
         int s = 0;
         uint32_t ph = 0;
         for (int it = 0; it < kc1 + kc3; ++it) {
@@ -71,19 +89,20 @@ __device__ __forceinline__ void attn_unit_t(const AttnParams& p, const AttnParam
                 const uint32_t dst = base + s * ATTN_STAGE_BYTES;
                 if (it < kc1) {
                     mbar_arrive_expect_tx(full_bar(s), 16384 + LT * 128);
-                    tma_load_2d(dst, &pm->qk_map, full_bar(s), it * 64, z * LT + qt * 128);
+                    tma_load_2d(dst, &p.qk_map, full_bar(s), it * 64, z * LT + qt * 128);
                     for (int j = 0; j < LT / 128; ++j)
-                        tma_load_2d(dst + 16384 + j * 16384, &pm->qk_map, full_bar(s), p.C + it * 64, z * LT + j * 128);
+                        tma_load_2d(dst + 16384 + j * 16384, &p.qk_map, full_bar(s), p.C + it * 64, z * LT + j * 128);
                 } else {
                     mbar_arrive_expect_tx(full_bar(s), DN * 128);
-                    for (int j = 0; j < DN / 128; ++j)
-                        tma_load_2d(dst + 16384 + j * 16384, &pm->vt_map, full_bar(s), (it - kc1) * 64, z * p.C + dc * DN + j * 128);
+                    for (int j = 0; j < DN / VB; ++j)
+                        tma_load_2d(dst + 16384 + j * VB * 128, &p.vt_map, full_bar(s), (it - kc1) * 64, z * p.C + dc * DN + j * VB);
                 }
             }
             __syncwarp();
             if (++s == ATTN_STAGES) { s = 0; ph ^= 1u; }
         }
-    } else if (warp < ATTN_PRODUCER_WARP) {
+    } else {
+        setmaxnreg_inc<ATTN_CONSUMER_REGS>();
         // ------------------------------------------------------------ warpgroup g: query rows [64 g, 64 g + 64) of the tile
         const int g = warp >> 2;
         const int wq = warp & 3;
@@ -113,17 +132,22 @@ __device__ __forceinline__ void attn_unit_t(const AttnParams& p, const AttnParam
         wgmma_wait<0>();
         wgmma_fence_regs(sacc);
         // thread rows: h = 0 / 1 -> row 16 wq + lane / 4 + 8 h of this warpgroup; key of register j: 8 (j / 4) + 2 (lane % 4) + j % 2
-        int rows[2], segs[2];
+        // Block-diagonal mask: key and row are in the same image iff key / HW == row / HW, i.e. 0 <= key - HW (row / HW) < HW.  With the
+        // lane's part of the key folded into seg0, that is one unsigned compare of a constant per register instead of a division.  A
+        // masked logit becomes -inf: the row maximum skips it and its exponential is exactly 0, as a masked P must be.
+        int rows[2], seg0[2];
         float mx[2] = {-3.0e38f, -3.0e38f}, sum[2] = {0.f, 0.f};
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             rows[h] = 64 * g + 16 * wq + (lane >> 2) + 8 * h;
-            segs[h] = (qt * 128 + rows[h]) / p.HW;         // image inside the batch (block-diagonal mask)
+            seg0[h] = (qt * 128 + rows[h]) / p.HW * p.HW - 2 * (lane & 3);   // first key of the row's image, less the lane's key offset
         }
+        auto same_image = [&](int jkey, int h) { return static_cast<unsigned>(jkey - seg0[h]) < static_cast<unsigned>(p.HW); };
 #pragma unroll
         for (int j = 0; j < LT / 2; ++j) {
-            const int h = (j >> 1) & 1, key = 8 * (j >> 2) + 2 * (lane & 3) + (j & 1);
-            if (key / p.HW == segs[h]) mx[h] = fmaxf(mx[h], sacc[j]);
+            const int h = (j >> 1) & 1;
+            if (!same_image(8 * (j >> 2) + (j & 1), h)) sacc[j] = -INFINITY;
+            mx[h] = fmaxf(mx[h], sacc[j]);
         }
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
@@ -134,8 +158,7 @@ __device__ __forceinline__ void attn_unit_t(const AttnParams& p, const AttnParam
 #pragma unroll
         for (int j = 0; j < LT / 2; j += 2) {
             const int h = (j >> 1) & 1, key = 8 * (j >> 2) + 2 * (lane & 3);
-            const float x0 = exp2f(fmaf(sacc[j], p.scale_log2e, -mxs[h])), x1 = exp2f(fmaf(sacc[j + 1], p.scale_log2e, -mxs[h]));
-            const float e0 = (key / p.HW == segs[h]) ? x0 : 0.f, e1 = ((key + 1) / p.HW == segs[h]) ? x1 : 0.f;
+            const float e0 = exp2f(fmaf(sacc[j], p.scale_log2e, -mxs[h])), e1 = exp2f(fmaf(sacc[j + 1], p.scale_log2e, -mxs[h]));
             sum[h] += e0 + e1;
             // K chunk of 64 keys = 128 B per row; 16-byte units XOR-swizzled with the row (128B swizzle)
             const int r = rows[h];
@@ -174,26 +197,6 @@ __device__ __forceinline__ void attn_unit_t(const AttnParams& p, const AttnParam
             *reinterpret_cast<__nv_bfloat162*>(o) = __floats2bfloat162_rn(oacc[j] * inv[h], oacc[j + 1] * inv[h]);
         }
     }
-    __syncthreads();
-}
-
-__device__ __forceinline__ void attn_unit(const AttnParams& p, const AttnParams* pm, const uint32_t base, uint8_t* base_ptr, const int qt,
-                                          const int dc, const int z) {
-    if (p.Lt == 256) {
-        if (p.dn == 256) attn_unit_t<256, 256>(p, pm, base, base_ptr, qt, dc, z);
-        else attn_unit_t<256, 128>(p, pm, base, base_ptr, qt, dc, z);
-    } else {
-        if (p.dn == 256) attn_unit_t<128, 256>(p, pm, base, base_ptr, qt, dc, z);
-        else attn_unit_t<128, 128>(p, pm, base, base_ptr, qt, dc, z);
-    }
-}
-
-__global__ void __launch_bounds__(ATTN_THREADS, 1) attn_kernel(const __grid_constant__ AttnParams p) {
-    extern __shared__ uint8_t smem_raw[];
-    const uint32_t raw = smem_u32(smem_raw);
-    const uint32_t base = (raw + 1023u) & ~1023u;
-    const int n_dc = p.C / p.dn;
-    attn_unit(p, &p, base, smem_raw + (base - raw), blockIdx.x / n_dc, blockIdx.x % n_dc, blockIdx.y);
 }
 
 }  // namespace sr3

@@ -478,11 +478,39 @@ Op make_gemm_op(const GemmDesc& d, DevAllocs& mem, sr3_gemm_geometry* geo = null
 // running maximum (attn_long_wgmma.cuh), and an attention batch is then always one image.
 bool attn_fusable(int Lt, int C) { return Lt >= 128 && Lt % 128 == 0 && C % 128 == 0 && C >= 128; }
 
-Op make_attn_op(const bf16* qk, const bf16* vT, bf16* out, int nz, int Lt, int HW, int C) {
+// Output channels per CTA of attn_kernel.  Each CTA needs ATTN_SMEM_BYTES (about 211 KB), so one fits per SM and a launch of more CTAs
+// than SMs runs in whole extra waves, each as long as one CTA.  A CTA recomputes S for its 128 query rows whatever its slice, so a
+// narrower slice only shortens its P v part: take the fewest waves, and among equal waves the narrowest slice (the most SMs busy).
+int attn_pick_dn(int nz, int Lt, int C, int sms) {
+    int best = 0;
+    long long best_waves = 0;
+    for (int dn : {256, 128, 64}) {
+        if (C % dn != 0) continue;
+        const long long ctas = (long long)(Lt / 128) * (C / dn) * nz;
+        const long long waves = (ctas + sms - 1) / sms;
+        if (best == 0 || waves <= best_waves) { best = dn; best_waves = waves; }
+    }
+    return best;
+}
+
+template <int LT, int DN>
+Op attn_op_t(const AttnParams& p, dim3 grid) {
+    static std::vector<int> seen;
+    if (first_use_on_device(seen)) CK(cudaFuncSetAttribute(attn_kernel<LT, DN>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATTN_SMEM_BYTES));
+    return [p, grid](cudaStream_t st) { launch_k(attn_kernel<LT, DN>, grid, dim3(ATTN_THREADS), ATTN_SMEM_BYTES, st, p); };
+}
+
+// dn = 0: attn_pick_dn; otherwise 64, 128 or 256 (up to 256 keys; test and timing hooks).
+Op make_attn_op(const bf16* qk, const bf16* vT, bf16* out, int nz, int Lt, int HW, int C, int dn = 0) {
     REQUIRE(attn_fusable(Lt, C) && Lt % HW == 0, "attention shape Lt=%d HW=%d C=%d is not supported by the fused kernel", Lt, HW, C);
     REQUIRE(Lt <= 256 || HW == Lt, "attention over %d tokens per batch takes one image per batch (HW=%d)", Lt, HW);
+    REQUIRE(dn == 0 || (Lt <= 256 && (dn == 64 || dn == 128 || dn == 256) && C % dn == 0),
+            "attention channel slice dn=%d is not supported for Lt=%d C=%d", dn, Lt, C);
     AttnParams p;
     memset(&p, 0, sizeof(p));
+    p.out = out; p.C = C; p.Lt = Lt; p.HW = HW; p.nz = nz;
+    p.dn = Lt > 256 ? ATTNL_DN : dn ? dn : attn_pick_dn(nz, Lt, C, num_sms());
+    p.scale_log2e = 1.4426950408889634f / sqrtf((float)C);
     {
         const uint64_t dims[2] = {(uint64_t)2 * C, (uint64_t)nz * Lt};
         const uint64_t str[1] = {(uint64_t)2 * C * 2};
@@ -492,23 +520,23 @@ Op make_attn_op(const bf16* qk, const bf16* vT, bf16* out, int nz, int Lt, int H
     {
         const uint64_t dims[2] = {(uint64_t)Lt, (uint64_t)nz * C};
         const uint64_t str[1] = {(uint64_t)Lt * 2};
-        const uint32_t box[2] = {64u, 128u};
+        const uint32_t box[2] = {64u, (uint32_t)(p.dn < 128 ? p.dn : 128)};
         p.vt_map = encode_map(2, vT, dims, str, box);
     }
-    p.out = out; p.C = C; p.Lt = Lt; p.HW = HW; p.nz = nz;
-    p.dn = (C % 256 == 0) ? 256 : 128;
-    p.scale_log2e = 1.4426950408889634f / sqrtf((float)C);
+    const dim3 grid((Lt / 128) * (C / p.dn), nz, 1);
     if (Lt > 256) {
-        p.dn = ATTNL_DN;
         static std::vector<int> seen_long;
         if (first_use_on_device(seen_long)) CK(cudaFuncSetAttribute(attn_long_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ATTNL_SMEM_BYTES));
-        const dim3 grid((Lt / 128) * (C / ATTNL_DN), nz, 1);
-        return [p, grid](cudaStream_t st) { launch_k(attn_long_kernel, grid, dim3(ATTN_THREADS), ATTNL_SMEM_BYTES, st, p); };
+        return [p, grid](cudaStream_t st) { launch_k(attn_long_kernel, grid, dim3(ATTNL_THREADS), ATTNL_SMEM_BYTES, st, p); };
     }
-    static std::vector<int> seen;
-    if (first_use_on_device(seen)) CK(cudaFuncSetAttribute(attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ATTN_SMEM_BYTES));
-    const dim3 grid((Lt / 128) * (C / p.dn), nz, 1);
-    return [p, grid](cudaStream_t st) { launch_k(attn_kernel, grid, dim3(ATTN_THREADS), ATTN_SMEM_BYTES, st, p); };
+    if (Lt == 256) {
+        if (p.dn == 256) return attn_op_t<256, 256>(p, grid);
+        if (p.dn == 128) return attn_op_t<256, 128>(p, grid);
+        return attn_op_t<256, 64>(p, grid);
+    }
+    if (p.dn == 256) return attn_op_t<128, 256>(p, grid);
+    if (p.dn == 128) return attn_op_t<128, 128>(p, grid);
+    return attn_op_t<128, 64>(p, grid);
 }
 
 void pick_image_box(int W, int H, int& w_box, int& h_box, int& b_box);
@@ -2867,6 +2895,51 @@ int sr3_test_attention(const void* qk, const void* vT, void* out, int nz, int Lt
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     op(st);
     CK(cudaStreamSynchronize(st));
+    API_END
+}
+
+int sr3_test_attention_dn(const void* qk, const void* vT, void* out, int nz, int Lt, int HW, int C, int dn, void* stream) {
+    API_BEGIN
+    Op op = make_attn_op(static_cast<const bf16*>(qk), static_cast<const bf16*>(vT), static_cast<bf16*>(out), nz, Lt, HW, C, dn);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    op(st);
+    CK(cudaStreamSynchronize(st));
+    API_END
+}
+
+int sr3_attention_dn(int nz, int Lt, int C, int sms, int* dn_out) {
+    API_BEGIN
+    REQUIRE(dn_out && nz > 0 && attn_fusable(Lt, C), "bad arguments");
+    *dn_out = Lt > 256 ? ATTNL_DN : attn_pick_dn(nz, Lt, C, sms > 0 ? sms : num_sms());
+    API_END
+}
+
+int sr3_bench_attention(const void* qk, const void* vT, void* out, int nz, int Lt, int HW, int C, int dn, int reps, float* ms_out) {
+    API_BEGIN
+    REQUIRE(ms_out && reps > 0, "bad arguments");
+    Op op = make_attn_op(static_cast<const bf16*>(qk), static_cast<const bf16*>(vT), static_cast<bf16*>(out), nz, Lt, HW, C, dn);
+    // timed as ONE captured graph of `reps` launches, as inside the step graph (see sr3_bench_conv)
+    cudaStream_t cs;
+    CK(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
+    for (int i = 0; i < 3; ++i) op(cs);
+    CK(cudaStreamSynchronize(cs));
+    cudaGraph_t g; cudaGraphExec_t ge;
+    CK(cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal));
+    for (int i = 0; i < reps; ++i) op(cs);
+    CK(cudaStreamEndCapture(cs, &g));
+    CK(cudaGraphInstantiate(&ge, g, 0));
+    CK(cudaGraphLaunch(ge, cs));
+    CK(cudaStreamSynchronize(cs));
+    cudaEvent_t e0, e1;
+    CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
+    CK(cudaEventRecord(e0, cs));
+    CK(cudaGraphLaunch(ge, cs));
+    CK(cudaEventRecord(e1, cs));
+    CK(cudaEventSynchronize(e1));
+    float ms = 0; CK(cudaEventElapsedTime(&ms, e0, e1));
+    cudaGraphExecDestroy(ge); cudaGraphDestroy(g); cudaStreamDestroy(cs);
+    cudaEventDestroy(e0); cudaEventDestroy(e1);
+    *ms_out = ms / reps;
     API_END
 }
 

@@ -330,6 +330,12 @@ int sr3_test_gemm(const void* a_bf16, const void* b_bf16, float* d, int M, int N
  * (q | k), vT bf16 [nz*C][Lt], out bf16 [nz*Lt][C]; Lt keys per attention batch (a multiple of 128), HW tokens per image (Lt % HW == 0; above 256 keys
  * HW == Lt and the streaming-softmax kernel runs). */
 int sr3_test_attention(const void* qk_bf16, const void* vT_bf16, void* out_bf16, int nz, int Lt, int HW, int C, void* stream);
+/* sr3_test_attention with attn_kernel's channel slice forced: dn = 64, 128 or 256 output channels per CTA (Lt <= 256, C % dn == 0), or
+ * 0 for the one make_attn_op picks.  Any dn computes the same bits. */
+int sr3_test_attention_dn(const void* qk_bf16, const void* vT_bf16, void* out_bf16, int nz, int Lt, int HW, int C, int dn, void* stream);
+/* The channel slice the fused attention core runs at for nz attention batches of Lt keys and C channels on a GPU of `sms` SMs
+ * (sms <= 0: the current device's): the fewest waves of one CTA per SM, then the narrowest slice. */
+int sr3_attention_dn(int nz, int Lt, int C, int sms, int* dn);
 /* Test hook for the unfused attention path (precise mode, training), the plan's three launches:
  * S = q k^T / sqrt(C) on the tile kernel, softmax_kernel over the keys of each image, O = P v on the tile kernel.  qk bf16 [nz*Lt][2C PW]
  * (rows [q | k], precise = 1: [q_hi | k_hi | q_lo | k_lo]), vT bf16 [nz*C][Lt PW] -> S fp32 [nz*Lt][Lt], P bf16 [nz*Lt][Lt PW],
@@ -452,6 +458,9 @@ int sr3_test_input_grad(const void* dy_bf16, const float* w_oihw, float* dx, int
 
 /* Timing harness for one conv shape on zero-filled buffers (kernel-tuning experiments): average ms over `reps` launches. */
 int sr3_bench_conv(int B, int H, int W, int Cin, int Cout, int ksize, int stride, int with_resid, int with_stats, int reps, float* ms_out);
+/* Timing harness for the fused attention core (operands as sr3_test_attention, dn as sr3_test_attention_dn): average ms over `reps`
+ * launches captured in one graph; out holds the result. */
+int sr3_bench_attention(const void* qk_bf16, const void* vT_bf16, void* out_bf16, int nz, int Lt, int HW, int C, int dn, int reps, float* ms_out);
 
 #ifdef __cplusplus
 }
