@@ -103,6 +103,9 @@ _SIGS = {
     "sr3_wstream_create": (c_int, [c_void_p, c_uint64, c_int, c_int, POINTER(c_void_p)]),
     "sr3_wstream_destroy": (None, [c_void_p]),
     "sr3_wstream_admit": (c_int, [c_void_p, POINTER(c_int), c_int, c_void_p, c_void_p, c_int, c_int, c_uint64, POINTER(c_int), c_void_p]),
+    "sr3_wstream_add_schedule": (c_int, [c_void_p, c_int] + [c_void_p] * 6 + [POINTER(c_int), c_void_p]),
+    "sr3_wstream_admit_scheduled": (c_int, [c_void_p, POINTER(c_int), c_int, c_void_p, c_void_p, c_int, c_int, c_uint64, c_int, POINTER(c_int),
+                                            c_void_p]),
     "sr3_wstream_step": (c_int, [c_void_p, c_void_p]),
     "sr3_wstream_retire": (c_int, [c_void_p, c_int, c_void_p]),
     "sr3_wstream_slot_state": (c_int, [c_void_p, POINTER(c_int), POINTER(c_int), POINTER(c_int)]),
@@ -308,13 +311,7 @@ class Engine:
             torch.cuda.current_stream().synchronize()
 
     def set_schedule(self, bufs: dict, sqrt_alphas_cumprod_prev):
-        import numpy as np
-        T = int(bufs["betas"].shape[0])
-        host = [bufs[k].detach().to("cpu", torch.float32).contiguous() for k in
-                ("sqrt_recip_alphas_cumprod", "sqrt_recipm1_alphas_cumprod", "posterior_mean_coef1", "posterior_mean_coef2",
-                 "posterior_log_variance_clipped")]
-        sp = np.ascontiguousarray(np.asarray(sqrt_alphas_cumprod_prev, dtype=np.float64))
-        assert sp.shape[0] == T + 1
+        T, host, sp = _schedule_host(bufs, sqrt_alphas_cumprod_prev)
         with torch.cuda.device(self.device):
             _check(lib().sr3_engine_set_schedule(self._h, T, *[c_void_p(h.data_ptr()) for h in host], c_void_p(sp.ctypes.data), _stream()))
         self.T = T
@@ -755,6 +752,22 @@ class WindowedSampler:
         return {"gather": ms[0], "engine": ms[1], "merge": ms[2]}
 
 
+MAX_TIMESTEPS = 4096     # the largest n_timestep an engine's schedule tables hold (sr3_engine T_cap)
+
+
+def _schedule_host(bufs: dict, sqrt_alphas_cumprod_prev):
+    """(T, the five fp32 host tables, fp64 sqrt_alphas_cumprod_prev) of a schedule's buffers, the arguments of sr3_engine_set_schedule and
+    sr3_wstream_add_schedule."""
+    import numpy as np
+    T = int(bufs["betas"].shape[0])
+    host = [bufs[k].detach().to("cpu", torch.float32).contiguous() for k in
+            ("sqrt_recip_alphas_cumprod", "sqrt_recipm1_alphas_cumprod", "posterior_mean_coef1", "posterior_mean_coef2",
+             "posterior_log_variance_clipped")]
+    sp = np.ascontiguousarray(np.asarray(sqrt_alphas_cumprod_prev, dtype=np.float64))
+    assert sp.shape[0] == T + 1
+    return T, host, sp
+
+
 def stream_plan(arrival_steps, slots, T):
     """The slot plan of continuous batching: for request n arriving before step arrival_steps[n] (non-decreasing; any iterable, read
     lazily, one value per request planned), yields (slot, admit_step, finish_step).  Requests are admitted first come first served, each
@@ -767,30 +780,33 @@ def stream_plan(arrival_steps, slots, T):
 
 
 def windowed_stream_plan(requests, slots, T):
-    """The slot plan of continuous batching when a request takes several slots: for request n = (arrival_step, n_windows) (arrival steps
-    non-decreasing; any iterable, read lazily, one value per request planned), yields (slot_list, admit_step, finish_step).  First come
-    first served with head-of-line blocking: a request is admitted at the first step at which it has arrived, every earlier request has
-    been admitted and n_windows slots are free -- a later, smaller request never overtakes it -- into the n_windows lowest free slots; it
-    runs T steps and its slots are free again from finish_step = admit_step + T on.  Pure host arithmetic:
+    """The slot plan of continuous batching when a request takes several slots: for request n = (arrival_step, n_windows) or
+    (arrival_step, n_windows, steps) (arrival steps non-decreasing; any iterable, read lazily, one value per request planned), yields
+    (slot_list, admit_step, finish_step).  First come first served with head-of-line blocking: a request is admitted at the first step at
+    which it has arrived, every earlier request has been admitted and n_windows slots are free -- a later, smaller request never overtakes
+    it -- into the n_windows lowest free slots; it runs `steps` steps (default T: a request on a schedule of its own runs that schedule's
+    n_timestep) and its slots are free again from finish_step = admit_step + steps on.  Pure host arithmetic:
     GaussianDiffusion.super_resolution_windowed_stream follows it step for step."""
     slots, T = int(slots), int(T)
     if slots < 1 or T < 1:
         raise ValueError("stream plans need slots >= 1 and T >= 1, got slots=%d T=%d" % (slots, T))
     free_at = [0] * slots                   # the step from which each slot is free
     last_arrival, last_admit = 0, 0
-    for a, n in requests:
-        a, n = int(a), int(n)
+    for req in requests:
+        a, n, steps = (tuple(int(v) for v in req) + (T,))[:3]
         if a < last_arrival:
             raise ValueError("arrival steps must be non-decreasing: %d after %d" % (a, last_arrival))
         if not 1 <= n <= slots:
             raise ValueError("a request of %d windows cannot run on %d slots" % (n, slots))
+        if steps < 1:
+            raise ValueError("a request of %d steps cannot run: steps must be >= 1" % steps)
         last_arrival = a
         k = max(a, last_admit, sorted(free_at)[n - 1])     # the first step at which n slots are free
         taken = [s for s in range(slots) if free_at[s] <= k][:n]
         for s in taken:
-            free_at[s] = k + T
+            free_at[s] = k + steps
         last_admit = k
-        yield taken, k, k + T
+        yield taken, k, k + steps
 
 
 class WindowedStreamSampler:
@@ -799,7 +815,8 @@ class WindowedStreamSampler:
     The online interface: a server calls admit() with free slots, step() once per reverse step and retire() for every request finished()
     lists.  This object owns each request's canvas (x_t, and a copy of the condition) until retire(), which returns x_0; the native side
     borrows them, so admission allocates nothing on the device.  Borrows the engine (and keeps it alive); nothing else may run on it while
-    requests are in flight."""
+    requests are in flight.  A request samples on the engine's noise schedule, or on one registered with add_schedule (requests on
+    different schedules share the batch)."""
 
     def __init__(self, engine, seed, overlap_h, overlap_w):
         self.engine = engine
@@ -824,9 +841,20 @@ class WindowedStreamSampler:
         """The number of windows (= slots) of a height x width canvas."""
         return len(window_grid(height, self.engine.height, self.overlap[0])) * len(window_grid(width, self.engine.width, self.overlap[1]))
 
-    def admit(self, slots, condition_x, x_T, sample_index):
+    def add_schedule(self, bufs: dict, sqrt_alphas_cumprod_prev):
+        """Register a noise schedule (Engine.set_schedule's arguments: GaussianDiffusion's buffers, see
+        diffusion.noise_schedule_buffers) for requests of this stream; returns its id for admit(schedule=...).  Allowed while requests run."""
+        T, host, sp = _schedule_host(bufs, sqrt_alphas_cumprod_prev)
+        sid = c_int()
+        with torch.cuda.device(self.device):
+            _check(lib().sr3_wstream_add_schedule(self._h, T, *[c_void_p(h.data_ptr()) for h in host], c_void_p(sp.ctypes.data),
+                                                  ctypes.byref(sid), _stream()))
+        return sid.value
+
+    def admit(self, slots, condition_x, x_T, sample_index, schedule=None):
         """Admit a request ([C_cond, H, W] condition, None for an unconditional model, and [C, H, W] x_T) into the free `slots`, one per
-        window of its grid (row-major); its Philox draws are keyed by the global `sample_index`.  Returns the request's id."""
+        window of its grid (row-major); its Philox draws are keyed by the global `sample_index`.  `schedule`: an id from add_schedule, or
+        None for the engine's schedule; the request starts at t = n_timestep - 1 of it.  Returns the request's id."""
         cond_c = self.engine.in_channel - self.engine.channels
         if condition_x is not None and (condition_x.dim() != 3 or condition_x.shape[0] != cond_c):
             raise ValueError("condition_x must be [%d, H, W], got %s" % (cond_c, tuple(condition_x.shape)))
@@ -838,8 +866,9 @@ class WindowedStreamSampler:
         sl = [int(s) for s in slots]
         rid = c_int()
         with torch.cuda.device(self.device):
-            _check(lib().sr3_wstream_admit(self._h, (c_int * max(len(sl), 1))(*sl), len(sl), _ptr(cond), _ptr(x), hw[0], hw[1],
-                                           int(sample_index), ctypes.byref(rid), _stream()))
+            _check(lib().sr3_wstream_admit_scheduled(self._h, (c_int * max(len(sl), 1))(*sl), len(sl), _ptr(cond), _ptr(x), hw[0], hw[1],
+                                                     int(sample_index), -1 if schedule is None else int(schedule), ctypes.byref(rid),
+                                                     _stream()))
         self._canvases[rid.value] = (x, cond)
         return rid.value
 

@@ -2057,11 +2057,28 @@ struct sr3_windowed {
     }
 };
 
+// ------------------------------------------------------------------------------------------------ noise schedule tables
+// The device form of a noise schedule of T steps, shared by sr3_engine_set_schedule and sr3_wstream_add_schedule so that both read
+// identical values: tab [5][stride] (stride >= T; rows sqrt_recip_alphas_cumprod, sqrt_recipm1_alphas_cumprod, posterior_mean_coef1,
+// posterior_mean_coef2, posterior_log_variance_clipped; entries T .. stride - 1 zero) and nl [T + 1] = fp32(sqrt_alphas_cumprod_prev), the
+// FloatTensor([f64]) rounding of diffusion.py:153.  Synchronises `st`: the host staging is gone when it returns.
+static void upload_schedule(int T, int stride, const float* a, const float* b, const float* c1, const float* c2, const float* lv,
+                            const double* sqrt_ac_prev, float* tab_dev, float* nl_dev, cudaStream_t st) {
+    std::vector<float> tab((size_t)5 * stride, 0.f), nl(T + 1);
+    const float* srcs[5] = {a, b, c1, c2, lv};
+    for (int k = 0; k < 5; ++k) memcpy(tab.data() + (size_t)k * stride, srcs[k], T * sizeof(float));
+    for (int i = 0; i <= T; ++i) nl[i] = static_cast<float>(sqrt_ac_prev[i]);
+    CK(cudaMemcpyAsync(tab_dev, tab.data(), tab.size() * 4, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(nl_dev, nl.data(), nl.size() * 4, cudaMemcpyHostToDevice, st));
+    CK(cudaStreamSynchronize(st));
+}
+
 // ------------------------------------------------------------------------------------------------ continuous batching of windowed canvases
 // The engine's B images are slots, one window each; a request is a canvas of any size whose ny x nx windows take as many slots and run at
 // the request's own timestep.  The caller owns each canvas (x_t, condition); the stream holds up to B request records, their window
 // geometry, the slot table and a means arena.  A step: wstream_gather_kernel -> the engine's step graph (UNet.forward form) ->
-// wstream_means_kernel -> wstream_merge_kernel.
+// wstream_means_kernel -> wstream_merge_kernel.  A request samples on the engine's schedule or on one registered with add_schedule; its
+// record carries that schedule's table pointers.
 struct sr3_wstream {
     sr3_engine* e = nullptr;               // borrowed
     uint64_t seed = 0;
@@ -2076,10 +2093,13 @@ struct sr3_wstream {
     std::vector<WStreamReq> host;          // exact mirror of the half the next step reads
     std::vector<char> held;                // the record holds a request: running (host[r].active) or finished and not yet retired
     std::vector<WStreamSlot> slots;        // mirror of slot_dev
-    int schedule_gen = 0;                  // e->schedule_gen when the requests in flight were admitted
+    int schedule_gen = 0;                  // e->schedule_gen when the requests in flight on the engine's schedule were admitted
+    struct Schedule { int T; float* tab; float* nl; };
+    std::vector<Schedule> schedules;       // registered schedules: device tab [5][T], nl [T + 1], allocated in mem
+    std::vector<int> sched_of;             // per record: the registered schedule its request samples on, -1: the engine's
 
-    bool any_running() const {
-        for (const WStreamReq& r : host) if (r.active) return true;
+    bool any_running_on_engine_schedule() const {
+        for (size_t r = 0; r < host.size(); ++r) if (host[r].active && sched_of[r] < 0) return true;
         return false;
     }
     void init(sr3_engine* eng, uint64_t sd, int ovh, int ovw) {
@@ -2088,8 +2108,9 @@ struct sr3_wstream {
         REQUIRE(ovh >= 0 && ovh < e->H && ovw >= 0 && ovw < e->W, "overlap %dx%d must be at least 0 and below the window %dx%d", ovh, ovw, e->H, e->W);
         CK(cudaSetDevice(e->dev));
         const int B = e->B;
-        host.assign(B, WStreamReq{-1, 0, 0ull, nullptr, nullptr, 0, 0, 0, 0});
+        host.assign(B, WStreamReq{-1, 0, 0ull, nullptr, nullptr, 0, 0, 0, 0, nullptr, nullptr, 0});
         held.assign(B, 0);
+        sched_of.assign(B, -1);
         slots.assign(B, WStreamSlot{-1, 0, 0});
         reqs = static_cast<WStreamReq*>(mem.alloc(2 * B * sizeof(WStreamReq)));
         slot_dev = static_cast<WStreamSlot*>(mem.alloc(B * sizeof(WStreamSlot)));
@@ -2106,14 +2127,26 @@ struct sr3_wstream {
         CK(cudaMemset(e->in_buf, 0, (size_t)B * e->H * e->W * e->in_C * e->PW * sizeof(bf16)));
         CK(cudaMemset(e->nl_buf, 0, B * sizeof(float)));
     }
+    // A request on a registered schedule is immune to sr3_engine_set_schedule; one on the engine's schedule is not.
     void check_schedule() const {
         REQUIRE(e->T > 0, "no noise schedule: call sr3_engine_set_schedule first");
-        REQUIRE(!any_running() || schedule_gen == e->schedule_gen,
+        REQUIRE(!any_running_on_engine_schedule() || schedule_gen == e->schedule_gen,
                 "the noise schedule changed while requests are in flight; they cannot finish on a mixed schedule");
     }
-    int admit(const int* sl, int n, const float* cond, float* x, int H, int W, uint64_t sample, cudaStream_t st) {
+    int add_schedule(int T, const float* a, const float* b, const float* c1, const float* c2, const float* lv, const double* sqrt_ac_prev,
+                     cudaStream_t st) {
+        REQUIRE(a && b && c1 && c2 && lv && sqrt_ac_prev, "null schedule table");
+        REQUIRE(T >= 1 && T <= e->T_cap, "n_timestep %d out of range (max %d)", T, e->T_cap);
+        CK(cudaSetDevice(e->dev));
+        Schedule sc{T, static_cast<float*>(mem.alloc((size_t)5 * T * 4, false)), static_cast<float*>(mem.alloc((size_t)(T + 1) * 4, false))};
+        upload_schedule(T, T, a, b, c1, c2, lv, sqrt_ac_prev, sc.tab, sc.nl, st);
+        schedules.push_back(sc);
+        return (int)schedules.size() - 1;
+    }
+    int admit(const int* sl, int n, const float* cond, float* x, int H, int W, uint64_t sample, int schedule, cudaStream_t st) {
         const int B = e->B, wh = e->H, ww = e->W;
         check_schedule();
+        REQUIRE(schedule >= -1 && schedule < (int)schedules.size(), "unknown schedule %d (%d registered)", schedule, (int)schedules.size());
         REQUIRE(x != nullptr, "null canvas");
         if (e->cfg.conditional) REQUIRE(cond != nullptr, "condition_x is required by a conditional model");
         else REQUIRE(cond == nullptr, "condition_x given to an unconditional model");
@@ -2131,7 +2164,7 @@ struct sr3_wstream {
         int r = 0;
         while (held[r]) ++r;                   // a free slot exists, so fewer than B requests are held
         CK(cudaSetDevice(e->dev));
-        if (!any_running()) schedule_gen = e->schedule_gen;
+        if (schedule < 0 && !any_running_on_engine_schedule()) schedule_gen = e->schedule_gen;
         const std::vector<float> gy = window_weights(ny, wh, overlap_h), gx = window_weights(nx, ww, overlap_w);
         CK(cudaMemcpyAsync(oy + r * B, ry.data(), ny * sizeof(int), cudaMemcpyHostToDevice, st));
         CK(cudaMemcpyAsync(ox + r * B, rx.data(), nx * sizeof(int), cudaMemcpyHostToDevice, st));
@@ -2140,8 +2173,13 @@ struct sr3_wstream {
         CK(cudaMemcpyAsync(slot_of + r * B, sl, n * sizeof(int), cudaMemcpyHostToDevice, st));
         for (int k = 0; k < n; ++k) slots[sl[k]] = WStreamSlot{r, k / nx, k % nx};
         CK(cudaMemcpyAsync(slot_dev, slots.data(), B * sizeof(WStreamSlot), cudaMemcpyHostToDevice, st));
-        host[r] = WStreamReq{e->T - 1, 1, (unsigned long long)sample, x, cond, H, W, ny, nx};
+        if (schedule < 0) host[r] = WStreamReq{e->T - 1, 1, (unsigned long long)sample, x, cond, H, W, ny, nx, e->post_tab, e->nl_table, e->T_cap};
+        else {
+            const Schedule& sc = schedules[schedule];
+            host[r] = WStreamReq{sc.T - 1, 1, (unsigned long long)sample, x, cond, H, W, ny, nx, sc.tab, sc.nl, sc.T};
+        }
         held[r] = 1;
+        sched_of[r] = schedule;
         CK(cudaMemcpyAsync(reqs + cur * B + r, &host[r], sizeof(WStreamReq), cudaMemcpyHostToDevice, st));
         return r;
     }
@@ -2157,7 +2195,7 @@ struct sr3_wstream {
         p.B = e->B; p.C = e->cfg.channels; p.cond_c = e->cond_c; p.wh = e->H; p.ww = e->W;
         p.in_buf = e->in_buf; p.in_ld = e->in_C * e->PW; p.lo_off = e->precise ? e->in_C : 0;
         p.x_state = e->x_state; p.eps = e->eps_buf; p.means = means;
-        p.tab = e->post_tab; p.tab_T = e->T_cap; p.nl_table = e->nl_table; p.nl_buf = e->nl_buf; p.seed = seed;
+        p.nl_buf = e->nl_buf; p.seed = seed;
         const long long total = 1LL * e->B * e->H * e->W;
         const dim3 grid((int)std::min<long long>((total + 255) / 256, num_sms() * 8LL));
         launch_k(wstream_gather_kernel, grid, dim3(256), 0, st, p);
@@ -2443,14 +2481,8 @@ int sr3_engine_set_schedule(sr3_engine* e, int T, const float* a, const float* b
     CK(cudaSetDevice(e->dev));
     e->T = T;
     ++e->schedule_gen;
-    std::vector<float> tab((size_t)5 * e->T_cap, 0.f), nl(T + 1);
-    const float* srcs[5] = {a, b, c1, c2, lv};
-    for (int k = 0; k < 5; ++k) memcpy(tab.data() + (size_t)k * e->T_cap, srcs[k], T * sizeof(float));
-    for (int i = 0; i <= T; ++i) nl[i] = static_cast<float>(sqrt_ac_prev[i]);     // FloatTensor([f64]) rounding, diffusion.py:153
     e->logvar_host.assign(lv, lv + T);
-    CK(cudaMemcpyAsync(e->post_tab, tab.data(), tab.size() * 4, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(e->nl_table, nl.data(), nl.size() * 4, cudaMemcpyHostToDevice, st));
-    CK(cudaStreamSynchronize(st));
+    upload_schedule(T, e->T_cap, a, b, c1, c2, lv, sqrt_ac_prev, e->post_tab, e->nl_table, st);
     API_END
 }
 
@@ -2708,12 +2740,24 @@ int sr3_wstream_create(sr3_engine* e, uint64_t seed, int overlap_h, int overlap_
     API_END
 }
 void sr3_wstream_destroy(sr3_wstream* s) { delete s; }
-int sr3_wstream_admit(sr3_wstream* s, const int* slots, int n_slots, const float* condition_x, float* x, int height, int width,
-                      uint64_t sample_index, int* request, void* stream) {
+int sr3_wstream_add_schedule(sr3_wstream* s, int T, const float* sqrt_recip_ac, const float* sqrt_recipm1_ac, const float* post_coef1,
+                             const float* post_coef2, const float* post_logvar, const double* sqrt_ac_prev, int* schedule, void* stream) {
+    API_BEGIN
+    REQUIRE(s && schedule, "null argument");
+    *schedule = s->add_schedule(T, sqrt_recip_ac, sqrt_recipm1_ac, post_coef1, post_coef2, post_logvar, sqrt_ac_prev,
+                                static_cast<cudaStream_t>(stream));
+    API_END
+}
+int sr3_wstream_admit_scheduled(sr3_wstream* s, const int* slots, int n_slots, const float* condition_x, float* x, int height, int width,
+                                uint64_t sample_index, int schedule, int* request, void* stream) {
     API_BEGIN
     REQUIRE(s && request, "null argument");
-    *request = s->admit(slots, n_slots, condition_x, x, height, width, sample_index, static_cast<cudaStream_t>(stream));
+    *request = s->admit(slots, n_slots, condition_x, x, height, width, sample_index, schedule, static_cast<cudaStream_t>(stream));
     API_END
+}
+int sr3_wstream_admit(sr3_wstream* s, const int* slots, int n_slots, const float* condition_x, float* x, int height, int width,
+                      uint64_t sample_index, int* request, void* stream) {
+    return sr3_wstream_admit_scheduled(s, slots, n_slots, condition_x, x, height, width, sample_index, -1, request, stream);
 }
 int sr3_wstream_step(sr3_wstream* s, void* stream) {
     API_BEGIN

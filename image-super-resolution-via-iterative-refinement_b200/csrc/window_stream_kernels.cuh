@@ -5,12 +5,15 @@
 //   wstream_gather_kernel  crops of each slot's canvas x_t and condition -> the engine's bf16 NHWC input and fp32 x_state; nl_buf per slot
 //   wstream_means_kernel   eps + x_t of every active slot -> its clipped posterior mean at its request's t (the means arena)
 //   wstream_merge_kernel   the window means blended per canvas pixel, + sigma_t * z -> the canvas x_{t-1}; advances the request table
+// Every request carries its own noise schedule (the engine's tables, or tables registered with sr3_wstream_add_schedule), so requests on
+// different schedules share the batch: the three kernels read the schedule of each slot's request, never one of the step.
 #pragma once
 #include "aux_kernels.cuh"
 
 namespace sr3 {
 
-// One request: a canvas the caller owns.  The host keeps an exact mirror: every request takes exactly T steps.
+// One request: a canvas the caller owns, and the schedule it samples on.  The host keeps an exact mirror: a request on a schedule of
+// T steps takes exactly T steps.
 struct WStreamReq {
     int t;                        // timestep of the request's next step while active; -1 once it has finished
     int active;                   // 1: the request's windows run
@@ -18,6 +21,9 @@ struct WStreamReq {
     float* x;                     // canvas x_t [C][H][W], overwritten with x_{t-1} every step (borrowed)
     const float* cond;            // canvas condition [cond_c][H][W] (borrowed)
     int H, W, ny, nx;             // canvas size and window grid
+    const float* tab;             // its schedule's [5][tab_T] table (sqrt_recip_ac, sqrt_recipm1_ac, post_coef1, post_coef2, post_logvar)
+    const float* nl_table;        // its schedule's fp32(sqrt_alphas_cumprod_prev) [T + 1]
+    int tab_T;                    // row stride of tab (>= the schedule's T)
 };
 
 // One slot: the window of a request it runs.  Written by the host only (admission and retirement).
@@ -41,23 +47,21 @@ struct WStreamStep {
     float* x_state;               // the engine's [B][C][wh][ww]: x_t of every slot's window
     const float* eps;             // the engine's eps_buf [B][C][wh][ww]
     float* means;                 // [B][C][wh][ww]
-    const float* tab;             // the engine's [5][tab_T] schedule table
-    int tab_T;
-    const float* nl_table;        // fp32(sqrt_alphas_cumprod_prev) [T + 1]
     float* nl_buf;                // [B]
     unsigned long long seed;
 };
 
 // One thread per (slot, window pixel), every channel.  An active slot gets its window's crop of the canvas (the values window_gather_kernel
 // writes for the same window: bf16 of x, and bf16 of x - bf16(x) in precise mode); an idle slot, or one whose request has finished, gets
-// zeros, so it never carries non-finite values.  Block 0 sets nl_buf[s] = nl_table[t + 1], the value the windowed sampler's step at t reads.
+// zeros, so it never carries non-finite values.  Block 0 sets nl_buf[s] = nl_table[t + 1] of the slot's request's schedule, the value the
+// windowed sampler's step at t reads after sr3_engine_set_schedule of that schedule.
 __global__ void __launch_bounds__(256) wstream_gather_kernel(const WStreamStep p) {
     pdl_launch_dependents();
     pdl_wait();
     if (blockIdx.x == 0) {
         for (int s = threadIdx.x; s < p.B; s += blockDim.x) {
             const int r = p.slots[s].req;
-            if (r >= 0 && p.cur[r].active) p.nl_buf[s] = p.nl_table[p.cur[r].t + 1];
+            if (r >= 0 && p.cur[r].active) p.nl_buf[s] = p.cur[r].nl_table[p.cur[r].t + 1];
         }
     }
     const int wplane = p.wh * p.ww;
@@ -96,7 +100,7 @@ __global__ void __launch_bounds__(256) wstream_gather_kernel(const WStreamStep p
 
 // One thread per (slot, window pixel), every channel: final_epilogue's (gemm_wgmma.cuh) clipped posterior mean, operation for operation
 // (the same separately rounded x0 = c1 x_t - c2 eps, clamp, mean = pc1 x0 + pc2 x_t), at the slot's request's own t.  This is the mean the
-// windowed sampler's engine writes for the same window.
+// windowed sampler's engine writes for the same window.  The coefficients are the request's schedule's.
 __global__ void __launch_bounds__(256) wstream_means_kernel(const WStreamStep p) {
     pdl_launch_dependents();
     pdl_wait();
@@ -108,7 +112,9 @@ __global__ void __launch_bounds__(256) wstream_means_kernel(const WStreamStep p)
         const int r = p.slots[s].req;
         if (r < 0 || !p.cur[r].active) continue;
         const int t = p.cur[r].t;
-        const float c1 = p.tab[t], c2 = p.tab[p.tab_T + t], pc1 = p.tab[2 * p.tab_T + t], pc2 = p.tab[3 * p.tab_T + t];
+        const float* tab = p.cur[r].tab;
+        const int tT = p.cur[r].tab_T;
+        const float c1 = tab[t], c2 = tab[tT + t], pc1 = tab[2 * tT + t], pc2 = tab[3 * tT + t];
         for (int c = 0; c < p.C; ++c) {
             const long long idx = (static_cast<long long>(s) * p.C + c) * wplane + wp;
             const float xt = p.x_state[idx];
@@ -123,7 +129,7 @@ __global__ void __launch_bounds__(256) wstream_means_kernel(const WStreamStep p)
 // its window OWNS p -- along each axis the window with the largest origin <= p, which covers p -- so every pixel of a running canvas is
 // written exactly once.  The covering windows are accumulated as window_merge_kernel does (ascending window index, separately rounded
 // products and sums, __fdiv_rn), with z keyed by (seed, the request's sample index, the pixel's index in its canvas, t): the windowed
-// sampler's x_{t-1} of image 0 bit for bit.  Block 0 advances the request table into `next`.
+// sampler's x_{t-1} of image 0 bit for bit; sigma_t is the request's schedule's.  Block 0 advances the request table into `next`.
 __global__ void __launch_bounds__(256) wstream_merge_kernel(const WStreamStep p) {
     pdl_launch_dependents();
     pdl_wait();
@@ -168,7 +174,7 @@ __global__ void __launch_bounds__(256) wstream_merge_kernel(const WStreamStep p)
             }
         }
         const int t = r->t;
-        const float sigma = posterior_sigma(p.tab, p.tab_T, t);
+        const float sigma = posterior_sigma(r->tab, r->tab_T, t);
         const long long plane = static_cast<long long>(r->H) * r->W;
         const long long pix = static_cast<long long>(y) * r->W + x;
         float z[4] = {0.f, 0.f, 0.f, 0.f};

@@ -238,34 +238,50 @@ int sr3_windowed_phase_merge(sr3_windowed* w, void* stream);
 /* ---- continuous batching: serve a stream of requests of ANY size (each at least the engine's H x W, the window) on one inference
  * engine, every request at its own timestep.  A request is a canvas whose ny x nx overlapping windows (the grid and fp32 blend weights of
  * sr3_windowed_*, with the stream's overlap) take ny * nx of the engine's B slots, one window each; all windows of a request run at the
- * request's own timestep, windows of different requests at different timesteps share the batch.  A request takes exactly T steps, one
- * per sr3_wstream_step, and then waits for sr3_wstream_retire.  A step is: a gather of every slot's window crop of its canvas (idle slots
- * get zeros), the engine's step graph in its UNet.forward form (noise level of slot s = sqrt_alphas_cumprod_prev[t + 1] of its request),
- * the clipped posterior mean of every running slot at its request's t, and a merge that blends the means on each canvas and adds sigma_t z
- * with z from Philox keyed by (seed, the request's sample_index, the pixel's index in its canvas, t), writing x_{t-1} into the canvas.
+ * request's own timestep, windows of different requests at different timesteps share the batch.  Every request samples on its own noise
+ * schedule: the engine's (sr3_engine_set_schedule), or one registered with sr3_wstream_add_schedule; requests on different schedules
+ * share the batch.  A request on a schedule of T steps takes exactly T steps, one per sr3_wstream_step, and then waits for
+ * sr3_wstream_retire.  A step is: a gather of every slot's window crop of its canvas (idle slots get zeros), the engine's step graph in its
+ * UNet.forward form (noise level of slot s = sqrt_alphas_cumprod_prev[t + 1] of its request's schedule), the clipped posterior mean of
+ * every running slot at its request's t, and a merge that blends the means on each canvas and adds sigma_t z with z from Philox keyed by
+ * (seed, the request's sample_index, the pixel's index in its canvas, t), writing x_{t-1} into the canvas.
  * Bit-exactness: a request's x_0 equals what sr3_windowed_* computes for that canvas alone as image 0 with first_sample_index =
- * sample_index on an engine of the same shape with its windows in the same slots, bit for bit, whatever the other slots hold and whenever
- * it was admitted (every UNet op is per image; the means and the merge are the windowed sampler's arithmetic operation for operation).
+ * sample_index on an engine of the same shape, after sr3_engine_set_schedule of the request's schedule, with its windows in the same slots,
+ * bit for bit, whatever the other slots hold and whenever it was admitted (every UNet op is per image; the means and the merge are the
+ * windowed sampler's arithmetic operation for operation, and both calls build the schedule's tables with the same host routine).
  * A window-sized request (one window, weight 1) in slot b equals what sr3_p_sample_loop computes for the same condition, x_T and
  * first_sample_index + b = sample_index at image b, bit for bit.  Whether the slots matter depends on the plan: on a 4x4-lowest-level
  * plan a window moved to another slot changes within rounding.
- * No step synchronises the host, copies to it or allocates: the host mirrors the request table, since every request takes exactly T steps.
+ * No step synchronises the host, copies to it or allocates: the host mirrors the request table, since every request takes exactly the
+ * T steps of its schedule.
  * The stream BORROWS the engine (which must outlive it; nothing else may run on it while requests are in flight, and all calls of one
  * stream go to one CUDA stream) and every admitted canvas until its request is retired.  Creating a stream zeroes the engine's state
  * and input.  Refused at creation: a training engine, an overlap outside [0, window side). */
 typedef struct sr3_wstream sr3_wstream;
 int sr3_wstream_create(sr3_engine* e, uint64_t seed, int overlap_h, int overlap_w, sr3_wstream** out);
 void sr3_wstream_destroy(sr3_wstream* s);
+/* Register a noise schedule of T steps for this stream's requests: the arrays, their meaning and the T range of sr3_engine_set_schedule
+ * (HOST, fp32 [T] each, sqrt_ac_prev fp64 [T + 1]).  *schedule = its id (0, 1, ... in registration order).  The device tables are allocated
+ * here, never in a step, and freed by sr3_wstream_destroy; the call synchronises `stream`.  Allowed while requests are in flight; a
+ * request on a registered schedule is unaffected by sr3_engine_set_schedule.  Refused, with nothing registered: a null table, T outside
+ * [1, the engine's maximum]. */
+int sr3_wstream_add_schedule(sr3_wstream* s, int T, const float* sqrt_recip_ac, const float* sqrt_recipm1_ac, const float* post_coef1,
+                             const float* post_coef2, const float* post_logvar, const double* sqrt_ac_prev, int* schedule, void* stream);
 /* Admit one request into the n_slots free slots `slots` (HOST, window k of the grid, row-major, into slots[k]).  condition_x: DEVICE fp32
  * [cond_c][height][width] (NULL for an unconditional model), x: DEVICE fp32 [3][height][width] holding x_T, overwritten with x_{t-1} by
  * every step and holding x_0 once the request has finished; both are BORROWED until sr3_wstream_retire, nothing is copied but the window geometry.  *request = the request's
- * id, its first step runs at t = T - 1.  Refused, with no slot or request changed: a slot out of range, busy or listed twice, n_slots other
- * than the canvas's window count, a canvas smaller than the window, a null x, a condition missing for a conditional model or given to an
- * unconditional one, an engine with no schedule, a schedule changed since the requests in flight were admitted. */
+ * id; it samples on the engine's schedule and its first step runs at t = T - 1.  Refused, with no slot or request changed: a slot out of
+ * range, busy or listed twice, n_slots other than the canvas's window count, a canvas smaller than the window, a null x, a condition
+ * missing for a conditional model or given to an unconditional one, an engine with no schedule, the engine's schedule changed since the
+ * requests in flight on it were admitted.  sr3_wstream_admit_scheduled with schedule -1. */
 int sr3_wstream_admit(sr3_wstream* s, const int* slots, int n_slots, const float* condition_x, float* x, int height, int width,
                       uint64_t sample_index, int* request, void* stream);
+/* sr3_wstream_admit of a request that samples on registered schedule `schedule` of T_S steps (-1: the engine's schedule): its first step
+ * runs at t = T_S - 1 and it finishes T_S steps later.  Also refused: an unknown schedule id. */
+int sr3_wstream_admit_scheduled(sr3_wstream* s, const int* slots, int n_slots, const float* condition_x, float* x, int height, int width,
+                                uint64_t sample_index, int schedule, int* request, void* stream);
 /* One reverse step of every running request.  Refused when the engine has no schedule or sr3_engine_set_schedule was called while
- * requests are in flight (they would finish on a mixed schedule). */
+ * requests on the engine's schedule are in flight (they would finish on a mixed schedule); requests on registered schedules do not count. */
 int sr3_wstream_step(sr3_wstream* s, void* stream);
 /* Free the slots of a finished request and end the borrow of its canvases (x holds x_0).  Refuses a running request or an id not held. */
 int sr3_wstream_retire(sr3_wstream* s, int request, void* stream);
