@@ -1,4 +1,5 @@
 """ctypes binding of libsr3_b200.so (include/sr3_b200.h).  torch is used only for device memory and streams."""
+import contextlib
 import ctypes
 import os
 from ctypes import POINTER, c_char_p, c_double, c_float, c_int, c_int64, c_uint64, c_void_p
@@ -96,6 +97,7 @@ _SIGS = {
     "sr3_windowed_read_state": (c_int, [c_void_p, c_void_p, c_void_p]),
     "sr3_windowed_grid": (c_int, [c_void_p, POINTER(c_int), POINTER(c_int), POINTER(c_int), POINTER(c_int), POINTER(c_float), POINTER(c_float)]),
     "sr3_windowed_profile_step": (c_int, [c_void_p, c_int, c_int, POINTER(c_float), c_void_p]),
+    "sr3_windowed_set_solver": (c_int, [c_void_p, c_int, c_void_p]),
     "sr3_windowed_create_range": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, POINTER(c_int), POINTER(c_void_p)]),
     "sr3_windowed_phase_begin": (c_int, [c_void_p, c_int, c_void_p]),
     "sr3_windowed_phase_means": (c_int, [c_void_p, c_void_p]),
@@ -315,6 +317,24 @@ class Engine:
         with torch.cuda.device(self.device):
             _check(lib().sr3_engine_set_schedule(self._h, T, *[c_void_p(h.data_ptr()) for h in host], c_void_p(sp.ctypes.data), _stream()))
         self.T = T
+        self._schedule = (bufs, sqrt_alphas_cumprod_prev)
+
+    @contextlib.contextmanager
+    def sampling_on(self, sampler):
+        """Runs the body on a few-step sampler's tables: `sampler` = (buffers, sqrt_alphas_cumprod_prev, solver) of
+        model.sr3_modules.samplers.sampler_schedule (None: the engine's schedule, unchanged).  The engine's schedule is set back when the
+        body ends, however it ends, so a later call without a sampler reads exactly the tables it read before."""
+        if sampler is None:
+            yield
+            return
+        saved = getattr(self, "_schedule", None)
+        if saved is None:
+            raise RuntimeError("set_new_noise_schedule has not been called")
+        self.set_schedule(sampler[0], sampler[1])
+        try:
+            yield
+        finally:
+            self.set_schedule(*saved)
 
     # ---- compute
     def _img(self):
@@ -508,7 +528,14 @@ class Engine:
             self._keep_masks[block_name] = mask_nchw_u8
         _check(lib().sr3_train_set_dropout_mask(self._h, block_name.encode(), _ptr(mask_nchw_u8)))
 
-    def p_sample_loop(self, condition_x, x_T, noises=None, seed=0, first_index=0, want_snapshots=True):
+    def p_sample_loop(self, condition_x, x_T, noises=None, seed=0, first_index=0, want_snapshots=True, sampler=None):
+        """The whole reverse loop; `sampler`: the tables of a DDIM spec (Engine.sampling_on), whose K steps then run instead of the
+        schedule's (noises [K, ...], K snapshots' worth of steps).  DPM-Solver++(2M) runs on a canvas (WindowedSampler.sample_loop)."""
+        if sampler is not None:
+            if sampler[2] is not None:
+                raise ValueError("DPM-Solver++(2M) keeps the previous step's x0 on a canvas: use WindowedSampler.sample_loop")
+            with self.sampling_on(sampler):
+                return self.p_sample_loop(condition_x, x_T, noises, seed, first_index, want_snapshots)
         c = None if condition_x is None else _f32c(condition_x, self.device)
         x_T = _f32c(x_T, self.device)
         n = None if noises is None else _f32c(noises, self.device)
@@ -719,8 +746,27 @@ class WindowedSampler:
             _check(lib().sr3_windowed_read_state(self._h, _ptr(out), _stream()))
         return out
 
-    def sample_loop(self, condition_x, x_T, noises=None, seed=0, first_index=0, want_snapshots=True):
-        """The whole reverse loop; returns (x_0, snapshots or None) like Engine.p_sample_loop."""
+    def set_solver(self, coefs):
+        """DPM-Solver++(2M) merges from the next step on: coefs [3, K] (A, B, C per step index; samplers.sampler_schedule), or None for
+        the posterior-sample merge (sr3_windowed_set_solver)."""
+        host = None if coefs is None else coefs.detach().to("cpu", torch.float32).contiguous()
+        if host is not None and (host.dim() != 2 or host.shape[0] != 3):
+            raise ValueError("solver coefficients must be [3, K], got %s" % (tuple(host.shape),))
+        with torch.cuda.device(self.device):
+            _check(lib().sr3_windowed_set_solver(self._h, 0 if host is None else host.shape[1], _ptr(host)))
+
+    def sample_loop(self, condition_x, x_T, noises=None, seed=0, first_index=0, want_snapshots=True, sampler=None):
+        """The whole reverse loop; returns (x_0, snapshots or None) like Engine.p_sample_loop.  `sampler`: the tables of a few-step
+        sampler (Engine.sampling_on), run instead of the engine's schedule; DPM-Solver++(2M) draws no noise and ignores `noises`."""
+        if sampler is not None:
+            with self.engine.sampling_on(sampler):
+                if sampler[2] is not None:
+                    self.set_solver(sampler[2])
+                try:
+                    return self.sample_loop(condition_x, x_T, noises, seed, first_index, want_snapshots)
+                finally:
+                    if sampler[2] is not None:
+                        self.set_solver(None)
         T = self.engine.T
         inter = 1 | (T // 10)
         cap = len([i for i in range(T) if i % inter == 0])

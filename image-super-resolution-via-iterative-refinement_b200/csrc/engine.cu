@@ -1934,12 +1934,16 @@ struct sr3_windowed {
     WindowCtl ctl{};
     uint64_t seed = 0, first_index = 0;
     float* snapshots = nullptr; int snapshot_cap = 0;
-    cudaGraphExec_t graph = nullptr, graph_means = nullptr, graph_merge = nullptr;
+    // DPM-Solver++(2M) (sr3_windowed_set_solver): solver_T > 0 steps run window_solver_merge_kernel with the [3][T_cap] A, B, C table
+    // solver_tab and the canvas-shaped x0 history x0_prev, both allocated at the first set_solver; 0: the posterior-sample merge
+    int solver_T = 0;
+    float *solver_tab = nullptr, *x0_prev = nullptr;
+    cudaGraphExec_t graph = nullptr, graph_means = nullptr, graph_merge = nullptr, graph_solver = nullptr;
     cudaStream_t cap_stream = nullptr;
     int phase_steps_left = 0; bool merge_due = false;  // host-side order of the phase calls
 
     ~sr3_windowed() {
-        for (cudaGraphExec_t g : {graph, graph_means, graph_merge})
+        for (cudaGraphExec_t g : {graph, graph_means, graph_merge, graph_solver})
             if (g) cudaGraphExecDestroy(g);
         if (cap_stream) cudaStreamDestroy(cap_stream);
     }
@@ -2013,7 +2017,14 @@ struct sr3_windowed {
         m.g = g; m.means = means; m.x = x; m.noise = noise; m.tab = e->post_tab; m.tab_T = e->T_cap; m.ctl = ctl_dev;
         m.band = band; m.band_rows = band_rows;
         const long long total = 1LL * B * (band ? band_rows : H) * W;
-        launch_k(window_merge_kernel, dim3((int)std::min<long long>((total + 255) / 256, num_sms() * 8LL)), dim3(256), 0, st, m);
+        const dim3 grid((int)std::min<long long>((total + 255) / 256, num_sms() * 8LL));
+        if (solver_T > 0) {                // a solver canvas is never ranged: no band
+            WindowSolverMerge sm{};
+            sm.m = m; sm.x0_prev = x0_prev; sm.coef = solver_tab; sm.stride = e->T_cap;
+            launch_k(window_solver_merge_kernel, grid, dim3(256), 0, st, sm);
+            return;
+        }
+        launch_k(window_merge_kernel, grid, dim3(256), 0, st, m);
     }
     // Phase (a) of a step: the timestep advance and the passes over this canvas's windows, their means stored into the arena.
     void record_means(cudaStream_t st) {
@@ -2039,7 +2050,24 @@ struct sr3_windowed {
         }
         CK(cudaGraphLaunch(exec, st));
     }
-    void run_step(cudaStream_t st) { launch_graph(graph, [this](cudaStream_t s) { record_step(s); }, st); }
+    void run_step(cudaStream_t st) { launch_graph(solver_T > 0 ? graph_solver : graph, [this](cudaStream_t s) { record_step(s); }, st); }
+    // Host table [3][T] (A, B, C of every step index) -> solver_tab; T == 0 returns to the posterior-sample merge.
+    void set_solver(int T, const float* coefs) {
+        REQUIRE(!ranged, "a canvas that runs a window range has no solver merge");
+        REQUIRE(T >= 0 && T <= e->T_cap, "solver steps %d out of range [0, %d]", T, e->T_cap);
+        REQUIRE(T == 0 || coefs != nullptr, "null solver table");
+        CK(cudaSetDevice(e->dev));
+        if (T > 0) {
+            if (!solver_tab) {
+                solver_tab = static_cast<float*>(mem.alloc((size_t)3 * e->T_cap * sizeof(float)));
+                x0_prev = static_cast<float*>(mem.alloc(canvas_elems() * sizeof(float)));      // zeroed
+            }
+            std::vector<float> tab((size_t)3 * e->T_cap, 0.f);
+            for (int r = 0; r < 3; ++r) memcpy(tab.data() + (size_t)r * e->T_cap, coefs + (size_t)r * T, T * sizeof(float));
+            CK(cudaMemcpy(solver_tab, tab.data(), tab.size() * sizeof(float), cudaMemcpyHostToDevice));
+        }
+        solver_T = T;
+    }
     // The two phases of a step as separate graphs, so that means of windows other canvases ran can be written into the arena between them.
     void run_means(cudaStream_t st) { launch_graph(graph_means, [this](cudaStream_t s) { record_means(s); }, st); }
     void run_merge(cudaStream_t st) { launch_graph(graph_merge, [this](cudaStream_t s) { merge(s); }, st); }
@@ -2661,6 +2689,7 @@ int sr3_windowed_begin(sr3_windowed* w, const float* cond, const float* x_T, uin
     CK(cudaSetDevice(w->e->dev));
     if (cond) CK(cudaMemcpyAsync(w->cond, cond, (size_t)w->B * w->e->cond_c * w->H * w->W * sizeof(float), cudaMemcpyDeviceToDevice, st));
     CK(cudaMemcpyAsync(w->x, x_T, w->canvas_elems() * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    if (w->x0_prev) CK(cudaMemsetAsync(w->x0_prev, 0, w->canvas_elems() * sizeof(float), st));     // the solver's first step has C = 0
     w->seed = seed; w->first_index = first_index;
     API_END
 }
@@ -2676,6 +2705,7 @@ int sr3_windowed_steps(sr3_windowed* w, int t_start, int steps, const float* noi
     REQUIRE(!w->ranged, "a canvas that runs a window range steps through sr3_windowed_phase_means / _merge");
     sr3_engine* e = w->e;
     REQUIRE(t_start < e->T && steps >= 0 && t_start - steps + 1 >= 0, "bad step range t_start=%d steps=%d T=%d", t_start, steps, e->T);
+    REQUIRE(w->solver_T == 0 || w->solver_T == e->T, "the solver table has %d steps but the engine's schedule %d", w->solver_T, e->T);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     CK(cudaSetDevice(e->dev));
     e->check_params();
@@ -2685,6 +2715,12 @@ int sr3_windowed_steps(sr3_windowed* w, int t_start, int steps, const float* noi
         if (noises) CK(cudaMemcpyAsync(w->noise, noises + (size_t)(t_start - i) * n, n * sizeof(float), cudaMemcpyDeviceToDevice, st));
         w->run_step(st);
     }
+    API_END
+}
+int sr3_windowed_set_solver(sr3_windowed* w, int steps, const float* coefs) {
+    API_BEGIN
+    REQUIRE(w, "null argument");
+    w->set_solver(steps, coefs);
     API_END
 }
 int sr3_windowed_create_range(sr3_engine* e, int batch, int height, int width, int overlap_h, int overlap_w, int first_window, int end_window,

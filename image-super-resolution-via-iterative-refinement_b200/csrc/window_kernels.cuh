@@ -3,6 +3,8 @@
 // their posterior means only.  Two kernels stand around the engine's step graph:
 //   window_gather_kernel  crops of the canvas x_t and of the condition -> the engine's bf16 NHWC input buffer and fp32 x_state
 //   window_merge_kernel   weighted average of the window means per canvas pixel, + sigma_t * z -> the canvas x_{t-1} (and a snapshot)
+//   window_solver_merge_kernel   the DPM-Solver++(2M) form of the merge: the windows' means are their clipped x0 (the engine runs with
+//                         pc1 = 1, pc2 = 0), blended alike, then x_{k-1} = A x_k + B x0 + C x0_prev; x0 is kept for the next step
 #pragma once
 #include "aux_kernels.cuh"
 
@@ -103,6 +105,38 @@ struct WindowMerge {
     int band_rows;           // max over images of y1 - y0 (the launch covers B x band_rows x W pixels)
 };
 
+// The weighted sum of the means of the windows covering canvas pixel `pix` of image b (num[c], c < C) and the sum of their weights (den):
+// windows in ascending index, separately rounded multiplies and adds, so the sum does not depend on the launch shape or on how many
+// windows a pass ran.
+__device__ __forceinline__ void blend_window_means(const WindowGeom& g, const float* means, int b, long long pix, float (&num)[4], float& den) {
+    const int wplane = g.wh * g.ww;
+    const int y = static_cast<int>(pix / g.W), x = static_cast<int>(pix - static_cast<long long>(y) * g.W);
+    num[0] = num[1] = num[2] = num[3] = 0.f; den = 0.f;
+    for (int iy = 0; iy < g.ny; ++iy) {
+        const int dy = y - g.oy[iy];
+        if (dy < 0 || dy >= g.wh) continue;
+        const float wyv = g.wy[iy * g.wh + dy];
+        for (int ix = 0; ix < g.nx; ++ix) {
+            const int dx = x - g.ox[ix];
+            if (dx < 0 || dx >= g.ww) continue;
+            const float w = __fmul_rn(wyv, g.wx[ix * g.ww + dx]);
+            const float* m = means + (static_cast<long long>(b) * g.ny + iy) * g.nx * g.C * wplane + static_cast<long long>(ix) * g.C * wplane + dy * g.ww + dx;
+#pragma unroll
+            for (int c = 0; c < 4; ++c)
+                if (c < g.C) num[c] = __fadd_rn(num[c], __fmul_rn(w, m[c * wplane]));
+            den = __fadd_rn(den, w);
+        }
+    }
+}
+
+// Snapshot slot of the step at t: p_sample_loop keeps x_{t-1} whenever t % (1 | T / 10) == 0 (diffusion.py:179-199), first kept image
+// first; nullptr when the step keeps none.
+__device__ __forceinline__ float* window_snapshot(const WindowCtl* ctl, int t, long long canvas_elems) {
+    const int inter = 1 | (ctl->T / 10);
+    const int slot = (ctl->T - 1) / inter - t / inter;
+    return (ctl->snapshots != nullptr && t % inter == 0 && slot < ctl->snapshot_cap) ? ctl->snapshots + slot * canvas_elems : nullptr;
+}
+
 // One thread per canvas pixel, all (<= 4) channels: the Philox draw of a pixel yields the z of its channels.  The covering windows are found
 // from the two per-axis origin tables and accumulated in ascending window index with separately rounded multiplies and adds, so the sum is
 // the same whatever the launch shape and however many windows a pass ran: no atomics, repeat runs are bit identical.  With a band table
@@ -115,13 +149,7 @@ __global__ void __launch_bounds__(256) window_merge_kernel(const WindowMerge p) 
     const int t = ctl.t_cur;
     const float sigma = posterior_sigma(p.tab, p.tab_T, t);
     const long long plane = static_cast<long long>(g.H) * g.W;
-    const int wplane = g.wh * g.ww;
-    float* snap = nullptr;
-    {   // p_sample_loop keeps x_{t-1} whenever t % (1 | T / 10) == 0 (diffusion.py:179-199), first kept image first
-        const int inter = 1 | (p.ctl->T / 10);
-        const int slot = (p.ctl->T - 1) / inter - t / inter;
-        if (p.ctl->snapshots != nullptr && t % inter == 0 && slot < p.ctl->snapshot_cap) snap = p.ctl->snapshots + slot * (plane * g.C * g.B);
-    }
+    float* snap = window_snapshot(p.ctl, t, plane * g.C * g.B);
     const long long bplane = p.band ? static_cast<long long>(p.band_rows) * g.W : plane;
     const long long total = bplane * g.B;
     for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total; i += static_cast<long long>(gridDim.x) * blockDim.x) {
@@ -131,23 +159,8 @@ __global__ void __launch_bounds__(256) window_merge_kernel(const WindowMerge p) 
             pix += static_cast<long long>(p.band[2 * b]) * g.W;
             if (pix >= static_cast<long long>(p.band[2 * b + 1]) * g.W) continue;
         }
-        const int y = static_cast<int>(pix / g.W), x = static_cast<int>(pix - static_cast<long long>(y) * g.W);
-        float num[4] = {0.f, 0.f, 0.f, 0.f}, den = 0.f;
-        for (int iy = 0; iy < g.ny; ++iy) {
-            const int dy = y - g.oy[iy];
-            if (dy < 0 || dy >= g.wh) continue;
-            const float wyv = g.wy[iy * g.wh + dy];
-            for (int ix = 0; ix < g.nx; ++ix) {
-                const int dx = x - g.ox[ix];
-                if (dx < 0 || dx >= g.ww) continue;
-                const float w = __fmul_rn(wyv, g.wx[ix * g.ww + dx]);
-                const float* m = p.means + (static_cast<long long>(b) * g.ny + iy) * g.nx * g.C * wplane + static_cast<long long>(ix) * g.C * wplane + dy * g.ww + dx;
-#pragma unroll
-                for (int c = 0; c < 4; ++c)
-                    if (c < g.C) num[c] = __fadd_rn(num[c], __fmul_rn(w, m[c * wplane]));
-                den = __fadd_rn(den, w);
-            }
-        }
+        float num[4], den;
+        blend_window_means(g, p.means, b, pix, num, den);
         float z[4] = {0.f, 0.f, 0.f, 0.f};
         if (t > 0) {
             if (ctl.use_noise_buf) {
@@ -164,6 +177,44 @@ __global__ void __launch_bounds__(256) window_merge_kernel(const WindowMerge p) 
                 const long long idx = (static_cast<long long>(b) * g.C + c) * plane + pix;
                 const float xn = posterior_sample(__fdiv_rn(num[c], den), z[c], sigma);
                 p.x[idx] = xn;
+                if (snap) snap[idx] = xn;
+            }
+        }
+    }
+}
+
+struct WindowSolverMerge {
+    WindowMerge m;           // geometry, means arena (the windows' clipped x0), canvas x_k, control block, band; noise and tab unused
+    float* x0_prev;          // canvas-shaped x0 of the previous step, overwritten with this step's (zero before the first step)
+    const float* coef;       // [3][stride]: A, B, C of step index k = t
+    int stride;
+};
+
+// DPM-Solver++(2M) (data prediction, multistep) on the canvas: x0 is the blend of the windows' clipped x0 (window_merge_kernel's blend and
+// division), then x_{k-1} = (A x_k + B x0) + C x0_prev in that order with separately rounded operations, and x0_prev = x0.  No noise.  The
+// update is linear and the blend weights sum to 1, so blending x0 and then stepping is stepping every window and blending the results.
+__global__ void __launch_bounds__(256) window_solver_merge_kernel(const WindowSolverMerge p) {
+    pdl_launch_dependents();
+    pdl_wait();
+    const WindowGeom& g = p.m.g;
+    const int t = p.m.ctl->step.t_cur;
+    const float A = p.coef[t], B = p.coef[p.stride + t], Cc = p.coef[2 * p.stride + t];
+    const long long plane = static_cast<long long>(g.H) * g.W;
+    float* snap = window_snapshot(p.m.ctl, t, plane * g.C * g.B);
+    const long long total = plane * g.B;
+    for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total; i += static_cast<long long>(gridDim.x) * blockDim.x) {
+        const int b = static_cast<int>(i / plane);
+        const long long pix = i - b * plane;
+        float num[4], den;
+        blend_window_means(g, p.m.means, b, pix, num, den);
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+            if (c < g.C) {
+                const long long idx = (static_cast<long long>(b) * g.C + c) * plane + pix;
+                const float x0 = __fdiv_rn(num[c], den);
+                const float xn = __fadd_rn(__fadd_rn(__fmul_rn(A, p.m.x[idx]), __fmul_rn(B, x0)), __fmul_rn(Cc, p.x0_prev[idx]));
+                p.x0_prev[idx] = x0;
+                p.m.x[idx] = xn;
                 if (snap) snap[idx] = xn;
             }
         }

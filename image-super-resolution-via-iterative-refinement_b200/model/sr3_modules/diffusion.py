@@ -7,6 +7,8 @@ import numpy as np
 import torch
 from torch import nn
 
+from . import samplers
+
 
 def _warmup_beta(linear_start, linear_end, n_timestep, warmup_frac):
     betas = linear_end * np.ones(n_timestep, dtype=np.float64)
@@ -125,6 +127,9 @@ class GaussianDiffusion(nn.Module):
 
     def set_new_noise_schedule(self, schedule_opt, device):
         bufs, self.sqrt_alphas_cumprod_prev = noise_schedule_buffers(schedule_opt, device)
+        # the fp64 schedule the few-step samplers respace (samplers.sampler_schedule)
+        self._trained_schedule = (schedule_opt["schedule"], int(schedule_opt["n_timestep"]), float(schedule_opt["linear_start"]),
+                                  float(schedule_opt["linear_end"]))
         self.num_timesteps = int(bufs["betas"].shape[0])
         for k in _BUFFERS:
             self.register_buffer(k, bufs[k])
@@ -137,6 +142,19 @@ class GaussianDiffusion(nn.Module):
     def q_posterior(self, x_start, x_t, t):
         mean = self.posterior_mean_coef1[t] * x_start + self.posterior_mean_coef2[t] * x_t
         return mean, self.posterior_log_variance_clipped[t]
+
+    def _sampler_spec(self, sampler):
+        """The canonical spec of a few-step sampler (samplers.check_sampler_spec) on the trained schedule, or None."""
+        if sampler is None:
+            return None
+        if getattr(self, "_trained_schedule", None) is None:
+            raise RuntimeError("set_new_noise_schedule has not been called")
+        return samplers.check_sampler_spec(sampler, self._trained_schedule[1])
+
+    def _sampler_tables(self, spec, trained=None):
+        """samplers.sampler_schedule of a canonical spec on `trained` (a canonical beta schedule tuple, default the module's)."""
+        name, T, ls, le = self._trained_schedule if trained is None else trained
+        return samplers.sampler_schedule(spec, make_beta_schedule(name, T, linear_start=ls, linear_end=le))
 
     def _engine(self, batch, height=None, width=None):
         """The inference engine for `batch` images of height x width (default image_size x image_size)."""
@@ -158,8 +176,15 @@ class GaussianDiffusion(nn.Module):
         return self._engine_for(x).p_sample(x, t, condition_x, noise, seed)
 
     @torch.no_grad()
-    def p_sample_loop(self, x_in, continous=False, x_T=None, noises=None, seed=None, first_index=0):
-        """diffusion.py:176-200.  Extra keyword arguments inject the random draws (tests, multi-GPU sharding)."""
+    def p_sample_loop(self, x_in, continous=False, x_T=None, noises=None, seed=None, first_index=0, sampler=None):
+        """diffusion.py:176-200.  Extra keyword arguments inject the random draws (tests, multi-GPU sharding).  `sampler`: a few-step
+        sampler spec (samplers.check_sampler_spec, DESIGN.md 3.11) that respaces the trained schedule to its K steps (noises [K, ...],
+        snapshots every 1 | K // 10 steps); DPM-Solver++(2M) runs as super_resolution_windowed with the window equal to the image."""
+        spec = self._sampler_spec(sampler)
+        if spec is not None and spec[0] == "dpmpp_2m":
+            shape = tuple(x_in) if not self.conditional else tuple(x_in.shape)
+            return self.super_resolution_windowed(x_in, window=shape[2:], overlap=0, continous=continous, x_T=x_T, noises=noises, seed=seed,
+                                                  first_index=first_index, sampler=sampler)
         device = self.betas.device
         if not self.conditional:
             shape = tuple(x_in)
@@ -170,15 +195,16 @@ class GaussianDiffusion(nn.Module):
         img = torch.randn(shape, device=device) if x_T is None else x_T.to(device)
         if seed is None:
             seed = int(torch.randint(0, 2 ** 62, (1,)).item())
-        final, snaps = self._engine(shape[0], shape[2], shape[3]).p_sample_loop(cond, img, noises, seed, first_index, want_snapshots=continous)
+        final, snaps = self._engine(shape[0], shape[2], shape[3]).p_sample_loop(
+            cond, img, noises, seed, first_index, want_snapshots=continous, sampler=None if spec is None else self._sampler_tables(spec))
         if continous:
             first = cond if self.conditional else img
             return torch.cat([first, snaps.reshape(-1, *shape[1:])], dim=0)
         return final[-1]      # the reference returns ret_img[-1]: the last image of the batch only
 
     @torch.no_grad()
-    def sample(self, batch_size=1, continous=False):
-        return self.p_sample_loop((batch_size, self.channels, self.image_size, self.image_size), continous)
+    def sample(self, batch_size=1, continous=False, sampler=None):
+        return self.p_sample_loop((batch_size, self.channels, self.image_size, self.image_size), continous, sampler=sampler)
 
     @torch.no_grad()
     def super_resolution(self, x_in, continous=False, **kw):
@@ -236,24 +262,28 @@ class GaussianDiffusion(nn.Module):
         return _native.WindowedSampler(eng, batch, height, width, ovh, ovw, window_range=(shard.n0, shard.n1), bands=shard.bands)
 
     @torch.no_grad()
-    def super_resolution_windowed(self, x_in, window=None, overlap=None, continous=False, x_T=None, noises=None, seed=None, first_index=0):
+    def super_resolution_windowed(self, x_in, window=None, overlap=None, continous=False, x_T=None, noises=None, seed=None, first_index=0,
+                                  sampler=None):
         """super_resolution for a conditioning image x_in [B, C, H, W] of ANY size H >= window height, W >= window width: the UNet runs on
         overlapping `window` = (wh, ww) crops (default image_size x image_size; any size _native.check_image_size accepts) whose posterior
         means are blended on the canvas inside every reverse step, so there is one x_t and one noise draw per canvas pixel and no seam.
         `overlap`: least overlap of neighbouring windows in pixels, an int or (rows, columns), default a quarter of the window side.
         With window == (H, W) this is super_resolution bit for bit.  Return conventions and the extra keyword arguments are
-        p_sample_loop's."""
+        p_sample_loop's.  `sampler`: a few-step sampler spec (DESIGN.md 3.11); DPM-Solver++(2M) blends the windows' x0 and steps the
+        canvas with it, and draws no noise."""
+        spec = self._sampler_spec(sampler)
         device = self.betas.device
         if not self.conditional:
             shape, cond = tuple(x_in), None
         else:
             cond = x_in.to(device)
             shape = tuple(cond.shape)
-        sampler = self._windowed_sampler(shape[0], shape[2], shape[3], window, overlap)
+        canvas = self._windowed_sampler(shape[0], shape[2], shape[3], window, overlap)
         img = torch.randn(shape, device=device) if x_T is None else x_T.to(device)
         if seed is None:
             seed = int(torch.randint(0, 2 ** 62, (1,)).item())
-        final, snaps = sampler.sample_loop(cond, img, noises, seed, first_index, want_snapshots=continous)
+        final, snaps = canvas.sample_loop(cond, img, noises, seed, first_index, want_snapshots=continous,
+                                          sampler=None if spec is None else self._sampler_tables(spec))
         if continous:
             first = cond if self.conditional else img
             return torch.cat([first, snaps.reshape(-1, *shape[1:])], dim=0)
@@ -288,7 +318,9 @@ class GaussianDiffusion(nn.Module):
         served once its windows' slots are free (_native.windowed_stream_plan) and its (key, image [C, H, W]) is yielded as soon as its T
         steps are done.  A request that names `schedule` (a beta_schedule dict: schedule, n_timestep, linear_start, linear_end) samples
         on it: it is admitted at t = n_timestep - 1 and finishes n_timestep steps later, next to requests on other schedules; one that
-        names none samples on the module's (set_new_noise_schedule).  The n-th request's draws are keyed by sample index first_index + n
+        names none samples on the module's (set_new_noise_schedule).  `schedule` may instead be a DDIM sampler spec ({"sampler": "ddim",
+        "steps": K, "eta": eta}, told apart by its "sampler" key, DESIGN.md 3.11): the request then runs K respaced steps of the module's
+        schedule and equals super_resolution_windowed(..., sampler=spec) of it alone; a dpmpp_2m spec is refused.  The n-th request's draws are keyed by sample index first_index + n
         (x_T ~ randn when not given): its image is super_resolution_windowed(x_in[None], window, overlap, x_T=x_T[None], seed=seed,
         first_index=first_index + n), computed after set_new_noise_schedule(schedule) on the same engine with its windows in the same
         slots, bit for bit (DESIGN.md 3.10: on some plans the slot a window runs in changes it within rounding).  A request is checked
@@ -312,7 +344,10 @@ class GaussianDiffusion(nn.Module):
         if not isinstance(req, (tuple, list)) or len(req) not in (2, 3, 4):
             raise ValueError("a request is (key, x_in), (key, x_in, x_T) or (key, x_in, x_T or None, schedule), got %r" % (type(req),))
         key, x_in, x_T, sched = (tuple(req) + (None, None))[:4]
-        if len(req) == 4:
+        if len(req) == 4 and isinstance(sched, dict) and "sampler" in sched:
+            spec = self._sampler_spec_of_request(sched, key)
+            sched = spec + (self._trained_schedule,)
+        elif len(req) == 4:
             sched = check_schedule_opt(sched, "request %r" % (key,))
         if self.conditional:
             cond_c = self.denoise_fn.arch["in_channel"] - self.channels
@@ -336,6 +371,16 @@ class GaussianDiffusion(nn.Module):
         if x_T is not None and tuple(x_T.shape) != (self.channels,) + hw:
             raise ValueError("request %r: x_T must be %s, got %s" % (key, (self.channels,) + hw, tuple(x_T.shape)))
         return geometry, (key, x_in, x_T, hw, n, sched)
+
+    def _sampler_spec_of_request(self, spec, key):
+        """The canonical spec of a stream request's sampler, or ValueError naming the request: streams run DDIM only."""
+        if getattr(self, "_trained_schedule", None) is None:
+            raise RuntimeError("set_new_noise_schedule has not been called")
+        spec = samplers.check_sampler_spec(spec, self._trained_schedule[1], "request %r" % (key,))
+        if spec[0] != "ddim":
+            raise ValueError("request %r: sampler %r cannot run in a stream (it needs a per-request x0 history); use ddim, or "
+                             "super_resolution_windowed for dpmpp_2m" % (key, spec[0]))
+        return spec
 
     @torch.no_grad()
     def _stream(self, requests, geometry, slots, seed, first_index):
@@ -383,7 +428,10 @@ class GaussianDiffusion(nn.Module):
             for read_at, key, cond, x_T, size, windows, sched in batch:
                 sid, steps = None, T
                 if sched is not None:
-                    if sched not in schedules:
+                    if sched not in schedules and sched[0] in samplers.SAMPLER_NAMES:     # (name, K, eta, trained schedule)
+                        bufs, sp, _ = self._sampler_tables(sched[:3], sched[3])
+                        schedules[sched] = (sampler.add_schedule(bufs, sp), sched[1])
+                    elif sched not in schedules:
                         bufs, sp = noise_schedule_buffers(dict(zip(SCHEDULE_KEYS, sched)))
                         schedules[sched] = (sampler.add_schedule(bufs, sp), sched[1])
                     sid, steps = schedules[sched]

@@ -217,6 +217,13 @@ int sr3_windowed_grid(const sr3_windowed* w, int* ny, int* nx, int* origins_y, i
 /* Profiling: eager canvas steps at timestep t (Philox noise), CUDA events around the launches; ms[3] = device time per step of the gathers,
  * of the engine passes and of the merge, averaged over `reps` steps after one warm-up.  Advances the canvas state. */
 int sr3_windowed_profile_step(sr3_windowed* w, int t, int reps, float* ms, void* stream);
+/* DPM-Solver++(2M) on the canvas (added in ABI 5).  coefs: HOST [3][steps] (copied), rows A, B, C per step index k; steps = 0 (coefs may
+ * be NULL) returns to the posterior-sample merge.  While set, the merge of the step at k blends the window means like the posterior-sample
+ * merge, takes the blend as x0 (the engine's schedule must then have pc1 = 1, pc2 = 0 and `steps` entries) and writes
+ *   x_{k-1} = (A_k x_k + B_k x0) + C_k x0_prev,   x0_prev = x0,
+ * separately rounded in that order, with no noise; sr3_windowed_begin zeroes x0_prev.  sr3_windowed_steps refuses to run when `steps` is not
+ * the engine's schedule length.  Refused for a ranged canvas. */
+int sr3_windowed_set_solver(sr3_windowed* w, int steps, const float* coefs);
 
 /* ---- windowed sampling sharded by window (one canvas on several GPUs).  A ranged canvas runs only windows [first_window, end_window) of
  * the list and stores their means into `means`, a DEVICE arena [N][3][window height][window width] of all N windows owned by the caller;
