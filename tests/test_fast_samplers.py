@@ -195,7 +195,14 @@ def test_gaussian_data_convergence_orders():
 
 
 @pytest.mark.parametrize("spec", [{"sampler": "ddim", "steps": 12, "eta": 0.0}, {"sampler": "ddim", "steps": 5, "eta": 0.6},
-                                  {"sampler": "dpmpp_2m", "steps": 9}, {"sampler": "dpmpp_2m", "steps": 2}])
+                                  {"sampler": "dpmpp_2m", "steps": 9}, {"sampler": "dpmpp_2m", "steps": 2},
+                                  # the specs the device step tests run (tests/test_gpu_fast_sampler_steps.py)
+                                  {"sampler": "ddim", "steps": 1, "eta": 0.0}, {"sampler": "ddim", "steps": 1, "eta": 1.0},
+                                  {"sampler": "ddim", "steps": 2, "eta": 0.5}, {"sampler": "ddim", "steps": 10, "eta": 1.0},
+                                  {"sampler": "ddim", "steps": 11, "eta": 0.5}, {"sampler": "ddim", "steps": 20, "eta": 0.5},
+                                  {"sampler": "ddim", "steps": 50, "eta": 0.0}, {"sampler": "ddim", "steps": 50, "eta": 0.5},
+                                  {"sampler": "ddim", "steps": 50, "eta": 1.0}, {"sampler": "dpmpp_2m", "steps": 3},
+                                  {"sampler": "dpmpp_2m", "steps": 10}, {"sampler": "dpmpp_2m", "steps": 20}])
 def test_oracle_agrees_with_the_tables(spec):
     """oracle/fast_sampler_oracle.py (definitions, abar only) and the package's tables drive the same loop to the same states."""
     K = spec["steps"]

@@ -4,7 +4,8 @@ the canvas's solver merge (window_solver_merge_kernel, sr3_windowed_set_solver).
 What is pinned: the engine against the fp64 oracle (oracle/fast_sampler_oracle.py) with injected x_T and noises, at the suite's tolerances;
 DDIM with K = T and eta = 1 is the default sampler to table rounding; one window is super_resolution bit for bit and a multi-window canvas
 matches the oracle's canvas-level solver; eta = 0 and DPM-Solver++ draw nothing, and runs repeat bit for bit; a default call after a spec'd
-one is unchanged bit for bit; DDIM requests share a stream with DDPM and beta_schedule requests and each equals its request alone."""
+one is unchanged bit for bit; DDIM requests share a stream with DDPM and beta_schedule requests and each equals its request alone, on the
+12-step schedule and on the trained 2000-step one (K = 1 .. 50 next to a 2000-step request)."""
 import functools
 
 import pytest
@@ -180,14 +181,26 @@ def test_unconditional_sample_takes_both_samplers(monkeypatch):
         assert torch.isfinite(out).all()
 
 
+# (module schedule, request sizes, per-request schedules or sampler specs; None = the module's schedule)
+STREAM_CASES = {
+    "sched12": (SCHED12, [(40, 56), (32, 32), (32, 72), (32, 32), (56, 48), (40, 40)],
+                [{"sampler": "ddim", "steps": 5, "eta": 0.0}, None, LIN5, {"sampler": "ddim", "steps": 7, "eta": 1.0},
+                 {"sampler": "ddim", "steps": 3, "eta": 0.5}, {"sampler": "ddim", "steps": 5, "eta": 0.0}]),
+    # the trained 2000-step schedule: K = 1 is admitted at t = 0 and finishes after one step, next to a 2000-step request
+    "sr3_2000": (si.SCHED, [(32, 32), (40, 56), (32, 32), (32, 72), (40, 40)],
+                 [{"sampler": "ddim", "steps": 1, "eta": 0.0}, None, {"sampler": "ddim", "steps": 2, "eta": 1.0},
+                  {"sampler": "ddim", "steps": 10, "eta": 0.5}, {"sampler": "ddim", "steps": 50, "eta": 0.0}]),
+}
+
+
 @pytest.mark.timeout(1800)
-@pytest.mark.parametrize("precision", ["bf16", "fp32"])
-def test_stream_ddim_requests_equal_each_request_alone(monkeypatch, precision):
-    net = build(monkeypatch, "tiny", precision)
+@pytest.mark.parametrize("precision,case", [pytest.param("bf16", "sched12", id="bf16"), pytest.param("fp32", "sched12", id="fp32"),
+                                            pytest.param("bf16", "sr3_2000", id="bf16-sr3_2000"),
+                                            pytest.param("fp32", "sr3_2000", id="fp32-sr3_2000")])
+def test_stream_ddim_requests_equal_each_request_alone(monkeypatch, precision, case):
+    sched, sizes, scheds = STREAM_CASES[case]
+    net = build(monkeypatch, "tiny", precision, sched=sched)
     monkeypatch.setattr(net, "WINDOW_PASS_SIZES", (8,))      # the references run on the stream's engine
-    sizes = [(40, 56), (32, 32), (32, 72), (32, 32), (56, 48), (40, 40)]
-    scheds = [{"sampler": "ddim", "steps": 5, "eta": 0.0}, None, LIN5, {"sampler": "ddim", "steps": 7, "eta": 1.0},
-              {"sampler": "ddim", "steps": 3, "eta": 0.5}, {"sampler": "ddim", "steps": 5, "eta": 0.0}]
     g = torch.Generator().manual_seed(21)
     reqs = [((torch.rand(3, H, W, generator=g) * 2 - 1).cuda(), torch.randn(3, H, W, generator=g).cuda()) for H, W in sizes]
     seed, first = 77, 3
@@ -200,7 +213,7 @@ def test_stream_ddim_requests_equal_each_request_alone(monkeypatch, precision):
             try:
                 ref = net.super_resolution_windowed(c[None], x_T=x[None], seed=seed, first_index=first + n)
             finally:
-                net.set_new_noise_schedule(SCHED12, "cuda")
+                net.set_new_noise_schedule(sched, "cuda")
         else:
             ref = net.super_resolution_windowed(c[None], x_T=x[None], seed=seed, first_index=first + n, sampler=s)
         assert torch.isfinite(ref).all() and torch.equal(out[n], ref), (n, s)
